@@ -26,6 +26,9 @@ SIGNATURES: dict[str, list] = {
     "es3_attention_bf16": [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
     "es3_attention_tc_bf16": [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
     "es3_attention_mma_bf16": [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
+    "es3_attention_causal_bf16": [_vp, _vp, _i, _i, _i, _i, _f, _vp],
+    "es3_text_embed": [_vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
+    "es3_repmixer_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp],
     "es3_tokens_f32_to_nchw": [_vp, _vp, _i, _i, _i, _vp],
     "es3_cast_f32_to_f16": [_vp, _vp, _ll, _vp],
     "es3_convt2x2_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp],

@@ -61,10 +61,12 @@ __device__ __forceinline__ long long token_row(const AttnArgs& a, int b, int wi,
   return (long long)b * a.H * a.W + (long long)(wy * a.win + i) * a.W + wx * a.win + j;
 }
 
+// CAUSAL: token l attends to tokens <= l only (the additive triu(-inf) mask of the text encoders, mobile_clip.py:825-831,
+// text_encoder_ve.py:220-226); KV tiles wholly above the diagonal of this CTA's query rows are not loaded.
 // MT = 16-row query tiles per warp.  K/V fragments loaded by ldmatrix are reused for all MT tiles: on this part
 // one m16n8k16 MMA (1 tensor-pipe cycle per SM at 2048 FMA/clk) consumes a 256-byte B fragment, i.e. 2 cycles of the
 // 128 B/clk shared-memory pipe -- with MT = 1 the kernel is smem-bandwidth-bound.
-template <int MT>
+template <int MT, bool CAUSAL = false>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   constexpr int AT_BM = 64 * MT;
   extern __shared__ __align__(16) uint8_t at_smem[];
@@ -120,7 +122,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
     l_run[mt][0] = l_run[mt][1] = 0.f;
   }
 
-  const int ntiles = (a.L + AT_BN - 1) / AT_BN;
+  int ntiles = (a.L + AT_BN - 1) / AT_BN;
+  if (CAUSAL) ntiles = min(ntiles, (qt * AT_BM + AT_BM - 1) / AT_BN + 1);
   for (int t = 0; t < ntiles; ++t) {
     const int buf = t & 1;
     if (t + 1 < ntiles) {
@@ -172,6 +175,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
           const int col = col0 + nt * 8 + t4 * 2 + (e & 1);
           float v = s[mt][nt][e] * a.scale_log2;
           if (col >= a.L) v = -INFINITY;
+          if (CAUSAL && col > qt * AT_BM + (warp * MT + mt) * 16 + g + ((e >> 1) << 3)) v = -INFINITY;
           s[mt][nt][e] = v;
           mx[e >> 1] = fmaxf(mx[e >> 1], v);
         }
@@ -269,8 +273,9 @@ extern "C" int es3_attention_bf16(const void* qkv, void* out, int B, int H, int 
   return es3_attention_mma_bf16(qkv, out, B, H, W, C, num_heads, win, scale, stream);
 }
 
-extern "C" int es3_attention_mma_bf16(const void* qkv, void* out, int B, int H, int W, int C, int num_heads, int win,
-                                      float scale, void* stream) {
+template <bool CAUSAL>
+static int attention_mma(const void* qkv, void* out, int B, int H, int W, int C, int num_heads, int win, float scale,
+                         void* stream) {
   ES3_REQUIRE(C == num_heads * AT_D, "es3_attention_bf16: head_dim must be 64 (C=%d heads=%d)", C, num_heads);
   ES3_REQUIRE(win == 0 || (H % win == 0 && W % win == 0), "es3_attention_bf16: H,W must be multiples of the window (%d,%d,%d)", H, W, win);
   AttnArgs a;
@@ -285,13 +290,26 @@ extern "C" int es3_attention_mma_bf16(const void* qkv, void* out, int B, int H, 
   const size_t smem = (size_t)(bm + 4 * AT_BN) * AT_RS;
   static bool configured = false;
   if (!configured) {
-    ES3_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    ES3_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    ES3_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<1, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    ES3_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<2, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     configured = true;
   }
   dim3 grid(ceil_div(a.L, bm), num_heads, B * a.nwin);
-  if (mt2) attn_fwd_kernel<2><<<grid, 128, smem, (cudaStream_t)stream>>>(a);
-  else attn_fwd_kernel<1><<<grid, 128, smem, (cudaStream_t)stream>>>(a);
+  if (mt2) attn_fwd_kernel<2, CAUSAL><<<grid, 128, smem, (cudaStream_t)stream>>>(a);
+  else attn_fwd_kernel<1, CAUSAL><<<grid, 128, smem, (cudaStream_t)stream>>>(a);
   ES3_LAUNCH_CHECK("attn_fwd_kernel");
   return 0;
+}
+
+extern "C" int es3_attention_mma_bf16(const void* qkv, void* out, int B, int H, int W, int C, int num_heads, int win,
+                                      float scale, void* stream) {
+  return attention_mma<false>(qkv, out, B, H, W, C, num_heads, win, scale, stream);
+}
+
+// Causal self-attention over B sequences of L tokens (the mma.sync kernel with CAUSAL = true; sequences are one row
+// of L tokens, global attention).
+extern "C" int es3_attention_causal_bf16(const void* qkv, void* out, int B, int L, int C, int num_heads, float scale,
+                                         void* stream) {
+  ES3_REQUIRE(L >= 1, "es3_attention_causal_bf16: L must be >= 1 (L=%d)", L);
+  return attention_mma<true>(qkv, out, B, 1, L, C, num_heads, 0, scale, stream);
 }

@@ -12,7 +12,8 @@ so a merged EfficientSAM3 checkpoint (`detector.backbone.vision_backbone.` + the
 unchanged.  Everything runs on the kernels the stage-1 student and the FPN already use; this file is composition only.
 `build_efficientsam3_point_segmenter` puts the SAM heads on top (the SAM-1-task use of EfficientSAM3,
 efficientsam3_examples/efficientsam3_for_sam1_task_example.py:161-198).  Out of scope: the detector / text side of
-`build_efficientsam3_image_model` (SURVEY.md section 2)."""
+`build_efficientsam3_image_model` (SURVEY.md section 2).  The text encoders of `_create_text_encoder` /
+`_create_student_text_encoder` (model_builder.py:487-556) are `create_text_encoder` / `create_student_text_encoder`."""
 from __future__ import annotations
 
 import torch
@@ -114,3 +115,21 @@ def build_efficientsam3_point_segmenter(backbone_type: str, model_name: str, ima
     from .model.sam1_task import Sam3PointPromptSegmenter
     return Sam3PointPromptSegmenter(image_size=image_size, vision_backbone=create_student_vision_backbone(
         backbone_type, model_name, enable_inst_interactivity=True, img_size=image_size, embed_size=image_size // 14))
+
+
+def create_text_encoder(bpe_path: str):
+    """`_create_text_encoder(bpe_path)` (model_builder.py:487-496): the SAM3 text encoder, width 1024, 16 heads, 24 layers,
+    32-entry positional table, resizer to d_model 256."""
+    from .model.text_encoder_ve import VETextEncoder
+    from .model.tokenizer_ve import SimpleTokenizer
+    return VETextEncoder(tokenizer=SimpleTokenizer(bpe_path=bpe_path), d_model=256, width=1024, heads=16, layers=24)
+
+
+def create_student_text_encoder(bpe_path: str, backbone_type: str, context_length: int = 32):
+    """`_create_student_text_encoder(bpe_path, backbone_type, context_length)` (model_builder.py:499-556): the MobileCLIP
+    student with a `context_length`-entry table, projector to d_model 256."""
+    from .model.text_encoder_student import TextStudentEncoder
+    from .stage1.model import text_student_cfg
+    cfg = text_student_cfg(backbone_type)
+    cfg["context_length"] = context_length
+    return TextStudentEncoder(cfg=cfg, context_length=context_length, output_dim=256, bpe_path=bpe_path)

@@ -488,6 +488,57 @@ def attention(qkv, B, H, W, C, num_heads, win, scale, impl=None):
     return out
 
 
+def attention_causal(qkv, B, L, C, num_heads, scale):
+    """qkv: [B*L, 3C] bf16 -> [B*L, C] bf16; token l attends to tokens <= l of its own sequence."""
+    _chk(qkv, torch.bfloat16, "qkv")
+    _ensure_init(qkv)
+    assert qkv.is_contiguous() and qkv.shape == (B * L, 3 * C)
+    out = torch.empty((B * L, C), device=qkv.device, dtype=torch.bfloat16)
+    _call("es3_attention_causal_bf16", f"attention_causal[L={L}]", _nb(qkv, out), 2 * B * L * (L + 1) * C, qkv.data_ptr(),
+          out.data_ptr(), B, L, C, num_heads, float(scale), _stream())
+    return out
+
+
+def text_embed(ids, table, pos=None, emb="none"):
+    """ids: [B,L] int64 CUDA, already checked against the table on the host; table [V,C] fp32; pos [L,C] fp32 | None.
+    Returns (x [B*L,C] fp32 residual stream, embedding [B*L,C] fp32 | None); emb = "none" | "pos" (x itself) | "plain"."""
+    _chk(ids, torch.int64, "ids"); _chk(table, torch.float32, "table")
+    _ensure_init(table)
+    assert ids.dim() == 2 and ids.is_contiguous() and table.dim() == 2 and table.is_contiguous()
+    B, L = ids.shape
+    V, C = table.shape
+    if pos is not None:
+        _chk(pos, torch.float32, "pos")
+        assert pos.is_contiguous() and pos.shape == (L, C), (pos.shape, L, C)
+    x = torch.empty((B * L, C), device=table.device, dtype=torch.float32)
+    e = torch.empty_like(x) if emb == "plain" else None
+    _call("es3_text_embed", "text_embed", _nb(ids, x, e, pos) + B * L * C * 4, 0, ids.data_ptr(), table.data_ptr(), V, _ptr(pos),
+          x.data_ptr(), _ptr(e), 0, B, L, C, _stream())
+    return x, (x if emb == "pos" else e)
+
+
+REPMIXER_MAX_L = 128
+
+
+def repmixer(x, B, L, wm, bm, wf, bf):
+    """RepMixerBlock prologue on x [B*L, C] fp32: (x1 fp32 [B*L,C], u bf16 [B*L,C]); taps [11, C] fp32, biases [C]."""
+    _chk(x, torch.float32, "x")
+    _ensure_init(x)
+    if not 1 <= L <= REPMIXER_MAX_L:
+        raise ValueError(f"RepMixerBlock: the native kernel keeps a sequence in shared memory and takes 1..{REPMIXER_MAX_L} "
+                         f"tokens, got {L}")
+    C = x.shape[1]
+    assert x.is_contiguous() and x.shape[0] == B * L
+    for t in (wm, bm, wf, bf):
+        _chk(t, torch.float32, "repmixer weights")
+        assert t.is_contiguous()
+    x1 = torch.empty_like(x)
+    u = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16)
+    _call("es3_repmixer_bf16", "repmixer", _nb(x, x1, u), 4 * 11 * B * L * C, x.data_ptr(), x1.data_ptr(), u.data_ptr(),
+          wm.data_ptr(), bm.data_ptr(), wf.data_ptr(), bf.data_ptr(), B, L, C, _stream())
+    return x1, u
+
+
 def tokens_f32_to_nchw(x, B, H, W):
     _chk(x, torch.float32, "x")
     _ensure_init(x)

@@ -5,6 +5,10 @@ dictionary work, no tensors are touched:
                             (`module.`, `student_trunk.`, already-merged prefixes stripped), re-rooted under
                             `detector.backbone.vision_backbone.trunk.model.` and laid over a full SAM3 checkpoint whose own trunk
                             weights are dropped
+  merge_text_student_into_sam3
+                            stage1/convert_text_encoder_weights_stage1.py:8-19, 102-163: the same for a stage-1 text student
+                            (`module.`, `detector.backbone.language_backbone.`, `backbone.language_backbone.` stripped), re-rooted
+                            under `detector.backbone.language_backbone.`; the teacher's keys under the replace prefix are dropped
   clean_merged_keys         sam3/sam3/model_builder.py:594-612 (`_load_checkpoint`): `detector.` and `student_trunk.` removed, so the
                             result loads into efficientsam3_b200.model_builder modules (`backbone.vision_backbone.trunk.model.*`)
 """
@@ -38,6 +42,32 @@ def merge_student_into_sam3(student_sd: dict, sam3_sd: dict, target_prefix: str 
         if rep and k.startswith(rep):
             continue                                  # the teacher's trunk is replaced by the student
         if any(k.startswith(p) for p in skips) or k in merged:
+            continue
+        merged[k] = v
+    return merged
+
+
+_TEXT_STUDENT_PREFIXES = ("module.", "detector.backbone.language_backbone.", "backbone.language_backbone.")
+
+
+def normalize_text_student_key(key: str) -> str:
+    for p in _TEXT_STUDENT_PREFIXES:
+        if key.startswith(p):
+            key = key[len(p):]
+    return key
+
+
+def merge_text_student_into_sam3(student_sd: dict, sam3_sd: dict, target_prefix: str = "detector.backbone.language_backbone.",
+                                 replace_prefix: str | None = None, skip_teacher_prefixes=()) -> dict:
+    """Returns the merged state_dict; the replace prefix defaults to the target prefix (the SAM3 text encoder's keys)."""
+    prefix = target_prefix.strip(".")
+    prefix = f"{prefix}." if prefix else ""
+    rep = replace_prefix.strip(".") if replace_prefix is not None else target_prefix.strip(".")
+    rep = f"{rep}." if rep else ""
+    skips = [p.strip(".") + "." for p in skip_teacher_prefixes if p is not None]
+    merged = {prefix + normalize_text_student_key(k): v for k, v in student_sd.items()}
+    for k, v in sam3_sd.items():
+        if (rep and k.startswith(rep)) or any(k.startswith(p) for p in skips) or k in merged:
             continue
         merged[k] = v
     return merged

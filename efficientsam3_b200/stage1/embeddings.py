@@ -9,6 +9,9 @@ Reference behaviour being replaced:
   * the student side decodes a record as seed = int32 at offset 0, embedding = fp16[topk * num_embedding] after it
     (stage1/data/augmentation/dataset_wrapper.py:50-62).
 
+The text dump (stage1/save_embedding_text_stage1.py:86-140) stores the same record, `int32 seed || fp16[Seq * 256]`, with the
+teacher's memory laid out [B, Seq, 256]; `save_text_embeddings_one_epoch` feeds it through the same writer and dumper.
+
 Design: the fp32 -> fp16 cast runs on the device (es3_cast_f32_to_f16) so the D2H copy moves 2 B/element; device and
 pinned host staging are double-buffered; the copy is issued on a side stream behind an event, and a host thread turns
 finished buffers into records -- so batch i's D2H and file writes overlap batch i+1's teacher forward (the reference
@@ -236,6 +239,41 @@ def save_embeddings_one_epoch(model, data_loader, path: str, rank: int = 0, max_
                     dumper = EmbeddingDumper(writer, dev, max(cap, out.numel()))
                 dumper.submit(out, keys, np.asarray(seeds).astype(np.int32))
                 n += x.shape[0]
+        finally:
+            if dumper is not None:
+                dumper.close()
+    return n
+
+
+def _text_batch(batch):
+    """(captions, keys, seeds) from either loader layout save_embedding_text_stage1.py:103-118 accepts:
+    [captions, [keys, seeds]] (column-oriented) or [(caption, (key, seed)), ...] (row-oriented)."""
+    if isinstance(batch, (list, tuple)) and len(batch) == 2 and isinstance(batch[0], (list, tuple)) and len(batch[0]) > 0 \
+            and isinstance(batch[0][0], str):
+        return list(batch[0]), list(batch[1][0]), list(batch[1][1])
+    if isinstance(batch, (list, tuple)) and len(batch) > 0 and isinstance(batch[0], tuple):
+        return [b[0] for b in batch], [b[1][0] for b in batch], [b[1][1] for b in batch]
+    raise ValueError(f"Unknown batch structure. Type: {type(batch)}")
+
+
+@torch.no_grad()
+def save_text_embeddings_one_epoch(model, loader, path: str, rank: int = 0):
+    """Native counterpart of the text dump (save_embedding_text_stage1.py:86-140): per batch, the text teacher's memory
+    [Seq, B, 256] is stored as one record per caption, `int32 seed || fp16[Seq * 256]` in [Seq, 256] order.  `model` is a
+    SAM3TextTeacherEncoder (or anything with its forward(captions, device)).  Returns the number of records written."""
+    model.eval()
+    dev = next(model.parameters()).device
+    dumper = None
+    n = 0
+    with EmbeddingStoreWriter(path, rank) as writer:
+        try:
+            for batch in loader:
+                captions, keys, seeds = _text_batch(batch)
+                out = model(captions, device=dev).transpose(0, 1).contiguous()     # [B, Seq, 256] fp32
+                if dumper is None:
+                    dumper = EmbeddingDumper(writer, dev, out.numel())
+                dumper.submit(out, [str(k) for k in keys], np.asarray(seeds).astype(np.int32))
+                n += len(captions)
         finally:
             if dumper is not None:
                 dumper.close()

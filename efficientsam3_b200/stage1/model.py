@@ -5,9 +5,13 @@ state_dict keys, forward on libes3.so.
   ImageStudentEncoder                 stage1/model.py:188-211   (head.0/1/3 keys preserved)
   EfficientViTAdapter                 stage1/model.py:327-335
   _build_backbone                     stage1/model.py:386-417
+  build_text_student_model(config)    stage1/model.py:42-165    (TextStudentEncoder, model/text_encoder_student.py)
+  build_text_teacher_model(config)    stage1/model.py:178-185
+  SAM3TextTeacherEncoder              stage1/model.py:252-284   (VETextEncoder, model/text_encoder_ve.py)
 
 `config` needs MODEL.BACKBONE, DATA.IMG_SIZE, DISTILL.EMBED_DIM, DISTILL.EMBED_SIZE (yacs CfgNode or any
-attribute namespace).
+attribute namespace); the text builders read MODEL.BACKBONE / PRETRAINED / RESUME, DISTILL.EMBED_DIM / CONTEXT_LENGTH /
+POS_EMBED_TABLE_SIZE and, for string input, the CLIP vocabulary path MODEL.BPE_PATH (the reference uses its bundled copy).
 """
 from __future__ import annotations
 
@@ -167,6 +171,102 @@ class StudentTrainFunction(torch.autograd.Function):
             arena.head_grads_ready()                               # the head's weights (2/3 of EV-M's parameters) are final: exchange them now
         body.backward(d, grads)
         return (None, None) + tuple(grads.get(p) for p in ctx.params)
+
+
+TEXT_STUDENT_DEFAULT_CFG = {   # stage1/model.py:46-59
+    "context_length": 77, "vocab_size": 49408, "dim": 512, "ffn_multiplier_per_layer": 4.0, "n_heads_per_layer": 8,
+    "n_transformer_layers": 12, "norm_layer": "layer_norm_fp32", "causal_masking": False, "model_name": "base",
+    "embed_dropout": 0.0, "no_scale_embedding": False, "no_pos_embedding": False}
+
+TEXT_STUDENT_VARIANTS = {      # stage1/model.py:61-96; any other name keeps the default cfg (no error, as in the reference)
+    "MobileCLIP-S0": dict(dim=512, n_transformer_layers=4, n_heads_per_layer=8, model_name="mct", ffn_multiplier_per_layer=4.0),
+    **{n: dict(dim=512, n_transformer_layers=12, n_heads_per_layer=8, model_name="base")
+       for n in ("MobileCLIP-S1", "MobileCLIP2-S0", "MobileCLIP2-S2")},
+    "MobileCLIP-B": dict(dim=512, n_transformer_layers=12, n_heads_per_layer=8, model_name="base", causal_masking=True),
+    **{n: dict(dim=768, n_transformer_layers=12, n_heads_per_layer=12, model_name="base")
+       for n in ("MobileCLIP2-S3", "MobileCLIP2-S4", "MobileCLIP2-L")},
+}
+
+
+def text_student_cfg(backbone: str) -> dict:
+    cfg = dict(TEXT_STUDENT_DEFAULT_CFG)
+    cfg.update(TEXT_STUDENT_VARIANTS.get(backbone, {}))
+    return cfg
+
+
+def build_text_student_model(config, logger=None):
+    """stage1/model.py:42-165.  MODEL.PRETRAINED: a student checkpoint or a full MobileCLIP checkpoint (its `text_encoder.*`
+    keys are renamed to `encoder.*`), loaded with strict=False; a load failure only warns, as in the reference."""
+    from ..model.text_encoder_student import TextStudentEncoder
+    cfg = text_student_cfg(config.MODEL.BACKBONE)
+    context_length = getattr(config.DISTILL, "CONTEXT_LENGTH", 32)
+    table = getattr(config.DISTILL, "POS_EMBED_TABLE_SIZE", 0)
+    cfg["context_length"] = context_length if table in (None, 0) else table
+    model = TextStudentEncoder(cfg=cfg, context_length=context_length, output_dim=config.DISTILL.EMBED_DIM,
+                               bpe_path=getattr(config.MODEL, "BPE_PATH", None))
+    if logger:
+        logger.info(f"Text encoder context_length: {context_length}")
+        logger.info(f"Text encoder pos_embed_table_size: {cfg['context_length']}")
+    path = getattr(config.MODEL, "PRETRAINED", None)
+    if path:
+        try:
+            sd = torch.load(path, map_location="cpu")
+            if "text_encoder.embedding_layer.weight" in sd:
+                sd = {k.replace("text_encoder.", "encoder.", 1): v for k, v in sd.items() if k.startswith("text_encoder.")}
+            missing, unexpected = model.load_state_dict(sd, strict=False)
+            if logger:
+                logger.info(f"Loaded pretrained weights: {len(missing)} missing, {len(unexpected)} unexpected keys")
+        except Exception as e:   # the reference continues from random initialisation (stage1/model.py:158-163)
+            msg = f"Failed to load pretrained weights: {e}"
+            if logger:
+                logger.error(msg)
+                logger.warning("Continuing with random initialization...")
+            else:
+                print(f"Warning: {msg}")
+    return model
+
+
+def build_text_teacher_model(config):
+    """stage1/model.py:178-185."""
+    checkpoint = getattr(config.MODEL, "RESUME", None) or None
+    return SAM3TextTeacherEncoder(checkpoint_path=checkpoint, context_length=getattr(config.DISTILL, "CONTEXT_LENGTH", 32),
+                                  bpe_path=getattr(config.MODEL, "BPE_PATH", None))
+
+
+class SAM3TextTeacherEncoder(nn.Module):
+    """stage1/model.py:252-284: the frozen SAM3 text encoder -> memory [Seq, B, 256] fp32.  Only the language backbone is
+    instantiated, under the reference's key prefix `sam3.backbone.language_backbone.`; checkpoints with the `detector.` prefix
+    load too.  It is built with its 32-entry positional table (VETextEncoder's default) and tokenises at `context_length`."""
+
+    def __init__(self, checkpoint_path=None, context_length=32, bpe_path=None, ve_overrides=None):
+        super().__init__()
+        from ..model.text_encoder_ve import VETextEncoder
+        from ..model.tokenizer_ve import SimpleTokenizer
+        self.context_length = context_length
+        kw = dict(d_model=256, width=1024, heads=16, layers=24)      # model_builder.py:487-496
+        kw.update(ve_overrides or {})
+        tok = SimpleTokenizer(bpe_path=bpe_path) if bpe_path is not None else None
+        self.sam3 = _Holder()
+        self.sam3.backbone = _Holder()
+        self.sam3.backbone.language_backbone = VETextEncoder(tokenizer=tok, **kw)
+        if checkpoint_path:
+            sd = torch.load(checkpoint_path, map_location="cpu")
+            sd = sd.get("model", sd)
+            sd = {("sam3." + k[len("detector."):] if k.startswith("detector.") else k): v for k, v in sd.items()}
+            own = set(self.state_dict().keys())
+            self.load_state_dict({k: v for k, v in sd.items() if k in own}, strict=False)
+        for p in self.parameters():
+            p.requires_grad = False
+        self.eval()
+        self.sam3.backbone.language_backbone.context_length = context_length
+
+    def train(self, mode: bool = True):  # frozen teacher: always eval
+        return super().train(False)
+
+    @torch.no_grad()
+    def forward(self, text, device=None):
+        _, memory, _ = self.sam3.backbone.language_backbone(text, input_boxes=None, device=device)
+        return memory[:self.context_length] if memory.shape[0] > self.context_length else memory
 
 
 def build_image_teacher_model(config):

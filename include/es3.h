@@ -186,6 +186,26 @@ int es3_cast_f32_to_f16(const float* in, void* out, long long n, void* stream);
 int es3_litemla_attn_tc(const void* ms, long long ld, float* kv_ws, void* att, long long ldo, int B, int HW, int heads2,
                         float eps, void* stream);
 
+/* ------------------------------------------------------------------------------------------ text encoders */
+/* Causal softmax attention, head_dim 64, over B sequences of L tokens on the fused qkv activation [B*L, 3C] bf16 ->
+ * [B*L, C] bf16: token l attends to tokens 0..l (the triu(-inf) additive mask of MobileCLIP-B and the SAM3 text
+ * teacher, mobile_clip.py:825-831, text_encoder_ve.py:220-226).  Non-causal text attention is es3_attention_bf16 with
+ * H = 1, W = L, win = 0. */
+int es3_attention_causal_bf16(const void* qkv, void* out, int B, int L, int C, int num_heads, float scale, void* stream);
+/* Token embedding: x[b*L+l] = table[ids[b,l]] (+ pos[l]) as fp32 [B*L, C] (the residual stream); emb (optional) receives
+ * the positional-added rows (emb_with_pos = 1, MobileCLIP forward_embedding, mobile_clip.py:815-823) or the plain table
+ * rows (0, the VE teacher's inputs_embeds, text_encoder_ve.py:303).  ids int64 (device), table [vocab, C] fp32, pos
+ * [L, C] fp32 or NULL; C % 4 == 0.  Callers validate ids against vocab on the host; an id outside the table is never
+ * dereferenced (its row reads as zeros). */
+int es3_text_embed(const long long* ids, const float* table, int vocab, const float* pos, float* x, float* emb, int emb_with_pos,
+                   int B, int L, int C, void* stream);
+/* RepMixerBlock prologue, eval mode (mobile_clip.py:545-702), over x [B*L, C] fp32 tokens (sequence axis = the conv's W):
+ * x1 = bm + sum_k wm[k] x[l+k-5] (RepMixer with BN_skip, BN(conv 1x11), identity and layer scale folded into the
+ * taps wm [11][C] and bias bm [C], zero padding) in fp32, then u = bf + sum_k wf[k] x1[l+k-5] (ConvFFN.conv: depthwise
+ * 1x11 + BN folded, wf [11][C], bf [C]) in bf16 -- the A operand of fc1.  1 <= L <= 128, C % 32 == 0. */
+int es3_repmixer_bf16(const float* x, float* x1, void* u, const float* wm, const float* bm, const float* wf, const float* bf,
+                      int B, int L, int C, void* stream);
+
 /* ------------------------------------------------------------------------------------------ SAM heads */
 /* PositionEmbeddingRandom over an h x w grid -> [h*w, 2F] fp32 (PromptEncoder.get_dense_pe, prompt_encoder.py:61-69). */
 int es3_dense_pe(const float* gauss, int F, int h, int w, float* out, void* stream);

@@ -29,6 +29,17 @@ SIGNATURES: dict[str, list] = {
     "es3_attention_causal_bf16": [_vp, _vp, _i, _i, _i, _i, _f, _vp],
     "es3_text_embed": [_vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "es3_repmixer_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp],
+    # text-student backward and text KD loss (text_bwd.cu)
+    "es3_text_attn_bwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp],
+    "es3_layernorm_bwd_f32": [_vp, _vp, _vp, _vp, _f, _vp, _vp, _ll, _i, _vp, _vp, _vp, _vp],
+    "es3_text_embed_grad": [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp],
+    "es3_text_pos_grad": [_vp, _i, _i, _i, _i, _vp, _vp],
+    "es3_text_pos_resize": [_vp, _i, _i, _i, _vp, _vp],
+    "es3_text_kd_loss_fwd": [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp],
+    "es3_text_kd_loss_bwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp],
+    "es3_text_consistency_fwd": [_vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp],
+    "es3_text_consistency_bwd": [_vp, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp],
+    "es3_cast_f32_to_bf16": [_vp, _vp, _ll, _vp],
     "es3_tokens_f32_to_nchw": [_vp, _vp, _i, _i, _i, _vp],
     "es3_cast_f32_to_f16": [_vp, _vp, _ll, _vp],
     "es3_convt2x2_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp],
@@ -122,6 +133,7 @@ SIZE_HELPERS: dict[str, list] = {
     "es3_dwconv_wgrad_tiled_ws_floats": [_i, _i, _i, _i, _i],
     "es3_se_bwd_ws_floats": [_i, _i, _i],
     "es3_layernorm_bwd_ws_floats": [_ll, _i],
+    "es3_layernorm_bwd_f32_ws_floats": [_ll, _i],
     "es3_colsum_f32_ws_floats": [_ll, _i],
     "es3_wgrad_tc_ws_floats": [_ll, _i, _i],
     "es3_litemla_attn_f32_ws_floats": [_i, _i, _i, _i],

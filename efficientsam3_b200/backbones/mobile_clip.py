@@ -2,7 +2,8 @@
 same class names, constructor arguments and state_dict keys (`embedding_layer.weight`,
 `positional_embedding.pos_embed.pos_embed`, `transformer.N.pre_norm_mha.{0,1.qkv_proj,1.out_proj}.*`,
 `transformer.N.pre_norm_ffn.{0,1,4}.*`, the RepMixerBlock's `token_mixer.{norm,mixer}.*`, `convffn.*`, `layer_scale`,
-`final_layer_norm.*`, `projection_layer`).  The nn modules are parameter containers; eval-mode forward only.
+`final_layer_norm.*`, `projection_layer`).  The nn modules are parameter containers.  Eval-mode forward for every student;
+train-mode forward + backward for the base (TransformerEncoder-only) students: TextStudentTrainGraph at the end of this file.
 
 Device path (all libes3.so; fp32 residual stream, bf16 GEMM operands, fp32 accumulation / LayerNorm / softmax):
   embedding gather + positional add                      es3_text_embed
@@ -22,7 +23,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
-from ..nn_utils import NativePlanMixin, bn_scale_bias
+from ..nn_utils import NativePlanMixin, bn_scale_bias, cached_pack
 
 
 # ----------------------------------------------------------------------------------------------- parameter containers
@@ -256,8 +257,8 @@ def run_layers(layers, x, B, L, causal):
 def check_native(module: nn.Module, what: str, training: bool):
     """The raise paths shared by the text modules: no CPU fallback, eval-mode only, no strict (fp32) mode yet."""
     if training:
-        raise NotImplementedError(f"{what}: the text encoders' native path is eval-mode (forward) only; training the text "
-                                  "student (backward, batch-statistics BatchNorm) is not built yet.  Call .eval() first.")
+        raise NotImplementedError(f"{what}: this module's native path is eval-mode (forward) only; training is built for "
+                                  "TextStudentEncoder with a TransformerEncoder (base) trunk.  Call .eval() first.")
     if ops.precision() == "strict":
         raise NotImplementedError(f"{what}: the strict (fp32) precision mode is not built for the text encoders")
     p = next(module.parameters())
@@ -338,7 +339,11 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
     @torch.no_grad()
     def embed_tokens(self, ids: torch.Tensor):
         """forward_embedding on validated ids -> fp32 [B*L, C] (token + positional embedding), also the residual stream."""
-        dev = check_native(self, "MobileCLIPTextTransformer", self.training)
+        check_native(self, "MobileCLIPTextTransformer", self.training)
+        return self._embed(ids)
+
+    def _embed(self, ids):
+        dev = next(self.parameters()).device
         h = host_ids(ids, self.vocab_size)
         p = self._plan()
         B, L = h.shape
@@ -352,6 +357,9 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
     def encode_tokens(self, x: torch.Tensor):
         """The transformer + final LayerNorm on embeddings x [B, L, C] fp32 CUDA -> (fp32 [B*L, C], bf16 [B*L, C])."""
         check_native(self, "MobileCLIPTextTransformer", self.training)
+        return self._encode(x)
+
+    def _encode(self, x):
         if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[2] == self.model_dim):
             raise ValueError(f"expected CUDA fp32 embeddings [B, L, {self.model_dim}]; the native path has no CPU fallback")
         B, L, C = x.shape
@@ -370,9 +378,9 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
             emb = text
         else:
             ids = host_ids(text, self.vocab_size)
-            emb = self.embed_tokens(ids)
+            emb = self._embed(ids)
         B, L, C = emb.shape
-        yf, yb = self.encode_tokens(emb)
+        yf, yb = self._encode(emb)
         if return_all_tokens:
             return yf.view(B, L, C)
         # pooled: EOT token (argmax of the ids) or, for embeddings, the last token (mobile_clip.py:873-882)
@@ -384,3 +392,199 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
     def forward(self, text_tokens, key_padding_mask=None, return_all_tokens=False, input_is_embeddings=False, *args, **kwargs):
         return self.encode_text(text_tokens, key_padding_mask=key_padding_mask, return_all_tokens=return_all_tokens,
                                 input_is_embeddings=input_is_embeddings)
+
+
+# ----------------------------------------------------------------------------------------------- training graph (base trunk)
+# Train-mode forward + backward of the base students (TransformerEncoder layers only), in the scheme of tinyvit_train.py: units
+# with forward(x) / backward(d, grads), wrapped into ONE autograd node by model.text_encoder_student.TextStudentTrainFunction.
+# The residual stream and its gradient are fp32 ([B*L, C]); GEMM operands are bf16 with fp32 accumulation.
+#   embedding + positional table        es3_text_embed (+ es3_text_pos_resize); grads es3_text_embed_grad, es3_text_pos_grad
+#   LayerNorm                           es3_layernorm_f32 / es3_layernorm_bwd_f32 (fp32 dx + the residual gradient, bf16 copy)
+#   nn.Linear (+ GELU)                  es3_gemm_bf16_ex [+ es3_affine_act]; grads es3_wgrad_pw, column sums / es3_bn_act_bwd_*,
+#                                       es3_gemm_bf16_ex on the cached W^T (nn_utils.cached_pack, invalidated by each optimiser step)
+#   attention                           es3_attention_bf16 | es3_attention_causal_bf16 / es3_text_attn_bwd
+def _grad_of(grads, p):
+    from .efficientvit_train import _grad_of as g
+    return g(grads, p)
+
+
+def check_trainable(module: nn.Module, enc: "MobileCLIPTextTransformer", what: str):
+    """The raise paths of the training graph: S0-style RepMixerBlocks, strict precision, CPU modules, dropout > 0."""
+    if any(isinstance(b, RepMixerBlock) for b in enc.transformer):
+        raise NotImplementedError(f"{what}: training is built for the TransformerEncoder (base) students; the RepMixerBlocks of "
+                                  "MobileCLIP-S0 (batch-statistics BatchNorm, 1x11 depthwise backward) are not built yet.  "
+                                  "Call .eval() first.")
+    if ops.precision() == "strict":
+        raise NotImplementedError(f"{what}: the strict (fp32) precision mode is not built for the text encoders")
+    for m in module.modules():
+        if isinstance(m, nn.Dropout) and m.p > 0:
+            raise NotImplementedError(f"{what}: dropout p={m.p} in train mode is not built (every shipped text student uses p = 0)")
+    p = next(module.parameters())
+    if not p.is_cuda:
+        raise RuntimeError(f"{what}: the module is on {p.device}; the native path runs on a CUDA device and has no CPU fallback")
+    return p.device
+
+
+class _TextLinear:
+    """nn.Linear [+ GELU] on [M, K] bf16 rows."""
+
+    def __init__(self, lin: nn.Linear, act=None):
+        self.lin, self.act = lin, act
+        self.saved = None
+
+    def _w(self):
+        lin = self.lin
+        return cached_pack(lin, "text_w", lin.weight, lambda: lin.weight.detach().to(torch.bfloat16).contiguous())
+
+    def _wt(self):
+        lin = self.lin
+        return cached_pack(lin, "text_wt", lin.weight, lambda: lin.weight.detach().to(torch.bfloat16).t().contiguous())
+
+    def forward(self, x2, residual=None, out_dtype=torch.bfloat16):
+        b = self.lin.bias.detach().float().contiguous()
+        if self.act is None:
+            self.saved = (x2, None, b)
+            return ops.gemm(x2, self._w(), bias=b, residual=residual, out_dtype=out_dtype)
+        z = ops.gemm(x2, self._w())
+        self.saved = (x2, z, b)
+        return ops.affine_act(z, None, b, self.act)
+
+    def backward(self, dy, grads, dy_f32=None, out_dtype=torch.bfloat16):
+        """dy: bf16 gradient of the output (dy_f32: the same in fp32, for the bias sum).  Returns the input gradient."""
+        x2, z, b = self.saved
+        self.saved = None
+        lin = self.lin
+        gb = _grad_of(grads, lin.bias)
+        if z is None:
+            dz = dy
+            if gb is not None:
+                if dy_f32 is not None:
+                    ops.colsum_f32(dy_f32, gb)
+                else:
+                    ops.bn_act_bwd(dz, dz, None, None, None, "none", dbeta=gb, apply=False)
+        else:
+            dz = ops.bn_act_bwd(dy, z, None, b, self.act, "none", dbeta=gb)
+        gw = _grad_of(grads, lin.weight)
+        if gw is not None:
+            ops.wgrad_pw(dz, x2, gw)
+        return ops.gemm(dz, self._wt(), out_dtype=out_dtype)
+
+
+def _ln_params(ln):
+    return ln.weight.detach().float().contiguous(), ln.bias.detach().float().contiguous(), ln.eps
+
+
+class TextEncoderLayerUnit:
+    """TransformerEncoder (mobile_clip.py:469-491): x1 = x + out_proj(attn(qkv(LN1(x)))); x2 = x1 + fc2(gelu(fc1(LN2(x1))))."""
+
+    def __init__(self, blk: TransformerEncoder, causal: bool):
+        self.n1, at, self.n2 = blk.pre_norm_mha[0], blk.pre_norm_mha[1], blk.pre_norm_ffn[0]
+        if at.head_dim != 64:
+            raise NotImplementedError(f"text attention backward is built for head_dim 64, got {at.head_dim}")
+        self.heads, self.scale, self.causal = at.num_heads, at.scaling, causal
+        self.qkv, self.proj = _TextLinear(at.qkv_proj), _TextLinear(at.out_proj)
+        self.fc1, self.fc2 = _TextLinear(blk.pre_norm_ffn[1], "gelu"), _TextLinear(blk.pre_norm_ffn[4])
+        self.saved = None
+
+    def forward(self, x, B, L):
+        C = x.shape[1]
+        y1, _ = ops.layernorm(x, *_ln_params(self.n1))
+        qkv = self.qkv.forward(y1)
+        if self.causal:
+            a = ops.attention_causal(qkv, B, L, C, self.heads, self.scale)
+        else:
+            a = ops.attention(qkv, B, 1, L, C, self.heads, 0, self.scale)
+        x1 = self.proj.forward(a, residual=x, out_dtype=torch.float32)
+        y2, _ = ops.layernorm(x1, *_ln_params(self.n2))
+        x2 = self.fc2.forward(self.fc1.forward(y2), residual=x1, out_dtype=torch.float32)
+        self.saved = (x, x1, qkv, a, B, L)
+        return x2
+
+    def backward(self, g, gb, grads, want_bf16=True):
+        """g: fp32 gradient of the layer output, gb: its bf16 copy -> (fp32 input gradient, bf16 copy | None)."""
+        x, x1, qkv, a, B, L = self.saved
+        self.saved = None
+        C = x.shape[1]
+        dh = self.fc2.backward(gb, grads, dy_f32=g)
+        dy2 = self.fc1.backward(dh, grads, out_dtype=torch.float32)
+        w2, _, eps2 = _ln_params(self.n2)
+        g1, g1b = ops.layernorm_bwd_f32(x1, dy2, w2, eps2, _grad_of(grads, self.n2.weight), _grad_of(grads, self.n2.bias), dres=g,
+                                        want_bf16=True)
+        da = self.proj.backward(g1b, grads, dy_f32=g1)
+        dqkv = ops.text_attn_bwd(qkv, a, da, B, L, C, self.heads, self.scale, self.causal)
+        dy1 = self.qkv.backward(dqkv, grads, out_dtype=torch.float32)
+        w1, _, eps1 = _ln_params(self.n1)
+        return ops.layernorm_bwd_f32(x, dy1, w1, eps1, _grad_of(grads, self.n1.weight), _grad_of(grads, self.n1.bias), dres=g1,
+                                     want_bf16=want_bf16)
+
+
+class TextEmbedUnit:
+    """forward_embedding (mobile_clip.py:815-823): table[ids] + the positional table, resized N -> L when they differ."""
+
+    def __init__(self, enc: "MobileCLIPTextTransformer"):
+        self.emb = enc.embedding_layer
+        self.lpe = enc.positional_embedding.pos_embed if enc.positional_embedding is not None else None
+        if self.lpe is not None and self.lpe.padding_idx is not None:
+            raise NotImplementedError("positional table with a padding_idx is not on the text students' path")
+        self.saved = None
+
+    def forward(self, ids_host, dev):
+        B, L = ids_host.shape
+        table = self.emb.weight.detach()
+        pos = None
+        if self.lpe is not None:
+            N, C = self.lpe.num_embeddings, self.lpe.embedding_dim
+            pos = self.lpe.pos_embed.detach().reshape(N, C)
+            if N != L:
+                pos = ops.text_pos_resize(pos.contiguous(), L)
+        x, _ = ops.text_embed(ids_host.to(dev, non_blocking=True), table.contiguous(), pos)
+        # the gradient's token grouping is built now, while the ids are on the host, and copied asynchronously
+        plan = ops.embed_grad_plan(ids_host, dev) if self.emb.weight.requires_grad else None
+        self.saved = (plan, B, L)
+        return x
+
+    def backward(self, dx, grads):
+        plan, B, L = self.saved
+        self.saved = None
+        ge = _grad_of(grads, self.emb.weight)
+        if ge is not None:
+            ops.text_embed_grad(dx, plan, ge)
+        if self.lpe is not None:
+            gp = _grad_of(grads, self.lpe.pos_embed)
+            if gp is not None:
+                ops.text_pos_grad(dx, B, L, gp)
+
+
+class TextStudentTrainGraph:
+    """TextStudentEncoder in train mode: embed -> TransformerEncoder layers -> final LayerNorm -> projector (fp32 memory)."""
+
+    def __init__(self, student):
+        enc = student.encoder
+        self.embed = TextEmbedUnit(enc)
+        self.layers = [TextEncoderLayerUnit(b, enc.causal_masking) for b in enc.transformer]
+        self.fln = enc.final_layer_norm
+        self.proj = _TextLinear(student.projector)
+        self.saved = None
+
+    def forward(self, ids_host, dev):
+        B, L = ids_host.shape
+        x0 = self.embed.forward(ids_host, dev)
+        x = x0
+        for u in self.layers:
+            x = u.forward(x, B, L)
+        yb, _ = ops.layernorm(x, *_ln_params(self.fln))
+        mem = self.proj.forward(yb, out_dtype=torch.float32)
+        self.saved = x
+        return mem.view(B, L, -1), x0.view(B, L, -1)
+
+    def backward(self, dmem, grads):
+        xs = self.saved
+        self.saved = None
+        dmem = dmem.reshape(-1, dmem.shape[-1]).contiguous()
+        dy = self.proj.backward(ops.cast_f32_to_bf16(dmem), grads, dy_f32=dmem, out_dtype=torch.float32)
+        w, _, eps = _ln_params(self.fln)
+        g, gb = ops.layernorm_bwd_f32(xs, dy, w, eps, _grad_of(grads, self.fln.weight), _grad_of(grads, self.fln.bias),
+                                      want_bf16=bool(self.layers))
+        for i in range(len(self.layers) - 1, -1, -1):
+            g, gb = self.layers[i].backward(g, gb, grads, want_bf16=i > 0)
+        self.embed.backward(g, grads)

@@ -539,6 +539,173 @@ def repmixer(x, B, L, wm, bm, wf, bf):
     return x1, u
 
 
+# ------------------------------------------------------------------------------------ text-student backward (text_bwd.cu)
+TEXT_ATTN_BWD_MAX_L = 128
+KERNELS_PER_CALL.update({"es3_layernorm_bwd_f32": 2, "es3_text_kd_loss_fwd": 2, "es3_text_consistency_fwd": 2,
+                         "es3_text_embed_grad": 2})
+
+
+def text_attn_bwd(qkv, o, dout, B, L, C, num_heads, scale, causal):
+    """Backward of attention / attention_causal on head_dim 64: qkv [B*L, 3C], o and dout [B*L, C] bf16 -> dqkv like qkv."""
+    if not 1 <= L <= TEXT_ATTN_BWD_MAX_L:
+        raise ValueError(f"text attention backward keeps a sequence in shared memory and takes 1..{TEXT_ATTN_BWD_MAX_L} tokens, "
+                         f"got {L}")
+    if C != 64 * num_heads:
+        raise ValueError(f"text attention backward is built for head_dim 64 (C={C}, heads={num_heads})")
+    for t, n in ((qkv, "qkv"), (o, "o"), (dout, "dout")):
+        _chk(t, torch.bfloat16, n)
+        assert t.is_contiguous()
+    _ensure_init(qkv)
+    assert qkv.shape == (B * L, 3 * C) and o.shape == (B * L, C) and dout.shape == (B * L, C)
+    dqkv = torch.empty_like(qkv)
+    _call("es3_text_attn_bwd", f"text_attn_bwd[L={L}]", _nb(qkv, o, dout, dqkv), 10 * B * L * L * C, qkv.data_ptr(), o.data_ptr(),
+          dout.data_ptr(), dqkv.data_ptr(), B, L, C, num_heads, int(bool(causal)), float(scale), _stream())
+    return dqkv
+
+
+def layernorm_bwd_f32(x, dy, gamma, eps, dgamma=None, dbeta=None, dres=None, want_bf16=False):
+    """nn.LayerNorm backward over fp32 rows: x, dy [M,C] fp32 -> (dx fp32 (+ dres), bf16 copy of dx | None);
+    dgamma / dbeta fp32 [C] accumulated in place."""
+    _chk(x, torch.float32, "x"); _chk(dy, torch.float32, "dy")
+    _ensure_init(x)
+    assert x.dim() == 2 and x.is_contiguous() and dy.is_contiguous() and dy.shape == x.shape
+    assert dres is None or (dres.is_contiguous() and dres.shape == x.shape and dres.dtype == torch.float32)
+    M, C = x.shape
+    dx = torch.empty_like(x)
+    dxb = torch.empty((M, C), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
+    ws = _f32ws(_lib.size("es3_layernorm_bwd_f32_ws_floats", M, C), x.device)
+    _call("es3_layernorm_bwd_f32", "layernorm_bwd_f32", _nb(x, dy, dx, dxb, dres), 12 * x.numel(), x.data_ptr(), dy.data_ptr(),
+          gamma.data_ptr(), _ptr(dres), float(eps), dx.data_ptr(), _ptr(dxb), M, C, ws.data_ptr(), _ptr(dgamma), _ptr(dbeta),
+          _stream())
+    return dx, dxb
+
+
+EMBED_GRAD_CHUNK = 32     # tokens per chunk of the embedding gradient's first pass
+
+
+def embed_grad_plan(ids_host: torch.Tensor, device):
+    """Host-side grouping of the token ids [B, L] (CPU int64) for text_embed_grad, built when the ids are tokenised: tokens sorted
+    by id and cut into chunks of at most EMBED_GRAD_CHUNK tokens of one id.  The index arrays go to `device` from pinned memory
+    (asynchronous copies, no stream synchronisation); the pinned sources are kept in the plan until the copies are done."""
+    flat = ids_host.reshape(-1)
+    order = torch.sort(flat, stable=True)
+    uid, counts = torch.unique_consecutive(order.values, return_counts=True)
+    nch = (counts + EMBED_GRAD_CHUNK - 1) // EMBED_GRAD_CHUNK               # chunks per distinct id
+    seg = torch.zeros(uid.numel() + 1, dtype=torch.int64)
+    seg[1:] = torch.cumsum(nch, 0)
+    starts = torch.zeros(uid.numel() + 1, dtype=torch.int64)
+    starts[1:] = torch.cumsum(counts, 0)
+    k = torch.arange(int(seg[-1]))
+    owner = torch.repeat_interleave(torch.arange(uid.numel()), nch)
+    chunk_start = torch.empty(int(seg[-1]) + 1, dtype=torch.int64)
+    chunk_start[:-1] = starts[owner] + (k - seg[owner]) * EMBED_GRAD_CHUNK
+    chunk_start[-1] = flat.numel()
+    host = [order.indices.to(torch.int32), chunk_start.to(torch.int32), seg.to(torch.int32), uid.contiguous()]
+    if device.type == "cuda":
+        host = [h.pin_memory() for h in host]
+    dev = [h.to(device, non_blocking=True) for h in host]
+    return dict(perm=dev[0], chunk_start=dev[1], seg=dev[2], uid=dev[3], nchunk=int(seg[-1]), host=host)
+
+
+def text_embed_grad(dx, plan, grad):
+    """grad [V, C] fp32 += nn.Embedding weight gradient of dx [B*L, C] fp32; plan from embed_grad_plan."""
+    _chk(dx, torch.float32, "dx"); _chk(grad, torch.float32, "grad")
+    _ensure_init(dx)
+    assert dx.is_contiguous() and grad.is_contiguous() and dx.shape[1] == grad.shape[-1]
+    C = dx.shape[1]
+    ws = _f32ws(plan["nchunk"] * C, dx.device)
+    _call("es3_text_embed_grad", "text_embed_grad", 2 * _nb(dx), dx.numel(), dx.data_ptr(), plan["perm"].data_ptr(),
+          plan["chunk_start"].data_ptr(), plan["nchunk"], plan["seg"].data_ptr(), plan["uid"].data_ptr(), plan["uid"].numel(), C,
+          ws.data_ptr(), grad.data_ptr(), _stream())
+    return grad
+
+
+def text_pos_grad(dx, B, L, grad):
+    """grad [.., N, C] fp32 += the positional-table gradient of dx [B*L, C] fp32 (bilinear N -> L resize transposed)."""
+    _chk(dx, torch.float32, "dx"); _chk(grad, torch.float32, "grad")
+    _ensure_init(dx)
+    assert dx.is_contiguous() and grad.is_contiguous() and dx.shape[0] == B * L
+    C = dx.shape[1]
+    N = grad.numel() // C
+    _call("es3_text_pos_grad", "text_pos_grad", _nb(dx, grad), dx.numel(), dx.data_ptr(), B, L, N, C, grad.data_ptr(), _stream())
+    return grad
+
+
+def text_pos_resize(table, L):
+    """table [N, C] fp32 -> [L, C] fp32 (the bilinear N -> L resize of LearnablePositionalEmbedding)."""
+    _chk(table, torch.float32, "table")
+    _ensure_init(table)
+    assert table.is_contiguous() and table.dim() == 2
+    N, C = table.shape
+    out = torch.empty((L, C), device=table.device, dtype=torch.float32)
+    _call("es3_text_pos_resize", "text_pos_resize", _nb(table, out), 3 * out.numel(), table.data_ptr(), N, L, C, out.data_ptr(),
+          _stream())
+    return out
+
+
+def text_kd_loss_fwd(preds, teacher, pad, cosine_weight):
+    """preds, teacher [B, L, D] fp32; pad [B, L] bool CUDA (True = padding token: masked loss) or None (plain loss).
+    Returns (out3 = (loss, mse, cos), per-sample partials [B, 3])."""
+    _chk(preds, torch.float32, "preds"); _chk(teacher, torch.float32, "teacher")
+    _ensure_init(preds)
+    assert preds.is_contiguous() and teacher.is_contiguous() and preds.shape == teacher.shape and preds.dim() == 3
+    B, L, D = preds.shape
+    if pad is not None:
+        _chk(pad, torch.bool, "pad")
+        assert pad.is_contiguous() and pad.shape == (B, L)
+    ws = torch.empty((B, 3), device=preds.device, dtype=torch.float32)
+    out = torch.empty((3,), device=preds.device, dtype=torch.float32)
+    _call("es3_text_kd_loss_fwd", "text_kd_loss_fwd", _nb(preds, teacher), 8 * preds.numel(), preds.data_ptr(), teacher.data_ptr(),
+          _ptr(pad), B, L, D, float(cosine_weight), ws.data_ptr(), out.data_ptr(), _stream())
+    return out, ws
+
+
+def text_kd_loss_bwd(preds, teacher, pad, ws, cosine_weight, grad_scale=1.0, scale_dev=None, gout=None):
+    _chk(preds, torch.float32, "preds"); _chk(teacher, torch.float32, "teacher")
+    _ensure_init(preds)
+    B, L, D = preds.shape
+    dp = torch.empty_like(preds)
+    _call("es3_text_kd_loss_bwd", "text_kd_loss_bwd", 3 * _nb(preds), 12 * preds.numel(), preds.data_ptr(), teacher.data_ptr(),
+          _ptr(pad), ws.data_ptr(), B, L, D, float(cosine_weight), float(grad_scale), _ptr(scale_dev), _ptr(gout), dp.data_ptr(),
+          _stream())
+    return dp
+
+
+def text_consistency_fwd(p, q, weight=0.0, loss=None):
+    """mse(mean_L(p), mean_L(q)) for p, q [B, L, D] fp32 -> (value [1] fp32, mean difference [B, D]); loss[0] += weight * value."""
+    _chk(p, torch.float32, "p"); _chk(q, torch.float32, "q")
+    _ensure_init(p)
+    assert p.is_contiguous() and q.is_contiguous() and p.shape == q.shape and p.dim() == 3
+    B, L, D = p.shape
+    mdiff = torch.empty((B, D), device=p.device, dtype=torch.float32)
+    ws = torch.empty((B,), device=p.device, dtype=torch.float32)
+    value = torch.empty((1,), device=p.device, dtype=torch.float32)
+    _call("es3_text_consistency_fwd", "text_consistency_fwd", _nb(p, q), 2 * p.numel(), p.data_ptr(), q.data_ptr(), B, L, D,
+          float(weight), mdiff.data_ptr(), ws.data_ptr(), _ptr(loss), value.data_ptr(), _stream())
+    return value, mdiff
+
+
+def text_consistency_bwd(mdiff, L, weight, dp, grad_scale=1.0, scale_dev=None, gout=None):
+    """dp [B, L, D] += d(weight * consistency)/dp; returns the gradient w.r.t. q."""
+    _chk(mdiff, torch.float32, "mdiff"); _chk(dp, torch.float32, "dp")
+    _ensure_init(dp)
+    assert dp.is_contiguous()
+    B, D = mdiff.shape
+    dq = torch.empty_like(dp)
+    _call("es3_text_consistency_bwd", "text_consistency_bwd", 3 * _nb(dp), dp.numel(), mdiff.data_ptr(), B, L, D, float(weight),
+          float(grad_scale), _ptr(scale_dev), _ptr(gout), dp.data_ptr(), dq.data_ptr(), _stream())
+    return dq
+
+
+def cast_f32_to_bf16(x):
+    _chk(x, torch.float32, "x")
+    _ensure_init(x)
+    assert x.is_contiguous()
+    y = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16)
+    _call("es3_cast_f32_to_bf16", "cast_f32_to_bf16", _nb(x, y), 0, x.data_ptr(), y.data_ptr(), x.numel(), _stream())
+    return y
+
+
 def tokens_f32_to_nchw(x, B, H, W):
     _chk(x, torch.float32, "x")
     _ensure_init(x)

@@ -57,10 +57,16 @@ class FlatAdamW:
 
     def __init__(self, model: torch.nn.Module, lr: float, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01,
                  loss_scale: float = 1.0, dynamic_loss_scale: bool = False, growth_interval: int = 2000,
-                 direct_grads: bool = True, overlap_allreduce: bool = True):
+                 direct_grads: bool = True, overlap_allreduce: bool = True, exclude=()):
         skip = model.no_weight_decay() if hasattr(model, "no_weight_decay") else ()
         skip_kw = model.no_weight_decay_keywords() if hasattr(model, "no_weight_decay_keywords") else ()
-        decay, no_decay = split_decay(model.named_parameters(), skip, skip_kw)
+        # `exclude`: parameter names left out of the arenas entirely (never updated, never decayed, `.grad` untouched), e.g. the
+        # text student's unused `encoder.projection_layer`, which torch AdamW skips in the reference because its grad stays None
+        excluded = set(exclude)
+        unknown = excluded - {n for n, _ in model.named_parameters()}
+        if unknown:
+            raise ValueError(f"FlatAdamW(exclude=...): no parameter named {sorted(unknown)}")
+        decay, no_decay = split_decay(((n, p) for n, p in model.named_parameters() if n not in excluded), skip, skip_kw)
         self._model = model
         self._plan_holders = None
         self.lr, self.betas, self.eps, self.weight_decay = lr, tuple(betas), eps, weight_decay
@@ -98,7 +104,7 @@ class FlatAdamW:
         self.overlap = bool(overlap_allreduce)
         head = [o for n, o in zip(self.names, self.offsets) if n.startswith("head.") and o < self.n_decay]
         self._head_lo = min(head) if head else self.n_decay        # [head_lo, n_decay): head.0.weight, head.3.weight (decay group tail)
-        if direct_grads and hasattr(model, "head"):
+        if direct_grads and (hasattr(model, "head") or getattr(model, "supports_direct_grads", False)):
             model._es3_grad_arena = self
         self.overlap_note = ("two buckets: the head's weight gradients [%d, %d) are all-reduced asynchronously as soon as the head's backward "
                              "has been enqueued (they overlap the backbone's backward), the rest after the backward returns"

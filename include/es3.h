@@ -206,6 +206,40 @@ int es3_text_embed(const long long* ids, const float* table, int vocab, const fl
 int es3_repmixer_bf16(const float* x, float* x1, void* u, const float* wm, const float* bm, const float* wf, const float* bf,
                       int B, int L, int C, void* stream);
 
+/* Text-student backward and the stage-1 text KD loss (text_bwd.cu).  Every reduction runs in a fixed order (no float atomics).
+ * es3_text_attn_bwd: backward of es3_attention_bf16 (H = 1, W = L) / es3_attention_causal_bf16 for head_dim 64, 1 <= L <= 128;
+ * qkv [B*L, 3C] bf16 in the forward's layout, o the forward output [B*L, C], dout like o -> dqkv [B*L, 3C] bf16 (softmax
+ * recomputed).  es3_layernorm_bwd_f32: nn.LayerNorm backward over fp32 rows (C % 4 == 0, C <= 768): dx = dLN(dy) (+ dres) in fp32,
+ * optionally also rounded to bf16 into dxb; dgamma += sum dy xhat, dbeta += sum dy; ws: es3_layernorm_bwd_f32_ws_floats(M, C).
+ * es3_text_embed_grad: grad [V][C] += segmented sums of dx rows, perm = token indices sorted by id (stable), cut into chunks
+ * (chunk_start [nchunk + 1]) that each hold tokens of one id, seg [U + 1] the first chunk of each distinct id uid [U]; summed
+ * per chunk into ws [nchunk][C], then per id in chunk order.  es3_text_pos_grad: grad [N][C] += batch sum of dx [B][L][C] through the transpose
+ * of the N -> L linear resize (F.interpolate bilinear, align_corners=False, on [1, 1, N, C]; identity when N == L).
+ * es3_text_kd_loss_fwd / _bwd: text MSE + cosine_weight * (1 - cosine) on preds / teacher [B][L][D] fp32, masked to the tokens
+ * with pad[b][l] == 0 (bytes; per-sample denominators, batch mean) when pad is non-null, plain means otherwise; out3 = (loss, mse, cos); ws: 3 B floats;
+ * the backward multiplies by grad_scale and the non-null device scalars scale_dev[0], gout[0].
+ * es3_text_consistency_fwd / _bwd: value = mse(mean_L(p), mean_L(q)), loss[0] += weight * value; backward dp += and dq = the
+ * gradients of weight * value.  es3_cast_f32_to_bf16: y = bf16(x), n % 4 == 0. */
+int es3_text_attn_bwd(const void* qkv, const void* o, const void* dout, void* dqkv, int B, int L, int C, int num_heads, int causal,
+                      float scale, void* stream);
+long long es3_layernorm_bwd_f32_ws_floats(long long M, int C);
+int es3_layernorm_bwd_f32(const float* x, const float* dy, const float* gamma, const float* dres, float eps, float* dx, void* dxb,
+                          long long M, int C, float* ws, float* dgamma, float* dbeta, void* stream);
+int es3_text_embed_grad(const float* dx, const int* perm, const int* chunk_start, int nchunk, const int* seg, const long long* uid,
+                        int U, int C, float* ws, float* grad, void* stream);
+int es3_text_pos_grad(const float* dx, int B, int L, int N, int C, float* grad, void* stream);
+/* The forward resize of the same table on the device: out [L][C] = resize(table [N][C]). */
+int es3_text_pos_resize(const float* table, int N, int L, int C, float* out, void* stream);
+int es3_text_kd_loss_fwd(const float* preds, const float* teacher, const unsigned char* pad, int B, int L, int D, float cosine_weight,
+                         float* ws, float* out3, void* stream);
+int es3_text_kd_loss_bwd(const float* preds, const float* teacher, const unsigned char* pad, const float* ws, int B, int L, int D,
+                         float cosine_weight, float grad_scale, const float* scale_dev, const float* gout, float* dpreds, void* stream);
+int es3_text_consistency_fwd(const float* p, const float* q, int B, int L, int D, float weight, float* mdiff, float* ws, float* loss,
+                             float* value, void* stream);
+int es3_text_consistency_bwd(const float* mdiff, int B, int L, int D, float weight, float grad_scale, const float* scale_dev,
+                             const float* gout, float* dp, float* dq, void* stream);
+int es3_cast_f32_to_bf16(const float* x, void* y, long long n, void* stream);
+
 /* ------------------------------------------------------------------------------------------ SAM heads */
 /* PositionEmbeddingRandom over an h x w grid -> [h*w, 2F] fp32 (PromptEncoder.get_dense_pe, prompt_encoder.py:61-69). */
 int es3_dense_pe(const float* gauss, int F, int h, int w, float* out, void* stream);

@@ -3,7 +3,8 @@ same class names, constructor arguments and state_dict keys (`embedding_layer.we
 `positional_embedding.pos_embed.pos_embed`, `transformer.N.pre_norm_mha.{0,1.qkv_proj,1.out_proj}.*`,
 `transformer.N.pre_norm_ffn.{0,1,4}.*`, the RepMixerBlock's `token_mixer.{norm,mixer}.*`, `convffn.*`, `layer_scale`,
 `final_layer_norm.*`, `projection_layer`).  The nn modules are parameter containers.  Eval-mode forward for every student;
-train-mode forward + backward for the base (TransformerEncoder-only) students: TextStudentTrainGraph at the end of this file.
+train-mode forward + backward for the base (TransformerEncoder-only) students and for MobileCLIP-S0 with its RepMixerBlocks'
+BatchNorms frozen in .eval(): TextStudentTrainGraph at the end of this file.
 
 Device path (all libes3.so; fp32 residual stream, bf16 GEMM operands, fp32 accumulation / LayerNorm / softmax):
   embedding gather + positional add                      es3_text_embed
@@ -210,10 +211,10 @@ def encoder_layer_plan(blk: TransformerEncoder):
                 heads=attn.num_heads, scale=attn.scaling)
 
 
-def repmixer_plan(blk: RepMixerBlock):
-    """Eval-mode RepMixerBlock folded to the es3_repmixer_bf16 taps and the two GEMMs (mobile_clip.py:594-702):
-    x1 = x + ls (BN_ms(x) + BN_mc(conv(x)) - BN_ns(x)) = sum_k wm[k] x[l+k-5] + bm,  u = BN_f(conv_f(x1)),
-    out = x1 + ls_blk (fc2(gelu(fc1(u))))."""
+def repmixer_fold(blk: RepMixerBlock):
+    """The RepMixerBlock's token mixer and ConvFFN conv with their BatchNorms' running statistics folded into es3_repmixer_bf16's
+    taps (mobile_clip.py:594-702): x1 = x + ls (BN_ms(x) + BN_mc(conv(x)) - BN_ns(x)) = sum_k wm[k] x[l+k-5] + bm,
+    u = BN_f(conv_f(x1)) = sum_k wf[k] x1[l+k-5] + bf.  Also returns the layer scales ls (token mixer) and lsb (block), fp32 [C]."""
     tm, ffn = blk.token_mixer, blk.convffn
     dim = tm.dim
     ls = _f32(tm.layer_scale).reshape(-1) if tm.use_layer_scale else torch.ones(dim, device=tm.mixer.rbr_skip.weight.device)
@@ -225,10 +226,19 @@ def repmixer_plan(blk: RepMixerBlock):
     bm = (ls * (b_ms + b_mc - b_ns)).contiguous()
     s_f, b_f = _bn(ffn.conv.bn)
     lsb = _f32(blk.layer_scale).reshape(-1) if blk.use_layer_scale else torch.ones_like(ls)
+    return dict(wm=wm.contiguous(), bm=bm, wf=_taps(ffn.conv.conv, s_f), bf=b_f.contiguous(), ls=ls.contiguous(),
+                lsb=lsb.contiguous())
+
+
+def repmixer_plan(blk: RepMixerBlock):
+    """Eval-mode RepMixerBlock: the folded taps (repmixer_fold) and the two GEMMs, out = x1 + ls_blk (fc2(gelu(fc1(u))))."""
+    ffn = blk.convffn
+    f = repmixer_fold(blk)
+    lsb = f["lsb"]
     w1 = ffn.fc1.weight.detach().reshape(ffn.fc1.out_channels, -1).to(torch.bfloat16).contiguous()
     w2 = ffn.fc2.weight.detach().reshape(ffn.fc2.out_channels, -1).to(torch.bfloat16).contiguous()
-    return dict(kind="repmixer", wm=wm.contiguous(), bm=bm, wf=_taps(ffn.conv.conv, s_f), bf=b_f.contiguous(),
-                fc1=(w1, _f32(ffn.fc1.bias)), fc2=(w2, lsb.contiguous(), (lsb * _f32(ffn.fc2.bias)).contiguous()))
+    return dict(kind="repmixer", wm=f["wm"], bm=f["bm"], wf=f["wf"], bf=f["bf"],
+                fc1=(w1, _f32(ffn.fc1.bias)), fc2=(w2, lsb, (lsb * _f32(ffn.fc2.bias)).contiguous()))
 
 
 def run_layers(layers, x, B, L, causal):
@@ -403,16 +413,21 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
 #   nn.Linear (+ GELU)                  es3_gemm_bf16_ex [+ es3_affine_act]; grads es3_wgrad_pw, column sums / es3_bn_act_bwd_*,
 #                                       es3_gemm_bf16_ex on the cached W^T (nn_utils.cached_pack, invalidated by each optimiser step)
 #   attention                           es3_attention_bf16 | es3_attention_causal_bf16 / es3_text_attn_bwd
+#   RepMixerBlock (frozen BatchNorm)    es3_repmixer_bf16 + fc1 / fc2 GEMMs; es3_repmixer_ls_bwd, es3_repmixer_ffn_bwd,
+#                                       es3_repmixer_tm_bwd (RepMixerUnit)
 def _grad_of(grads, p):
     from .efficientvit_train import _grad_of as g
     return g(grads, p)
 
 
 def check_trainable(module: nn.Module, enc: "MobileCLIPTextTransformer", what: str):
-    """The raise paths of the training graph: S0-style RepMixerBlocks, strict precision, CPU modules, dropout > 0."""
-    if any(isinstance(b, RepMixerBlock) for b in enc.transformer):
-        raise NotImplementedError(f"{what}: training is built for the TransformerEncoder (base) students; the RepMixerBlocks of "
-                                  "MobileCLIP-S0 (batch-statistics BatchNorm, 1x11 depthwise backward) are not built yet.  "
+    """The raise paths of the training graph: S0-style RepMixerBlocks with a BatchNorm in train mode, strict precision, CPU
+    modules, dropout > 0."""
+    bns = [m for b in enc.transformer if isinstance(b, RepMixerBlock) for m in b.modules() if isinstance(m, nn.BatchNorm2d)]
+    if any(m.training for m in bns):
+        raise NotImplementedError(f"{what}: the RepMixerBlocks of MobileCLIP-S0 train with frozen BatchNorm only (running "
+                                  "statistics; batch-statistics BatchNorm is not built).  To train, put every BatchNorm in .eval() "
+                                  "after .train() (set_bn_state with TRAIN.EVAL_BN_WHEN_TRAINING does); for inference, "
                                   "Call .eval() first.")
     if ops.precision() == "strict":
         raise NotImplementedError(f"{what}: the strict (fp32) precision mode is not built for the text encoders")
@@ -470,12 +485,28 @@ class _TextLinear:
         return ops.gemm(dz, self._wt(), out_dtype=out_dtype)
 
 
+class _TextConv1x1(_TextLinear):
+    """A 1x1 nn.Conv2d (ConvFFN.fc1 / fc2, weight [N, K, 1, 1]) as _TextLinear on [M, K] bf16 rows."""
+
+    def _w(self):
+        lin = self.lin
+        return cached_pack(lin, "text_w", lin.weight,
+                           lambda: lin.weight.detach().reshape(lin.out_channels, -1).to(torch.bfloat16).contiguous())
+
+    def _wt(self):
+        lin = self.lin
+        return cached_pack(lin, "text_wt", lin.weight,
+                           lambda: lin.weight.detach().reshape(lin.out_channels, -1).to(torch.bfloat16).t().contiguous())
+
+
 def _ln_params(ln):
     return ln.weight.detach().float().contiguous(), ln.bias.detach().float().contiguous(), ln.eps
 
 
 class TextEncoderLayerUnit:
     """TransformerEncoder (mobile_clip.py:469-491): x1 = x + out_proj(attn(qkv(LN1(x)))); x2 = x1 + fc2(gelu(fc1(LN2(x1))))."""
+
+    wants_bf16_grad = True      # fc2's backward takes the bf16 copy of the output gradient
 
     def __init__(self, blk: TransformerEncoder, causal: bool):
         self.n1, at, self.n2 = blk.pre_norm_mha[0], blk.pre_norm_mha[1], blk.pre_norm_ffn[0]
@@ -518,6 +549,74 @@ class TextEncoderLayerUnit:
                                      want_bf16=want_bf16)
 
 
+def _bn_rows(bn: nn.BatchNorm2d):
+    """A frozen BatchNorm2d as fp32 [4, C]: scale and shift (as folded for the forward), running mean, 1 / sqrt(running var + eps)."""
+    s, b = _bn(bn)
+    return torch.stack([s, b, _f32(bn.running_mean), torch.rsqrt(_f32(bn.running_var) + bn.eps)])
+
+
+class RepMixerUnit:
+    """RepMixerBlock (mobile_clip.py:594-702) with frozen BatchNorm (every BN in .eval(): running statistics, so the block is its
+    eval function).  Forward: es3_repmixer_bf16 on the taps folded from the current parameters (repmixer_fold, cached until the
+    next optimiser step), fc1 + GELU, fc2 x layer scale + residual.  Backward (repmixer_bwd.cu): fc2's output y is recomputed in
+    fp32 from the saved hidden h (deriving it as (x2 - x1) / ls_blk would scale x1's rounding by 1 / ls_blk, 1e5 at init);
+    es3_repmixer_ls_bwd -> fc2 / GELU / fc1 backward -> es3_repmixer_ffn_bwd -> es3_repmixer_tm_bwd.  The BatchNorms' running
+    statistics and num_batches_tracked are read, never written."""
+
+    wants_bf16_grad = False     # the backward reads the fp32 output gradient only
+
+    def __init__(self, blk: RepMixerBlock):
+        tm = blk.token_mixer
+        if not (blk.use_layer_scale and tm.use_layer_scale):
+            raise NotImplementedError("RepMixerBlock training is built for the layer-scaled block of MobileCLIP-S0")
+        self.blk, self.tm, self.ffn = blk, tm, blk.convffn
+        self.fc1, self.fc2 = _TextConv1x1(self.ffn.fc1, "gelu"), _TextConv1x1(self.ffn.fc2)
+        self.saved = None
+
+    def _pack(self):
+        blk, tm, ffn = self.blk, self.tm, self.ffn
+
+        def build():
+            p = repmixer_fold(blk)
+            one = torch.ones_like(p["ls"])
+            p["bnp"] = torch.cat([_bn_rows(tm.mixer.rbr_skip), _bn_rows(tm.mixer.rbr_conv[0].bn), _bn_rows(tm.norm.rbr_skip),
+                                  p["ls"].view(1, -1)]).contiguous()
+            p["bnf"] = _bn_rows(ffn.conv.bn).contiguous()
+            p["tm_taps"], p["f_taps"] = _taps(tm.mixer.rbr_conv[0].conv, one), _taps(ffn.conv.conv, one)
+            p["b2"] = _f32(ffn.fc2.bias)
+            p["b2s"] = (p["lsb"] * p["b2"]).contiguous()
+            return p
+        return cached_pack(blk, "train_fold", blk.layer_scale, build)
+
+    def forward(self, x, B, L):
+        p = self._pack()
+        x1, u = ops.repmixer(x, B, L, p["wm"], p["bm"], p["wf"], p["bf"])
+        h = self.fc1.forward(u)
+        x2 = ops.gemm(h, self.fc2._w(), scale=p["lsb"], bias=p["b2s"], residual=x1, out_dtype=torch.float32)
+        self.saved = (x, x1, h, p, B, L)
+        return x2
+
+    def backward(self, g, gb, grads, want_bf16=True):
+        """g: fp32 gradient of the block output (gb, its bf16 copy, is not needed) -> (fp32 input gradient, bf16 copy | None)."""
+        x, x1, h, p, B, L = self.saved
+        self.saved = None
+        tm, ffn = self.tm, self.ffn
+        y = ops.gemm(h, self.fc2._w(), bias=p["b2"], out_dtype=torch.float32)
+        dy = ops.repmixer_ls_bwd(g, y, p["lsb"], B, L, dls=_grad_of(grads, self.blk.layer_scale),
+                                 dbias=_grad_of(grads, ffn.fc2.bias))
+        gw2 = _grad_of(grads, ffn.fc2.weight)
+        if gw2 is not None:
+            ops.wgrad_pw(dy, h, gw2)
+        du = self.fc1.backward(ops.gemm(dy, self.fc2._wt()), grads, out_dtype=torch.float32)
+        bnf = ffn.conv.bn
+        e = ops.repmixer_ffn_bwd(x1, du, g, p["f_taps"], p["bnf"], B, L, dtaps=_grad_of(grads, ffn.conv.conv.weight),
+                                 dgamma=_grad_of(grads, bnf.weight), dbeta=_grad_of(grads, bnf.bias))
+        bns = (tm.mixer.rbr_skip, tm.mixer.rbr_conv[0].bn, tm.norm.rbr_skip)
+        return ops.repmixer_tm_bwd(x, e, p["tm_taps"], p["bnp"], B, L, dtaps=_grad_of(grads, tm.mixer.rbr_conv[0].conv.weight),
+                                   dls=_grad_of(grads, tm.layer_scale),
+                                   dbn=[_grad_of(grads, t) for bn in bns for t in (bn.weight, bn.bias)], want_bf16=want_bf16)
+
+
 class TextEmbedUnit:
     """forward_embedding (mobile_clip.py:815-823): table[ids] + the positional table, resized N -> L when they differ."""
 
@@ -556,12 +655,14 @@ class TextEmbedUnit:
 
 
 class TextStudentTrainGraph:
-    """TextStudentEncoder in train mode: embed -> TransformerEncoder layers -> final LayerNorm -> projector (fp32 memory)."""
+    """TextStudentEncoder in train mode: embed -> TransformerEncoder layers (and MobileCLIP-S0's RepMixerBlocks, frozen BN) ->
+    final LayerNorm -> projector (fp32 memory)."""
 
     def __init__(self, student):
         enc = student.encoder
         self.embed = TextEmbedUnit(enc)
-        self.layers = [TextEncoderLayerUnit(b, enc.causal_masking) for b in enc.transformer]
+        self.layers = [RepMixerUnit(b) if isinstance(b, RepMixerBlock) else TextEncoderLayerUnit(b, enc.causal_masking)
+                       for b in enc.transformer]
         self.fln = enc.final_layer_norm
         self.proj = _TextLinear(student.projector)
         self.saved = None
@@ -584,7 +685,7 @@ class TextStudentTrainGraph:
         dy = self.proj.backward(ops.cast_f32_to_bf16(dmem), grads, dy_f32=dmem, out_dtype=torch.float32)
         w, _, eps = _ln_params(self.fln)
         g, gb = ops.layernorm_bwd_f32(xs, dy, w, eps, _grad_of(grads, self.fln.weight), _grad_of(grads, self.fln.bias),
-                                      want_bf16=bool(self.layers))
+                                      want_bf16=bool(self.layers) and self.layers[-1].wants_bf16_grad)
         for i in range(len(self.layers) - 1, -1, -1):
-            g, gb = self.layers[i].backward(g, gb, grads, want_bf16=i > 0)
+            g, gb = self.layers[i].backward(g, gb, grads, want_bf16=i > 0 and self.layers[i - 1].wants_bf16_grad)
         self.embed.backward(g, grads)

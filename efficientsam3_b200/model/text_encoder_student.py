@@ -6,9 +6,9 @@ fp32 = token + positional embedding), the reference's sequence-first layout as t
 in attention, as in the reference (no key_padding_mask is passed), so a caption's output depends on the context length
 but not on the other captions of the batch.
 
-Train mode (base students: every TransformerEncoder trunk, i.e. all builder names but MobileCLIP-S0) with grad enabled records the
-forward as ONE autograd node (TextStudentTrainFunction) whose backward runs the native kernels (backbones/mobile_clip.py
-TextStudentTrainGraph).  `encoder.projection_layer` is not used here (the reference calls the encoder with return_all_tokens=True):
+Train mode (base students: every TransformerEncoder trunk; MobileCLIP-S0 once every BatchNorm of its RepMixerBlocks is in .eval(),
+i.e. frozen BN as set_bn_state / TRAIN.EVAL_BN_WHEN_TRAINING leaves it) with grad enabled records the forward as ONE autograd
+node (TextStudentTrainFunction) whose backward runs the native kernels (backbones/mobile_clip.py TextStudentTrainGraph).  `encoder.projection_layer` is not used here (the reference calls the encoder with return_all_tokens=True):
 it gets no gradient, so optimisers skip it (build stage1.optim.FlatAdamW with exclude=TextStudentEncoder.UNUSED_PARAMETERS).
 A train-mode module under torch.no_grad() runs the eval path: the base students have no train-time behaviour besides gradients.
 """

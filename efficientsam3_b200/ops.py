@@ -539,6 +539,80 @@ def repmixer(x, B, L, wm, bm, wf, bf):
     return x1, u
 
 
+# ------------------------------------------------------------------------------------ RepMixerBlock backward (repmixer_bwd.cu)
+KERNELS_PER_CALL.update({"es3_repmixer_ls_bwd": 2, "es3_repmixer_ffn_bwd": 2, "es3_repmixer_tm_bwd": 2})
+
+
+def _repmixer_bwd_args(name, rows, B, L, params):
+    """Host-side checks of the RepMixerBlock backward (before any launch): rows [B*L, C] fp32, 1 <= L <= 128, C % 32 == 0;
+    params: (tensor, shape) pairs of fp32 contiguous per-channel tensors.  Returns C."""
+    if not 1 <= L <= REPMIXER_MAX_L:
+        raise ValueError(f"{name}: the RepMixerBlock backward keeps a sequence in shared memory and takes 1..{REPMIXER_MAX_L} "
+                         f"tokens, got {L}")
+    C = rows[0].shape[-1]
+    if B < 1 or C < 32 or C % 32:
+        raise ValueError(f"{name}: needs B >= 1 and a channel count that is a multiple of 32 (B={B}, C={C})")
+    for t in rows:
+        _chk(t, torch.float32, name)
+        if not (t.is_contiguous() and tuple(t.shape) == (B * L, C)):
+            raise ValueError(f"{name}: expected contiguous fp32 rows [{B * L}, {C}], got {tuple(t.shape)}")
+    for t, shape in params:
+        _chk(t, torch.float32, name)
+        if not (t.is_contiguous() and tuple(t.shape) == shape):
+            raise ValueError(f"{name}: expected a contiguous fp32 {shape}, got {tuple(t.shape)}")
+    _ensure_init(rows[0])
+    return C
+
+
+def _grad_dst(t, numel, name):
+    if t is None:
+        return 0
+    _chk(t, torch.float32, name)
+    if not (t.is_contiguous() and t.numel() == numel):
+        raise ValueError(f"{name}: expected a contiguous fp32 gradient of {numel} elements, got {tuple(t.shape)}")
+    return t.data_ptr()
+
+
+def repmixer_ls_bwd(g, y, ls, B, L, dls=None, dbias=None):
+    """Layer scale x2 = x1 + ls * y: g, y [B*L, C] fp32, ls [C] -> dy = ls g in bf16; dls [C(,1,1)] += sum g y,
+    dbias [C] += sum ls g (fc2's bias)."""
+    C = _repmixer_bwd_args("repmixer_ls_bwd", (g, y), B, L, ((ls, (g.shape[-1],)),))
+    pl, pb = _grad_dst(dls, C, "dls"), _grad_dst(dbias, C, "dbias")
+    dy = torch.empty((B * L, C), device=g.device, dtype=torch.bfloat16)
+    ws = _f32ws(_lib.size("es3_repmixer_bwd_ws_floats", B, C), g.device)
+    _call("es3_repmixer_ls_bwd", "repmixer_ls_bwd", _nb(g, y, dy), 3 * g.numel(), g.data_ptr(), y.data_ptr(), ls.data_ptr(),
+          dy.data_ptr(), ws.data_ptr(), pl, pb, B, L, C, _stream())
+    return dy
+
+
+def repmixer_ffn_bwd(x1, du, g, taps, bnf, B, L, dtaps=None, dgamma=None, dbeta=None):
+    """ConvFFN.conv + BN_f backward: x1, du, g [B*L, C] fp32; taps [11, C] (raw), bnf [4, C] = (scale, shift, running mean,
+    1/sqrt(running var + eps)).  Returns e = g + dw^T(scale du) fp32; dtaps [C,1,1,11], dgamma, dbeta [C] accumulated."""
+    C = x1.shape[-1]
+    _repmixer_bwd_args("repmixer_ffn_bwd", (x1, du, g), B, L, ((taps, (11, C)), (bnf, (4, C))))
+    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dgamma, C, "dgamma"), _grad_dst(dbeta, C, "dbeta")]
+    e = torch.empty_like(x1)
+    ws = _f32ws(_lib.size("es3_repmixer_bwd_ws_floats", B, C), x1.device)
+    _call("es3_repmixer_ffn_bwd", "repmixer_ffn_bwd", _nb(x1, du, g, e), 6 * 11 * x1.numel(), x1.data_ptr(), du.data_ptr(),
+          g.data_ptr(), taps.data_ptr(), bnf.data_ptr(), e.data_ptr(), ws.data_ptr(), *ptrs, B, L, C, _stream())
+    return e
+
+
+def repmixer_tm_bwd(x, e, taps, bnp, B, L, dtaps=None, dls=None, dbn=(None,) * 6, want_bf16=False):
+    """RepMixer token mixer backward: x, e [B*L, C] fp32; taps [11, C] (raw mixer.rbr_conv.0.conv), bnp [13, C] = the (scale,
+    shift, running mean, invstd) rows of mixer.rbr_skip, mixer.rbr_conv.0.bn, norm.rbr_skip, then the layer scale.  Returns
+    (dx fp32, bf16 copy | None); dtaps [C,1,1,11], dls [C,1,1] and dbn = (dgamma, dbeta) x (ms, mc, ns) accumulated."""
+    C = x.shape[-1]
+    _repmixer_bwd_args("repmixer_tm_bwd", (x, e), B, L, ((taps, (11, C)), (bnp, (13, C))))
+    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dls, C, "dls")] + [_grad_dst(t, C, "dbn") for t in dbn]
+    dx = torch.empty_like(x)
+    dxb = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
+    ws = _f32ws(_lib.size("es3_repmixer_bwd_ws_floats", B, C), x.device)
+    _call("es3_repmixer_tm_bwd", "repmixer_tm_bwd", _nb(x, e, dx, dxb), 8 * 11 * x.numel(), x.data_ptr(), e.data_ptr(),
+          taps.data_ptr(), bnp.data_ptr(), dx.data_ptr(), _ptr(dxb), ws.data_ptr(), *ptrs, B, L, C, _stream())
+    return dx, dxb
+
+
 # ------------------------------------------------------------------------------------ text-student backward (text_bwd.cu)
 TEXT_ATTN_BWD_MAX_L = 128
 KERNELS_PER_CALL.update({"es3_layernorm_bwd_f32": 2, "es3_text_kd_loss_fwd": 2, "es3_text_consistency_fwd": 2,

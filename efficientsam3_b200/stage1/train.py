@@ -95,9 +95,14 @@ def train_text_one_epoch(config, model, data_loader, optimizer, epoch, lr_at=Non
     stage1.optim.FlatAdamW over `model` (build it with exclude=TextStudentEncoder.UNUSED_PARAMETERS, as the reference's AdamW
     never sees a gradient for encoder.projection_layer).  Reads DISTILL.NUM_EMBED / EMBED_DIM (the stored embeddings' shape),
     MASK_PAD_TOKENS, COSINE and CONSISTENCY_LOSS; TRAIN.ACCUMULATION_STEPS / CLIP_GRAD and the cosine schedule as
-    train_one_epoch does.  Returns the list of per-iteration losses (device scalars)."""
+    train_one_epoch does.  With TRAIN.EVAL_BN_WHEN_TRAINING (read with a default of False) every BatchNorm goes back to eval mode
+    after model.train(), as set_bn_state does: MobileCLIP-S0 trains natively only with frozen BatchNorm.  The reference's text
+    trainer leaves that call commented out (train_text_encoder_stage1.py:173); its text configs all set the key False.
+    Returns the list of per-iteration losses (device scalars)."""
     from .losses import text_kd_train_step
     model.train()
+    if getattr(config.TRAIN, "EVAL_BN_WHEN_TRAINING", False):
+        set_bn_state(config, model)
     optimizer.zero_grad()
     num_steps = len(data_loader)
     accum = int(config.TRAIN.ACCUMULATION_STEPS)

@@ -240,6 +240,24 @@ int es3_text_consistency_bwd(const float* mdiff, int B, int L, int D, float weig
                              const float* gout, float* dp, float* dq, void* stream);
 int es3_cast_f32_to_bf16(const float* x, void* y, long long n, void* stream);
 
+/* Backward of MobileCLIP-S0's RepMixerBlock with frozen BatchNorm (repmixer_bwd.cu), 1 <= L <= 128, C % 32 == 0; one CTA per
+ * (sequence, 32 channels).  Rows are [B*L, C] fp32; taps [11][C] fp32 tap-major (the raw depthwise weights); per-CTA partials go
+ * to ws (es3_repmixer_bwd_ws_floats(B, C)) and are summed over the sequences in order, then added (+=) into the gradients in torch
+ * layouts (taps [C,1,1,11], layer scales [C,1,1], gamma / beta [C]); a null gradient pointer is skipped.
+ * es3_repmixer_ls_bwd: dy = bf16(ls g); dls += sum g y; dbias += sum ls g.
+ * es3_repmixer_ffn_bwd: ConvFFN.conv + BN_f, bnf [4][C] = (s, b, rm, invstd): e = g + dw^T(s du; wf); dwf, dgamma, dbeta.
+ * es3_repmixer_tm_bwd: the token mixer, bnp [13][C] = (s, b, rm, invstd) of mixer.rbr_skip, mixer.rbr_conv.0.bn, norm.rbr_skip,
+ * then the layer scale: dx = e + (s_ms - s_ns) ls e + dw^T(s_mc ls e; wmc) in fp32 (+ bf16 copy dxb); the taps, the layer scale
+ * and the three BNs' gamma / beta. */
+long long es3_repmixer_bwd_ws_floats(int B, int C);
+int es3_repmixer_ls_bwd(const float* g, const float* y, const float* ls, void* dy, float* ws, float* dls, float* dbias, int B, int L,
+                        int C, void* stream);
+int es3_repmixer_ffn_bwd(const float* x1, const float* du, const float* g, const float* wf, const float* bnf, float* e, float* ws,
+                         float* dwf, float* dgamma, float* dbeta, int B, int L, int C, void* stream);
+int es3_repmixer_tm_bwd(const float* x, const float* e, const float* wmc, const float* bnp, float* dx, void* dxb, float* ws, float* dwmc,
+                        float* dls, float* dg_ms, float* db_ms, float* dg_mc, float* db_mc, float* dg_ns, float* db_ns, int B, int L,
+                        int C, void* stream);
+
 /* ------------------------------------------------------------------------------------------ SAM heads */
 /* PositionEmbeddingRandom over an h x w grid -> [h*w, 2F] fp32 (PromptEncoder.get_dense_pe, prompt_encoder.py:61-69). */
 int es3_dense_pe(const float* gauss, int F, int h, int w, float* out, void* stream);

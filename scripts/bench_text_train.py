@@ -4,14 +4,15 @@ reference trains (fp16 autocast, torch.amp.GradScaler, torch.optim.AdamW) and on
 
     python scripts/bench_text_train.py [--steps 20] [--warmup 5]
 
-One timed iteration is the configured one of the text_{s1,l}_ctx{16,32} configs (their es_mc_m / es_mc_l bases set
+One timed iteration is the configured one of the text_{s1,l,s0}_ctx{16,32} configs (their es_mc_m / es_mc_l bases set
 MASK_PAD_TOKENS True, COSINE 2.0, CONSISTENCY_LOSS 0.05): captions -> tokenise -> forward -> masked text MSE + 2.0 * cosine ->
 the consistency block twice (permute_words, tokenise, a second and a third forward, mse of the L-means) -> backward through all
 three forwards -> global-norm clip 5.0 -> AdamW.  Both arms tokenise on the host inside the timed region.  The median and the
 10th / 90th percentiles of `--steps` per-iteration CUDA-event times after `--warmup` iterations are reported.  Captions are
 seeded word sequences (3-14 words) over the words of the test strings, tokenised with the CLIP merge subset the tests rebuild
 (tests/golden/text_bpe_subset.json); teacher embeddings are seeded random fp16 values upcast to fp32, as stored.
-Algorithmic FLOPs per step (train_flops): three forwards (oracle.text.flops_mobileclip) and three backwards, each GEMM's backward
+MobileCLIP-S0 runs with every BatchNorm frozen in .eval() (TRAIN.EVAL_BN_WHEN_TRAINING: running statistics, as the oracle's BN
+in both eager arms).  Algorithmic FLOPs per step (train_flops): three forwards (oracle.text.flops_mobileclip) and three backwards, each GEMM's backward
 2x its forward, the attention backward 10 B L^2 C per layer (S recomputed, dP, dV, dQ, dK) against the forward's 4 B L^2 C.
 """
 from __future__ import annotations
@@ -70,11 +71,13 @@ def per_step_ms(fn, steps, warmup):
     return statistics.median(times), q[0], q[-1]
 
 
-def eager_arm(sd_dev, tok, ctx, caps, teacher, cfg, amp):
-    """The oracle graph trained as the reference's loop does (train_text_encoder_stage1.py:221-288), consistency block twice."""
+def eager_arm(sd_dev, tok, ctx, caps, teacher, cfg, amp, trainable=None):
+    """The oracle graph trained as the reference's loop does (train_text_encoder_stage1.py:221-288), consistency block twice.
+    trainable: the parameter names (default: every state_dict entry; BatchNorm buffers are not parameters)."""
     from efficientsam3_b200.stage1.losses import permute_words
     from oracle import text as OT
-    params = {k: v.clone().requires_grad_(True) for k, v in sd_dev.items() if k != "encoder.projection_layer"}
+    params = {k: v.clone().requires_grad_(True) for k, v in sd_dev.items()
+              if k != "encoder.projection_layer" and (trainable is None or k in trainable)}
     sd = dict(sd_dev, **params)
     opt = torch.optim.AdamW(list(params.values()), lr=1e-4, weight_decay=0.05)
     scaler = torch.amp.GradScaler("cuda", enabled=amp)
@@ -126,17 +129,25 @@ def main():
                loss=dict(mask_pad_tokens=True, cosine=COSINE, consistency=CONSISTENCY))
     for tag, backbone, B, L in (("mobileclip_s1_b64_ctx32", "MobileCLIP-S1", 64, 32), ("mobileclip_s1_b64_ctx16", "MobileCLIP-S1", 64, 16),
                                 ("mobileclip2_l_b32_ctx32", "MobileCLIP2-L", 32, 32), ("mobileclip2_l_b32_ctx16", "MobileCLIP2-L", 32, 16),
-                                ("mobileclip_b_b64_ctx32", "MobileCLIP-B", 64, 32)):
+                                ("mobileclip_b_b64_ctx32", "MobileCLIP-B", 64, 32),
+                                ("mobileclip_s0_b64_ctx32", "MobileCLIP-S0", 64, 32), ("mobileclip_s0_b64_ctx16", "MobileCLIP-S0", 64, 16)):
         m = build_text_student_model(NS(MODEL=NS(BACKBONE=backbone, BPE_PATH=BPE), DISTILL=NS(EMBED_DIM=256, CONTEXT_LENGTH=L)))
         sd = fill_state_dict(m.state_dict(), 1)
         m.load_state_dict(sd)
         m = m.to(dev).train()
+        enc = m.encoder
+        mct = enc.transformer[0].__class__.__name__ == "RepMixerBlock"
+        if mct:       # S0 trains with frozen BatchNorm (TRAIN.EVAL_BN_WHEN_TRAINING); the oracle's BN uses running statistics too
+            for mod in m.modules():
+                if isinstance(mod, torch.nn.modules.batchnorm._BatchNorm):
+                    mod.eval()
         caps = captions(B, 0)
         teacher = (torch.randn(B, L, 256, generator=torch.Generator().manual_seed(2)) * 0.5).half().float().to(dev)
         opt = FlatAdamW(m, lr=1e-4, weight_decay=0.05, exclude=TextStudentEncoder.UNUSED_PARAMETERS)
-        enc = m.encoder
-        cfg = dict(causal_masking=enc.causal_masking, model_name="base", n_transformer_layers=len(enc.transformer),
-                   n_heads_per_layer=enc.transformer[0].pre_norm_mha[1].num_heads, dim=enc.model_dim, ffn_multiplier_per_layer=4.0)
+        cfg = dict(causal_masking=enc.causal_masking, model_name="mct" if mct else "base",
+                   n_transformer_layers=len(enc.transformer) - (2 if mct else 0),
+                   n_heads_per_layer=enc.transformer[1 if mct else 0].pre_norm_mha[1].num_heads, dim=enc.model_dim,
+                   ffn_multiplier_per_layer=4.0)
         random.seed(0)
 
         def native():
@@ -149,11 +160,14 @@ def main():
         launches = ops.launch_count - n0
         ms, ms_lo, ms_hi = per_step_ms(native, args.steps, args.warmup)
         sd_dev = {k: v.to(dev) for k, v in sd.items()}
-        ms16, ms16_lo, ms16_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, True), args.steps, args.warmup)
-        ms32, ms32_lo, ms32_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, False), args.steps, args.warmup)
+        names = {n for n, _ in m.named_parameters()}
+        ms16, ms16_lo, ms16_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, True, names), args.steps,
+                                             args.warmup)
+        ms32, ms32_lo, ms32_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, False, names), args.steps,
+                                             args.warmup)
         flops = train_flops(cfg, B, L, 256)
         r3 = lambda *v: [round(x, 3) for x in v]  # noqa: E731
-        res[tag] = dict(batch=B, ctx=L, native_ms=round(ms, 3), native_p10_p90_ms=r3(ms_lo, ms_hi), launches_per_step=launches,
+        res[tag] = dict(batch=B, ctx=L, **(dict(frozen_bn=True) if mct else {}), native_ms=round(ms, 3), native_p10_p90_ms=r3(ms_lo, ms_hi), launches_per_step=launches,
                         gflop_per_step=round(flops / 1e9, 1), native_tflops=round(flops / ms / 1e9, 2),
                         eager_fp16_autocast_ms=round(ms16, 3), eager_fp16_autocast_p10_p90_ms=r3(ms16_lo, ms16_hi),
                         eager_fp32_ms=round(ms32, 3), eager_fp32_p10_p90_ms=r3(ms32_lo, ms32_hi),

@@ -44,6 +44,10 @@ SIGNATURES: dict[str, list] = {
     "es3_repmixer_ls_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp],
     "es3_repmixer_ffn_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp],
     "es3_repmixer_tm_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp],
+    # MobileCLIP-S0 RepMixerBlock with batch-statistics BatchNorm (repmixer_bn_train.cu)
+    "es3_repmixer_bn_fwd": [_vp] * 17 + [_f] * 8 + [_vp] * 3 + [_i, _i, _i, _vp],
+    "es3_repmixer_bn_ffn_bwd": [_vp] * 11 + [_i, _i, _i, _vp],
+    "es3_repmixer_bn_tm_bwd": [_vp] * 16 + [_i, _i, _i, _vp],
     "es3_tokens_f32_to_nchw": [_vp, _vp, _i, _i, _i, _vp],
     "es3_cast_f32_to_f16": [_vp, _vp, _ll, _vp],
     "es3_convt2x2_bf16": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp],
@@ -139,6 +143,7 @@ SIZE_HELPERS: dict[str, list] = {
     "es3_layernorm_bwd_ws_floats": [_ll, _i],
     "es3_layernorm_bwd_f32_ws_floats": [_ll, _i],
     "es3_repmixer_bwd_ws_floats": [_i, _i],
+    "es3_repmixer_bn_ws_floats": [_i, _i],
     "es3_colsum_f32_ws_floats": [_ll, _i],
     "es3_wgrad_tc_ws_floats": [_ll, _i, _i],
     "es3_litemla_attn_f32_ws_floats": [_i, _i, _i, _i],

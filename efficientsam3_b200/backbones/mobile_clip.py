@@ -4,7 +4,8 @@ same class names, constructor arguments and state_dict keys (`embedding_layer.we
 `transformer.N.pre_norm_ffn.{0,1,4}.*`, the RepMixerBlock's `token_mixer.{norm,mixer}.*`, `convffn.*`, `layer_scale`,
 `final_layer_norm.*`, `projection_layer`).  The nn modules are parameter containers.  Eval-mode forward for every student;
 train-mode forward + backward for the base (TransformerEncoder-only) students and for MobileCLIP-S0 with its RepMixerBlocks'
-BatchNorms frozen in .eval(): TextStudentTrainGraph at the end of this file.
+BatchNorms frozen in .eval() or, after enable_batch_stat_bn(), in train mode (batch statistics): TextStudentTrainGraph at the end of
+this file.
 
 Device path (all libes3.so; fp32 residual stream, bf16 GEMM operands, fp32 accumulation / LayerNorm / softmax):
   embedding gather + positional add                      es3_text_embed
@@ -241,12 +242,53 @@ def repmixer_plan(blk: RepMixerBlock):
                 fc1=(w1, _f32(ffn.fc1.bias)), fc2=(w2, lsb, (lsb * _f32(ffn.fc2.bias)).contiguous()))
 
 
-def run_layers(layers, x, B, L, causal):
-    """The residual trunk on x [B*L, C] fp32 (not modified) -> fp32 [B*L, C]."""
+def repmixer_bns(blk: RepMixerBlock):
+    """The block's four BatchNorms in the kernels' order: BN_ms (mixer.rbr_skip), BN_mc (mixer.rbr_conv.0.bn), BN_ns
+    (norm.rbr_skip), BN_f (convffn.conv.bn)."""
+    tm = blk.token_mixer
+    return (tm.mixer.rbr_skip, tm.mixer.rbr_conv[0].bn, tm.norm.rbr_skip, blk.convffn.conv.bn)
+
+
+def repmixer_bn_pack(blk: RepMixerBlock):
+    """The parameters es3_repmixer_bn_* read, cached until the next optimiser step: taps [2, 11, C] (raw w_mc, w_f), aff [9, C]
+    (ls_tm, then gamma / beta of repmixer_bns), and fc2's layer scale / bias.  No running statistics: they change every forward."""
+    tm, ffn = blk.token_mixer, blk.convffn
+
+    def build():
+        one = torch.ones(tm.dim, device=blk.layer_scale.device)
+        aff = [_f32(tm.layer_scale).reshape(-1)] + [_f32(t) for bn in repmixer_bns(blk) for t in (bn.weight, bn.bias)]
+        lsb, b2 = _f32(blk.layer_scale).reshape(-1), _f32(ffn.fc2.bias)
+        return dict(taps=torch.stack([_taps(tm.mixer.rbr_conv[0].conv, one), _taps(ffn.conv.conv, one)]).contiguous(),
+                    aff=torch.stack(aff).contiguous(), lsb=lsb.contiguous(), b2=b2, b2s=(lsb * b2).contiguous())
+    return cached_pack(blk, "bn_train", blk.layer_scale, build)
+
+
+def repmixer_bn_forward(blk: RepMixerBlock, x, B, L):
+    """The block's prologue with batch-statistics BatchNorm (updates its running buffers): (x1 fp32, u bf16, stats [8, C], pack)."""
+    p = repmixer_bn_pack(blk)
+    x1, u, _, stats = ops.repmixer_bn_fwd(x, B, L, p["taps"], p["aff"], repmixer_bns(blk))
+    return x1, u, stats, p
+
+
+def invalidate_running_folds(enc: "MobileCLIPTextTransformer"):
+    """Drop every cached fold of the RepMixerBlocks' running statistics (the eval plan and RepMixerUnit's train_fold).  The
+    batch-statistics kernels write the running buffers in place, which torch's _version does not see."""
+    enc._plan_key = None
+    for b in enc.transformer:
+        if isinstance(b, RepMixerBlock):
+            b.__dict__.get("_es3_pack_cache", {}).pop("train_fold", None)
+
+
+def run_layers(layers, x, B, L, causal, bn_blocks=None):
+    """The residual trunk on x [B*L, C] fp32 (not modified) -> fp32 [B*L, C].  bn_blocks: the trunk's modules when the
+    RepMixerBlocks normalise with batch statistics (their running buffers are updated), else None."""
     C = x.shape[1]
-    for lp in layers:
+    for i, lp in enumerate(layers):
         if lp["kind"] == "repmixer":
-            x1, u = ops.repmixer(x, B, L, lp["wm"], lp["bm"], lp["wf"], lp["bf"])
+            if bn_blocks is not None:
+                x1, u, _, _ = repmixer_bn_forward(bn_blocks[i], x, B, L)
+            else:
+                x1, u = ops.repmixer(x, B, L, lp["wm"], lp["bm"], lp["wf"], lp["bf"])
             h = ops.gemm(u, lp["fc1"][0], bias=lp["fc1"][1], act="gelu")
             w2, s2, b2 = lp["fc2"]
             x = ops.gemm(h, w2, scale=s2, bias=b2, residual=x1, out_dtype=torch.float32)
@@ -322,6 +364,14 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
         nn.init.normal_(self.projection_layer, std=model_dim ** -0.5)
         self.model_dim = model_dim
         self.causal_masking = cfg["causal_masking"]
+        # train-mode RepMixerBlock BatchNorms normalise with batch statistics (TextStudentEncoder.enable_batch_stat_bn); not state
+        self.batch_stat_bn = False
+
+    def batch_stat_active(self) -> bool:
+        """True when the RepMixerBlocks' BatchNorms are in train mode and batch statistics were asked for (check_trainable
+        rejects a mixed train / eval state before this is consulted)."""
+        return self.batch_stat_bn and any(m.training for b in self.transformer if isinstance(b, RepMixerBlock)
+                                          for m in repmixer_bns(b))
 
     def resize_pos_embed(self, new_length: int):
         """mobile_clip.py:709-724: truncates the table (a new Parameter) when new_length is shorter; never grows it."""
@@ -374,7 +424,10 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
             raise ValueError(f"expected CUDA fp32 embeddings [B, L, {self.model_dim}]; the native path has no CPU fallback")
         B, L, C = x.shape
         p = self._plan()
-        xs = run_layers(p["layers"], x.reshape(B * L, C).contiguous(), B, L, self.causal_masking)
+        bn_blocks = list(self.transformer) if self.batch_stat_active() else None
+        xs = run_layers(p["layers"], x.reshape(B * L, C).contiguous(), B, L, self.causal_masking, bn_blocks)
+        if bn_blocks is not None:
+            invalidate_running_folds(self)
         yb, yf = ops.layernorm(xs, *p["ln"], out_bf16=True, out_f32=True)
         return yf, yb
 
@@ -415,20 +468,33 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
 #   attention                           es3_attention_bf16 | es3_attention_causal_bf16 / es3_text_attn_bwd
 #   RepMixerBlock (frozen BatchNorm)    es3_repmixer_bf16 + fc1 / fc2 GEMMs; es3_repmixer_ls_bwd, es3_repmixer_ffn_bwd,
 #                                       es3_repmixer_tm_bwd (RepMixerUnit)
+#   RepMixerBlock (batch-statistics BN) es3_repmixer_bn_fwd + fc1 / fc2 GEMMs; es3_repmixer_ls_bwd, es3_repmixer_bn_ffn_bwd,
+#                                       es3_repmixer_bn_tm_bwd (RepMixerBatchStatUnit)
 def _grad_of(grads, p):
     from .efficientvit_train import _grad_of as g
     return g(grads, p)
 
 
 def check_trainable(module: nn.Module, enc: "MobileCLIPTextTransformer", what: str):
-    """The raise paths of the training graph: S0-style RepMixerBlocks with a BatchNorm in train mode, strict precision, CPU
-    modules, dropout > 0."""
+    """The raise paths of the training graph: S0-style RepMixerBlocks with a BatchNorm in train mode unless batch statistics were
+    enabled (then: a mixed train / eval state, momentum=None, track_running_stats=False), strict precision, CPU modules,
+    dropout > 0."""
     bns = [m for b in enc.transformer if isinstance(b, RepMixerBlock) for m in b.modules() if isinstance(m, nn.BatchNorm2d)]
     if any(m.training for m in bns):
-        raise NotImplementedError(f"{what}: the RepMixerBlocks of MobileCLIP-S0 train with frozen BatchNorm only (running "
-                                  "statistics; batch-statistics BatchNorm is not built).  To train, put every BatchNorm in .eval() "
-                                  "after .train() (set_bn_state with TRAIN.EVAL_BN_WHEN_TRAINING does); for inference, "
-                                  "Call .eval() first.")
+        if not enc.batch_stat_bn:
+            raise NotImplementedError(f"{what}: the RepMixerBlocks of MobileCLIP-S0 train with frozen BatchNorm (running "
+                                      "statistics) unless batch statistics are enabled.  To train, put every BatchNorm in .eval() "
+                                      "after .train() (set_bn_state with TRAIN.EVAL_BN_WHEN_TRAINING does) or call "
+                                      "enable_batch_stat_bn() to normalise with batch statistics; for inference, Call .eval() first.")
+        if not all(m.training for m in bns):
+            raise NotImplementedError(f"{what}: batch-statistics BatchNorm needs every BatchNorm of the RepMixerBlocks in train mode; "
+                                      "a mixed train / eval state is not built (set_bn_state freezes all of them)")
+        for m in bns:
+            if m.momentum is None:
+                raise NotImplementedError(f"{what}: BatchNorm momentum=None (a cumulative moving average) is not built for "
+                                          "batch-statistics BatchNorm")
+            if not m.track_running_stats or m.running_mean is None:
+                raise NotImplementedError(f"{what}: batch-statistics BatchNorm is built with track_running_stats=True only")
     if ops.precision() == "strict":
         raise NotImplementedError(f"{what}: the strict (fp32) precision mode is not built for the text encoders")
     for m in module.modules():
@@ -617,6 +683,45 @@ class RepMixerUnit:
                                    dbn=[_grad_of(grads, t) for bn in bns for t in (bn.weight, bn.bias)], want_bf16=want_bf16)
 
 
+class RepMixerBatchStatUnit(RepMixerUnit):
+    """RepMixerBlock with every BatchNorm in train mode (batch statistics, as nn.BatchNorm2d trains; enable_batch_stat_bn).
+    Forward: es3_repmixer_bn_fwd (statistics over the B*L tokens, running buffers and num_batches_tracked updated on the device,
+    taps folded on the device, then es3_repmixer_bf16), fc1 + GELU, fc2 x layer scale + residual; the batch statistics are kept
+    for the backward.  Backward: as RepMixerUnit, with es3_repmixer_bn_ffn_bwd / es3_repmixer_bn_tm_bwd, which add the two
+    mean terms of the BatchNorm input gradient."""
+
+    def __init__(self, blk: RepMixerBlock, enc: "MobileCLIPTextTransformer"):
+        super().__init__(blk)
+        self.enc = enc
+
+    def forward(self, x, B, L):
+        x1, u, stats, p = repmixer_bn_forward(self.blk, x, B, L)
+        invalidate_running_folds(self.enc)
+        h = self.fc1.forward(u)
+        x2 = ops.gemm(h, self.fc2._w(), scale=p["lsb"], bias=p["b2s"], residual=x1, out_dtype=torch.float32)
+        self.saved = (x, x1, h, p, stats, B, L)
+        return x2
+
+    def backward(self, g, gb, grads, want_bf16=True):
+        x, x1, h, p, stats, B, L = self.saved
+        self.saved = None
+        tm, ffn = self.tm, self.ffn
+        y = ops.gemm(h, self.fc2._w(), bias=p["b2"], out_dtype=torch.float32)
+        dy = ops.repmixer_ls_bwd(g, y, p["lsb"], B, L, dls=_grad_of(grads, self.blk.layer_scale),
+                                 dbias=_grad_of(grads, ffn.fc2.bias))
+        gw2 = _grad_of(grads, ffn.fc2.weight)
+        if gw2 is not None:
+            ops.wgrad_pw(dy, h, gw2)
+        du = self.fc1.backward(ops.gemm(dy, self.fc2._wt()), grads, out_dtype=torch.float32)
+        bnf = ffn.conv.bn
+        e = ops.repmixer_bn_ffn_bwd(x1, du, g, p["taps"], p["aff"], stats, B, L, dtaps=_grad_of(grads, ffn.conv.conv.weight),
+                                    dgamma=_grad_of(grads, bnf.weight), dbeta=_grad_of(grads, bnf.bias))
+        bns = repmixer_bns(self.blk)[:3]
+        return ops.repmixer_bn_tm_bwd(x, e, p["taps"], p["aff"], stats, B, L,
+                                      dtaps=_grad_of(grads, tm.mixer.rbr_conv[0].conv.weight), dls=_grad_of(grads, tm.layer_scale),
+                                      dbn=[_grad_of(grads, t) for bn in bns for t in (bn.weight, bn.bias)], want_bf16=want_bf16)
+
+
 class TextEmbedUnit:
     """forward_embedding (mobile_clip.py:815-823): table[ids] + the positional table, resized N -> L when they differ."""
 
@@ -655,14 +760,19 @@ class TextEmbedUnit:
 
 
 class TextStudentTrainGraph:
-    """TextStudentEncoder in train mode: embed -> TransformerEncoder layers (and MobileCLIP-S0's RepMixerBlocks, frozen BN) ->
-    final LayerNorm -> projector (fp32 memory)."""
+    """TextStudentEncoder in train mode: embed -> TransformerEncoder layers (and MobileCLIP-S0's RepMixerBlocks, frozen or
+    batch-statistics BN) -> final LayerNorm -> projector (fp32 memory)."""
 
     def __init__(self, student):
         enc = student.encoder
         self.embed = TextEmbedUnit(enc)
-        self.layers = [RepMixerUnit(b) if isinstance(b, RepMixerBlock) else TextEncoderLayerUnit(b, enc.causal_masking)
-                       for b in enc.transformer]
+        bstat = enc.batch_stat_active()
+
+        def unit(b):
+            if isinstance(b, RepMixerBlock):
+                return RepMixerBatchStatUnit(b, enc) if bstat else RepMixerUnit(b)
+            return TextEncoderLayerUnit(b, enc.causal_masking)
+        self.layers = [unit(b) for b in enc.transformer]
         self.fln = enc.final_layer_norm
         self.proj = _TextLinear(student.projector)
         self.saved = None

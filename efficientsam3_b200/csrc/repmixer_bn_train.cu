@@ -1,0 +1,501 @@
+// MobileCLIP-S0's RepMixerBlock (mobile_clip.py:545-702) with batch-statistics BatchNorm: every BN in train mode, as
+// nn.BatchNorm2d trains.  Each BN normalises with the mean and biased variance of its input over all B*L tokens (padding
+// included) and updates its running buffers.  BN_ms (mixer.rbr_skip) and BN_ns (norm.rbr_skip) both see x, so their statistics
+// are taken once:
+//   c = dw(x; w_mc)   r = BN_ms(x) + BN_mc(c) - BN_ns(x)   x1 = x + ls_tm r
+//   f = dw(x1; w_f)   u = BN_f(f)   y = fc2(gelu(fc1(u)))   x2 = x1 + ls_blk y
+// Forward (es3_repmixer_bn_fwd): statistics of x and c -> finalize (running buffers, folded token-mixer taps) -> statistics of f
+// on x1 recomputed with those taps in repmixer_kernel's FMA order (so they describe exactly the x1 the prologue writes) ->
+// finalize BN_f -> es3_repmixer_bf16 on the device-folded taps.  Backward: with M = B*L and vhat the normalised input, a BN's
+// input gradient is gamma invstd (d - sum(d) / M - vhat sum(d vhat) / M); the two sums are the BN's beta / gamma gradients, so
+// each sequence kernel of repmixer_bwd.cu splits into a sums pass and an apply pass with a fixed-order reduction between them.
+// Layout as repmixer_bwd.cu: one CTA per (sequence, 32 channels), the sequence plus zero halos in shared memory; per-CTA partials
+// in part [B][Q][C] summed over the sequences in index order.  Statistics are fp32 sums shifted by a per-sequence pivot (the
+// sequence's first token), combined across sequences in fp64.  No float atomics: every result is bit-reproducible.
+#include "common.cuh"
+
+namespace es3 {
+namespace {
+
+constexpr int BS_KS = 11, BS_HALO = BS_KS / 2, BS_CH = 32, BS_MAXL = 128, BS_THREADS = 256, BS_ROWS = BS_THREADS / BS_CH;
+constexpr int BS_PAD = BS_MAXL + 2 * BS_HALO;
+constexpr int BS_Q_XC = 6, BS_Q_F = 3, BS_Q_FFN = BS_KS, BS_Q_TM = BS_KS + 1, BS_Q_MAX = BS_Q_TM, BS_NSUM = 3;
+static_assert(BS_Q_MAX * BS_ROWS <= BS_PAD, "the partials' reduction reuses a sequence buffer");
+
+// affine rows [9][C]: ls_tm, then (gamma, beta) of BN_ms, BN_mc, BN_ns, BN_f.  stats rows [8][C]: (mean, invstd) of the same four.
+enum { A_LS = 0, A_G_MS, A_B_MS, A_G_MC, A_B_MC, A_G_NS, A_B_NS, A_G_F, A_B_F };
+enum { S_M_MS = 0, S_I_MS, S_M_MC, S_I_MC, S_M_NS, S_I_NS, S_M_F, S_I_F };
+
+// part[(b Q + q) C + ch0 + c] = sum over the CTA's row groups (in order) of v[q] (as in repmixer_bwd.cu).
+template <int Q>
+__device__ __forceinline__ void cta_partials(const float (&v)[Q], float* red, float* __restrict__ part, int b, int C, int ch0) {
+  const int c = threadIdx.x % BS_CH, r = threadIdx.x / BS_CH;
+  __syncthreads();
+#pragma unroll
+  for (int q = 0; q < Q; ++q) red[(q * BS_ROWS + r) * BS_CH + c] = v[q];
+  __syncthreads();
+  for (int i = threadIdx.x; i < Q * BS_CH; i += BS_THREADS) {
+    const int q = i / BS_CH, cc = i % BS_CH;
+    float s = 0.f;
+#pragma unroll
+    for (int rr = 0; rr < BS_ROWS; ++rr) s += red[(q * BS_ROWS + rr) * BS_CH + cc];
+    part[((long long)b * Q + q) * C + ch0 + cc] = s;
+  }
+}
+
+// s[l + 5] = the sequence's rows, zero halos.
+__device__ __forceinline__ void load_seq(const float* __restrict__ src, float* s, long long base, int L, int C) {
+  const int c = threadIdx.x % BS_CH;
+  for (int l = threadIdx.x / BS_CH; l < L + 2 * BS_HALO; l += BS_ROWS) {
+    const int t = l - BS_HALO;
+    s[l * BS_CH + c] = (t >= 0 && t < L) ? src[base + (long long)t * C] : 0.f;
+  }
+}
+
+__device__ __forceinline__ float conv_at(const float (&w)[BS_KS], const float* s, int l, float acc) {
+  const int c = threadIdx.x % BS_CH;
+#pragma unroll
+  for (int k = 0; k < BS_KS; ++k) acc = fmaf(w[k], s[(l + k) * BS_CH + c], acc);
+  return acc;
+}
+
+// Shifted sums of one value: (pivot, sum (v - pivot), sum (v - pivot)^2); the pivot is counted by row group 0 only.
+__device__ __forceinline__ void shifted(float* v, float piv, float val) {
+  const float d = val - piv;
+  v[1] += d;
+  v[2] = fmaf(d, d, v[2]);
+}
+
+// MODE 0: statistics of x and c = dw(x; w_mc) (part Q = 6).  MODE 1: x1 = bm + dw(x; wm) exactly as repmixer_kernel computes
+// it, then statistics of f = dw(x1; w_f) (part Q = 3).  taps [2][11][C] raw (w_mc, w_f); fold [24][C] (wm, bm, wf, bf).
+template <int MODE>
+__global__ void __launch_bounds__(BS_THREADS) repmixer_bn_stats_kernel(const float* __restrict__ x, const float* __restrict__ taps,
+                                                                       const float* __restrict__ fold, float* __restrict__ part,
+                                                                       int L, int C) {
+  constexpr int Q = MODE == 0 ? BS_Q_XC : BS_Q_F;
+  __shared__ float sx[BS_PAD * BS_CH];
+  __shared__ float sy[BS_PAD * BS_CH];
+  const int c = threadIdx.x % BS_CH, r0 = threadIdx.x / BS_CH;
+  const int ch = blockIdx.x * BS_CH + c;
+  const long long base = (long long)blockIdx.y * L * C + ch;
+  load_seq(x, sx, base, L, C);
+  float w[BS_KS];
+  float v[Q];
+#pragma unroll
+  for (int q = 0; q < Q; ++q) v[q] = 0.f;
+  if constexpr (MODE == 0) {
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) w[k] = taps[k * C + ch];
+    __syncthreads();
+    const float px = sx[BS_HALO * BS_CH + c], pc = conv_at(w, sx, 0, 0.f);
+    if (r0 == 0) { v[0] = px; v[3] = pc; }
+    for (int l = r0; l < L; l += BS_ROWS) {
+      shifted(v, px, sx[(l + BS_HALO) * BS_CH + c]);
+      shifted(v + 3, pc, conv_at(w, sx, l, 0.f));
+    }
+  } else {
+    for (int l = r0; l < L + 2 * BS_HALO; l += BS_ROWS)
+      if (l < BS_HALO || l >= L + BS_HALO) sy[l * BS_CH + c] = 0.f;
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) w[k] = fold[k * C + ch];
+    const float b = fold[BS_KS * C + ch];
+    __syncthreads();
+    for (int l = r0; l < L; l += BS_ROWS) sy[(l + BS_HALO) * BS_CH + c] = conv_at(w, sx, l, b);
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) w[k] = taps[(BS_KS + k) * C + ch];
+    __syncthreads();
+    const float pf = conv_at(w, sy, 0, 0.f);
+    if (r0 == 0) v[0] = pf;
+    for (int l = r0; l < L; l += BS_ROWS) shifted(v, pf, conv_at(w, sy, l, 0.f));
+  }
+  cta_partials<Q>(v, sx, part, blockIdx.y, C, blockIdx.x * BS_CH);
+}
+
+struct BnRun {
+  float* rm;
+  float* rv;
+  long long* nbt;
+  float eps, momentum;
+};
+
+struct BnFinalize {
+  BnRun bn[4];                      // BN_ms, BN_mc, BN_ns, BN_f
+  const float* taps;                // [2][11][C] raw w_mc, w_f
+  const float* aff;                 // [9][C]
+  float* fold;                      // [24][C] wm, bm, wf, bf (repmixer_fold's form)
+  float* stats;                     // [8][C]
+};
+
+// Mean and biased variance (fp64) of one value from the per-sequence shifted sums at q0 .. q0 + 2 of part [B][Q][C]: Chan's
+// combination, sum_b (M2_b + L (mean_b - mean)^2), so no large-magnitude cancellation when |mean| >> std.
+__device__ void combine(const float* __restrict__ part, int Q, int q0, int B, int L, int C, int ch, double& mean, double& var) {
+  const double n = L, M = (double)B * L;
+  double s = 0.0;
+  for (int b = 0; b < B; ++b) {
+    const float* p = part + ((long long)b * Q + q0) * C + ch;
+    s += n * (double)p[0] + (double)p[C];
+  }
+  mean = s / M;
+  double m2 = 0.0;
+  for (int b = 0; b < B; ++b) {
+    const float* p = part + ((long long)b * Q + q0) * C + ch;
+    const double s1 = p[C], mb = (double)p[0] + s1 / n - mean;
+    m2 += ((double)p[2 * C] - s1 * s1 / n) + n * mb * mb;
+  }
+  var = fmax(m2 / M, 0.0);
+}
+
+// Running buffers as nn.BatchNorm2d updates them (unbiased variance, momentum); returns invstd with the biased variance.
+__device__ float bn_update(const BnRun& r, int ch, double mean, double var, double M) {
+  const double mom = r.momentum;
+  r.rm[ch] = (float)((1.0 - mom) * (double)r.rm[ch] + mom * mean);
+  r.rv[ch] = (float)((1.0 - mom) * (double)r.rv[ch] + mom * var * M / (M - 1.0));
+  if (ch == 0) r.nbt[0] += 1;
+  return (float)(1.0 / sqrt(var + (double)r.eps));
+}
+
+// One thread per channel.  MODE 0: BN_ms, BN_ns (statistics of x) and BN_mc (of c); writes wm, bm.  MODE 1: BN_f; writes wf, bf.
+template <int MODE>
+__global__ void repmixer_bn_finalize_kernel(const float* __restrict__ part, int B, int L, int C, BnFinalize f) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= C) return;
+  const double M = (double)B * L;
+  const float* aff = f.aff;
+  if constexpr (MODE == 0) {
+    double mx, vx, mc, vc;
+    combine(part, BS_Q_XC, 0, B, L, C, ch, mx, vx);
+    combine(part, BS_Q_XC, 3, B, L, C, ch, mc, vc);
+    const float i_ms = bn_update(f.bn[0], ch, mx, vx, M), i_mc = bn_update(f.bn[1], ch, mc, vc, M);
+    const float i_ns = bn_update(f.bn[2], ch, mx, vx, M);
+    const float fmx = (float)mx, fmc = (float)mc;
+    float* st = f.stats;
+    st[S_M_MS * C + ch] = fmx; st[S_I_MS * C + ch] = i_ms;
+    st[S_M_MC * C + ch] = fmc; st[S_I_MC * C + ch] = i_mc;
+    st[S_M_NS * C + ch] = fmx; st[S_I_NS * C + ch] = i_ns;
+    const float ls = aff[A_LS * C + ch];
+    const float s_ms = aff[A_G_MS * C + ch] * i_ms, s_mc = aff[A_G_MC * C + ch] * i_mc, s_ns = aff[A_G_NS * C + ch] * i_ns;
+    const float b_ms = aff[A_B_MS * C + ch] - fmx * s_ms, b_mc = aff[A_B_MC * C + ch] - fmc * s_mc;
+    const float b_ns = aff[A_B_NS * C + ch] - fmx * s_ns;
+    const float sw = ls * s_mc;
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) {
+      float wk = f.taps[k * C + ch] * sw;
+      if (k == BS_HALO) wk += 1.f + ls * (s_ms - s_ns);
+      f.fold[k * C + ch] = wk;
+    }
+    f.fold[BS_KS * C + ch] = ls * (b_ms + b_mc - b_ns);
+  } else {
+    double mf, vf;
+    combine(part, BS_Q_F, 0, B, L, C, ch, mf, vf);
+    const float i_f = bn_update(f.bn[3], ch, mf, vf, M), fmf = (float)mf;
+    f.stats[S_M_F * C + ch] = fmf;
+    f.stats[S_I_F * C + ch] = i_f;
+    const float s_f = aff[A_G_F * C + ch] * i_f;
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) f.fold[(BS_KS + 1 + k) * C + ch] = f.taps[(BS_KS + k) * C + ch] * s_f;
+    f.fold[(2 * BS_KS + 1) * C + ch] = aff[A_B_F * C + ch] - fmf * s_f;
+  }
+}
+
+// ConvFFN sums pass: sum du and sum du fhat (BN_f's beta / gamma gradients), fhat = (dw(x1; w_f) - mean_f) invstd_f.
+__global__ void __launch_bounds__(BS_THREADS) repmixer_bn_ffn_sums_kernel(const float* __restrict__ x1, const float* __restrict__ du,
+                                                                          const float* __restrict__ taps, const float* __restrict__ stats,
+                                                                          float* __restrict__ part, int L, int C) {
+  __shared__ float sx1[BS_PAD * BS_CH];
+  const int c = threadIdx.x % BS_CH, r0 = threadIdx.x / BS_CH;
+  const int ch = blockIdx.x * BS_CH + c;
+  const long long base = (long long)blockIdx.y * L * C + ch;
+  load_seq(x1, sx1, base, L, C);
+  float w[BS_KS];
+#pragma unroll
+  for (int k = 0; k < BS_KS; ++k) w[k] = taps[(BS_KS + k) * C + ch];
+  const float mf = stats[S_M_F * C + ch], inv = stats[S_I_F * C + ch];
+  float v[2] = {0.f, 0.f};
+  __syncthreads();
+  for (int l = r0; l < L; l += BS_ROWS) {
+    const float d = du[base + (long long)l * C];
+    v[0] += d;
+    v[1] = fmaf(d, (conv_at(w, sx1, l, 0.f) - mf) * inv, v[1]);
+  }
+  cta_partials<2>(v, sx1, part, blockIdx.y, C, blockIdx.x * BS_CH);
+}
+
+// ConvFFN apply pass: df = s_f (du - S0 / M - fhat S1 / M), e = g + dw^T(df; w_f); partials: the taps' sums df[l] x1[l+k-5].
+__global__ void __launch_bounds__(BS_THREADS) repmixer_bn_ffn_apply_kernel(const float* __restrict__ x1, const float* __restrict__ du,
+                                                                           const float* __restrict__ g, const float* __restrict__ taps,
+                                                                           const float* __restrict__ aff, const float* __restrict__ stats,
+                                                                           const float* __restrict__ sums, float* __restrict__ e,
+                                                                           float* __restrict__ part, int B, int L, int C) {
+  __shared__ float sx1[BS_PAD * BS_CH];
+  __shared__ float sdf[BS_PAD * BS_CH];
+  const int c = threadIdx.x % BS_CH, r0 = threadIdx.x / BS_CH;
+  const int ch = blockIdx.x * BS_CH + c;
+  const long long base = (long long)blockIdx.y * L * C + ch;
+  load_seq(x1, sx1, base, L, C);
+  for (int l = r0; l < L + 2 * BS_HALO; l += BS_ROWS)
+    if (l < BS_HALO || l >= L + BS_HALO) sdf[l * BS_CH + c] = 0.f;
+  float w[BS_KS];
+#pragma unroll
+  for (int k = 0; k < BS_KS; ++k) w[k] = taps[(BS_KS + k) * C + ch];
+  const float mf = stats[S_M_F * C + ch], inv = stats[S_I_F * C + ch], s_f = aff[A_G_F * C + ch] * inv;
+  const float rM = 1.f / ((float)B * (float)L), m0 = sums[ch] * rM, m1 = sums[C + ch] * rM;
+  float v[BS_Q_FFN];
+#pragma unroll
+  for (int q = 0; q < BS_Q_FFN; ++q) v[q] = 0.f;
+  __syncthreads();
+  for (int l = r0; l < L; l += BS_ROWS) {
+    const float fh = (conv_at(w, sx1, l, 0.f) - mf) * inv;
+    const float df = s_f * (du[base + (long long)l * C] - m0 - fh * m1);
+    sdf[(l + BS_HALO) * BS_CH + c] = df;
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) v[k] = fmaf(df, sx1[(l + k) * BS_CH + c], v[k]);
+  }
+  __syncthreads();
+  for (int l = r0; l < L; l += BS_ROWS) {
+    float t = 0.f;
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) t = fmaf(w[k], sdf[(l + 2 * BS_HALO - k) * BS_CH + c], t);   // df[l - k + 5]
+    const long long i = base + (long long)l * C;
+    e[i] = g[i] + t;
+  }
+  cta_partials<BS_Q_FFN>(v, sx1, part, blockIdx.y, C, blockIdx.x * BS_CH);
+}
+
+// Token-mixer sums pass, e' = ls e: sum e', sum e' chat, sum e' (x - mean_x).  BN_ms's gamma gradient is invstd_ms times the last,
+// BN_ns's is -invstd_ns times it (one xhat up to eps).
+__global__ void __launch_bounds__(BS_THREADS) repmixer_bn_tm_sums_kernel(const float* __restrict__ x, const float* __restrict__ e,
+                                                                         const float* __restrict__ taps, const float* __restrict__ aff,
+                                                                         const float* __restrict__ stats, float* __restrict__ part,
+                                                                         int L, int C) {
+  __shared__ float sx[BS_PAD * BS_CH];
+  const int c = threadIdx.x % BS_CH, r0 = threadIdx.x / BS_CH;
+  const int ch = blockIdx.x * BS_CH + c;
+  const long long base = (long long)blockIdx.y * L * C + ch;
+  load_seq(x, sx, base, L, C);
+  float w[BS_KS];
+#pragma unroll
+  for (int k = 0; k < BS_KS; ++k) w[k] = taps[k * C + ch];
+  const float ls = aff[A_LS * C + ch], mx = stats[S_M_MS * C + ch], mc = stats[S_M_MC * C + ch], i_mc = stats[S_I_MC * C + ch];
+  float v[3] = {0.f, 0.f, 0.f};
+  __syncthreads();
+  for (int l = r0; l < L; l += BS_ROWS) {
+    const float ep = ls * e[base + (long long)l * C];
+    v[0] += ep;
+    v[1] = fmaf(ep, (conv_at(w, sx, l, 0.f) - mc) * i_mc, v[1]);
+    v[2] = fmaf(ep, sx[(l + BS_HALO) * BS_CH + c] - mx, v[2]);
+  }
+  cta_partials<3>(v, sx, part, blockIdx.y, C, blockIdx.x * BS_CH);
+}
+
+// Token-mixer apply pass: dc = s_mc (e' - S0/M - chat S1/M), dx = e + [s_ms (e' - S0/M - xhat_ms i_ms S2/M) - s_ns (e' - S0/M -
+// xhat_ns i_ns S2/M)] + dw^T(dc; w_mc); partials: the taps' sums dc[l] x[l+k-5] and the layer scale's sum e r.
+__global__ void __launch_bounds__(BS_THREADS) repmixer_bn_tm_apply_kernel(const float* __restrict__ x, const float* __restrict__ e,
+                                                                          const float* __restrict__ taps, const float* __restrict__ aff,
+                                                                          const float* __restrict__ stats, const float* __restrict__ sums,
+                                                                          float* __restrict__ dx, bf16* __restrict__ dxb,
+                                                                          float* __restrict__ part, int B, int L, int C) {
+  __shared__ float sx[BS_PAD * BS_CH];
+  __shared__ float sdc[BS_PAD * BS_CH];
+  const int c = threadIdx.x % BS_CH, r0 = threadIdx.x / BS_CH;
+  const int ch = blockIdx.x * BS_CH + c;
+  const long long base = (long long)blockIdx.y * L * C + ch;
+  load_seq(x, sx, base, L, C);
+  for (int l = r0; l < L + 2 * BS_HALO; l += BS_ROWS)
+    if (l < BS_HALO || l >= L + BS_HALO) sdc[l * BS_CH + c] = 0.f;
+  float w[BS_KS];
+#pragma unroll
+  for (int k = 0; k < BS_KS; ++k) w[k] = taps[k * C + ch];
+  const float ls = aff[A_LS * C + ch], mx = stats[S_M_MS * C + ch];
+  const float i_ms = stats[S_I_MS * C + ch], mc = stats[S_M_MC * C + ch], i_mc = stats[S_I_MC * C + ch], i_ns = stats[S_I_NS * C + ch];
+  const float g_ms = aff[A_G_MS * C + ch], g_mc = aff[A_G_MC * C + ch], g_ns = aff[A_G_NS * C + ch];
+  const float s_ms = g_ms * i_ms, s_mc = g_mc * i_mc, s_ns = g_ns * i_ns;
+  const float br = aff[A_B_MS * C + ch] + aff[A_B_MC * C + ch] - aff[A_B_NS * C + ch];
+  const float rM = 1.f / ((float)B * (float)L), m0 = sums[ch] * rM, m1 = sums[C + ch] * rM, m2 = sums[2 * C + ch] * rM;
+  const float k_ms = s_ms * i_ms * i_ms * m2, k_ns = s_ns * i_ns * i_ns * m2;     // xhat i S2 / M, per unit (x - mean)
+  float v[BS_Q_TM];
+#pragma unroll
+  for (int q = 0; q < BS_Q_TM; ++q) v[q] = 0.f;
+  __syncthreads();
+  for (int l = r0; l < L; l += BS_ROWS) {
+    const float ev = e[base + (long long)l * C], ep = ls * ev;
+    const float ch_ = (conv_at(w, sx, l, 0.f) - mc) * i_mc, xc = sx[(l + BS_HALO) * BS_CH + c] - mx;
+    const float dc = s_mc * (ep - m0 - ch_ * m1);
+    sdc[(l + BS_HALO) * BS_CH + c] = dc;
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) v[k] = fmaf(dc, sx[(l + k) * BS_CH + c], v[k]);
+    const float r = fmaf(g_ms * i_ms - g_ns * i_ns, xc, fmaf(g_mc, ch_, br));
+    v[BS_KS] = fmaf(ev, r, v[BS_KS]);
+  }
+  __syncthreads();
+  for (int l = r0; l < L; l += BS_ROWS) {
+    const long long i = base + (long long)l * C;
+    const float ev = e[i], ep = ls * ev, xc = sx[(l + BS_HALO) * BS_CH + c] - mx;
+    float t = 0.f;
+#pragma unroll
+    for (int k = 0; k < BS_KS; ++k) t = fmaf(w[k], sdc[(l + 2 * BS_HALO - k) * BS_CH + c], t);   // dc[l - k + 5]
+    const float d0 = ep - m0;
+    const float out = ev + ((s_ms - s_ns) * d0 - (k_ms - k_ns) * xc) + t;
+    dx[i] = out;
+    if (dxb != nullptr) dxb[i] = __float2bfloat16_rn(out);
+  }
+  cta_partials<BS_Q_TM>(v, sx, part, blockIdx.y, C, blockIdx.x * BS_CH);
+}
+
+// Sums of the sums passes: sums[q][c] = sum_b part[b][q][c] (index order); then dst[j][c] += sign[j] (scale[j][c]) sums[src[j]][c].
+constexpr int BS_MAXDST = 6;
+struct BnGradDst {
+  int n;
+  int src[BS_MAXDST];
+  float sign[BS_MAXDST];
+  const float* scale[BS_MAXDST];
+  float* dst[BS_MAXDST];
+};
+
+template <int Q>
+__global__ void repmixer_bn_sums_kernel(const float* __restrict__ part, int nseq, int C, float* __restrict__ sums, BnGradDst d) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float acc[Q];
+#pragma unroll
+  for (int q = 0; q < Q; ++q) acc[q] = 0.f;
+  for (int b = 0; b < nseq; ++b) {
+#pragma unroll
+    for (int q = 0; q < Q; ++q) acc[q] += part[((long long)b * Q + q) * C + c];
+  }
+#pragma unroll
+  for (int q = 0; q < Q; ++q) sums[q * C + c] = acc[q];
+  for (int j = 0; j < d.n; ++j) {
+    float a = 0.f;
+#pragma unroll
+    for (int q = 0; q < Q; ++q) if (q == d.src[j]) a = acc[q];
+    if (d.scale[j] != nullptr) a *= d.scale[j][c];
+    d.dst[j][c] += d.sign[j] * a;
+  }
+}
+
+struct DstBuilder {
+  BnGradDst d;
+  DstBuilder() { d.n = 0; }
+  void add(int src, float* dst, float sign = 1.f, const float* scale = nullptr) {
+    if (dst == nullptr) return;
+    d.src[d.n] = src; d.dst[d.n] = dst; d.sign[d.n] = sign; d.scale[d.n] = scale;
+    ++d.n;
+  }
+};
+
+// Taps / layer-scale partials into torch layouts: dst[j][c * stride[j]] += sum_b part[b][src[j]][c] (as repmixer_sum_kernel).
+constexpr int BS_MAXSUM = 12;
+struct BsSums {
+  int n, Q;
+  int src[BS_MAXSUM], stride[BS_MAXSUM];
+  float* dst[BS_MAXSUM];
+};
+
+__global__ void repmixer_bn_grad_sum_kernel(const float* __restrict__ part, int nseq, int C, BsSums s) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y;
+  if (c >= C) return;
+  const int q = s.src[j];
+  float acc = 0.f;
+  for (int b = 0; b < nseq; ++b) acc += part[((long long)b * s.Q + q) * C + c];
+  s.dst[j][(long long)c * s.stride[j]] += acc;
+}
+
+int launch_grad_sums(const float* part, int Q, float* dtaps, float* dls, int B, int C, cudaStream_t st) {
+  BsSums s;
+  s.n = 0; s.Q = Q;
+  if (dtaps != nullptr)
+    for (int k = 0; k < BS_KS; ++k) { s.src[s.n] = k; s.dst[s.n] = dtaps + k; s.stride[s.n] = BS_KS; ++s.n; }
+  if (dls != nullptr) { s.src[s.n] = BS_KS; s.dst[s.n] = dls; s.stride[s.n] = 1; ++s.n; }
+  if (s.n == 0) return 0;
+  repmixer_bn_grad_sum_kernel<<<dim3(ceil_div(C, 128), s.n), 128, 0, st>>>(part, B, C, s);
+  ES3_LAUNCH_CHECK("repmixer_bn_grad_sum_kernel");
+  return 0;
+}
+
+}  // namespace
+}  // namespace es3
+
+using namespace es3;
+
+extern "C" int es3_repmixer_bf16(const float* x, float* x1, void* u, const float* wm, const float* bm, const float* wf,
+                                 const float* bf, int B, int L, int C, void* stream);
+
+#define BS_CHECK_SHAPE(fn)                                                                                                     \
+  ES3_REQUIRE(L >= 1 && L <= BS_MAXL, fn ": sequence length %d outside 1..%d (the sequence is kept in shared memory)", L,  \
+              BS_MAXL);                                                                                                        \
+  ES3_REQUIRE(B >= 1 && C >= BS_CH && C % BS_CH == 0, fn ": need B >= 1 and C %% %d == 0 (B=%d C=%d)", BS_CH, B, C);          \
+  ES3_REQUIRE((long long)B * L >= 2, fn ": batch statistics need more than one value per channel (B*L=%d)", B * L)
+
+extern "C" long long es3_repmixer_bn_ws_floats(int B, int C) { return ((long long)B * BS_Q_MAX + BS_NSUM) * C; }
+
+/* Batch-statistics forward: x [B*L, C] fp32 -> x1 fp32, u bf16 (as es3_repmixer_bf16); updates the four BNs' running buffers and
+ * num_batches_tracked; writes fold [24][C] (wm, bm, wf, bf) and stats [8][C] ((mean, invstd) of BN_ms, BN_mc, BN_ns, BN_f). */
+extern "C" int es3_repmixer_bn_fwd(const float* x, float* x1, void* u, const float* taps, const float* aff, float* rm_ms, float* rv_ms,
+                                   long long* nbt_ms, float* rm_mc, float* rv_mc, long long* nbt_mc, float* rm_ns, float* rv_ns,
+                                   long long* nbt_ns, float* rm_f, float* rv_f, long long* nbt_f, float eps_ms, float eps_mc,
+                                   float eps_ns, float eps_f, float mom_ms, float mom_mc, float mom_ns, float mom_f, float* fold,
+                                   float* stats, float* ws, int B, int L, int C, void* stream) {
+  BS_CHECK_SHAPE("es3_repmixer_bn_fwd");
+  cudaStream_t st = (cudaStream_t)stream;
+  BnFinalize f;
+  f.bn[0] = BnRun{rm_ms, rv_ms, nbt_ms, eps_ms, mom_ms};
+  f.bn[1] = BnRun{rm_mc, rv_mc, nbt_mc, eps_mc, mom_mc};
+  f.bn[2] = BnRun{rm_ns, rv_ns, nbt_ns, eps_ns, mom_ns};
+  f.bn[3] = BnRun{rm_f, rv_f, nbt_f, eps_f, mom_f};
+  f.taps = taps; f.aff = aff; f.fold = fold; f.stats = stats;
+  const dim3 grid(C / BS_CH, B);
+  repmixer_bn_stats_kernel<0><<<grid, BS_THREADS, 0, st>>>(x, taps, fold, ws, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_stats_kernel<xc>");
+  repmixer_bn_finalize_kernel<0><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, L, C, f);
+  ES3_LAUNCH_CHECK("repmixer_bn_finalize_kernel<xc>");
+  repmixer_bn_stats_kernel<1><<<grid, BS_THREADS, 0, st>>>(x, taps, fold, ws, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_stats_kernel<f>");
+  repmixer_bn_finalize_kernel<1><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, L, C, f);
+  ES3_LAUNCH_CHECK("repmixer_bn_finalize_kernel<f>");
+  return es3_repmixer_bf16(x, x1, u, fold, fold + BS_KS * C, fold + (BS_KS + 1) * C, fold + (2 * BS_KS + 1) * C, B, L, C, stream);
+}
+
+/* ConvFFN.conv + BN_f backward with batch statistics: e = g + dw^T(df; w_f); dwf [C,1,1,11], dgamma, dbeta [C] += (may be null). */
+extern "C" int es3_repmixer_bn_ffn_bwd(const float* x1, const float* du, const float* g, const float* taps, const float* aff,
+                                       const float* stats, float* e, float* ws, float* dwf, float* dgamma, float* dbeta, int B, int L,
+                                       int C, void* stream) {
+  BS_CHECK_SHAPE("es3_repmixer_bn_ffn_bwd");
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid(C / BS_CH, B);
+  float* sums = ws + (long long)B * BS_Q_MAX * C;
+  repmixer_bn_ffn_sums_kernel<<<grid, BS_THREADS, 0, st>>>(x1, du, taps, stats, ws, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_ffn_sums_kernel");
+  DstBuilder db;
+  db.add(0, dbeta);
+  db.add(1, dgamma);
+  repmixer_bn_sums_kernel<2><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, C, sums, db.d);
+  ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<ffn>");
+  repmixer_bn_ffn_apply_kernel<<<grid, BS_THREADS, 0, st>>>(x1, du, g, taps, aff, stats, sums, e, ws, B, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_ffn_apply_kernel");
+  return launch_grad_sums(ws, BS_Q_FFN, dwf, nullptr, B, C, st);
+}
+
+/* Token-mixer backward with batch statistics: dx fp32 (+ bf16 copy dxb, may be null); dwmc [C,1,1,11], dls [C,1,1] and the gamma /
+ * beta gradients [C] of BN_ms, BN_mc, BN_ns += theirs (each may be null). */
+extern "C" int es3_repmixer_bn_tm_bwd(const float* x, const float* e, const float* taps, const float* aff, const float* stats, float* dx,
+                                      void* dxb, float* ws, float* dwmc, float* dls, float* dg_ms, float* db_ms, float* dg_mc,
+                                      float* db_mc, float* dg_ns, float* db_ns, int B, int L, int C, void* stream) {
+  BS_CHECK_SHAPE("es3_repmixer_bn_tm_bwd");
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid(C / BS_CH, B);
+  float* sums = ws + (long long)B * BS_Q_MAX * C;
+  repmixer_bn_tm_sums_kernel<<<grid, BS_THREADS, 0, st>>>(x, e, taps, aff, stats, ws, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_tm_sums_kernel");
+  DstBuilder db;
+  db.add(0, db_ms);
+  db.add(0, db_mc);
+  db.add(0, db_ns, -1.f);
+  db.add(1, dg_mc);
+  db.add(2, dg_ms, 1.f, stats + S_I_MS * C);
+  db.add(2, dg_ns, -1.f, stats + S_I_NS * C);
+  repmixer_bn_sums_kernel<3><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, C, sums, db.d);
+  ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<tm>");
+  repmixer_bn_tm_apply_kernel<<<grid, BS_THREADS, 0, st>>>(x, e, taps, aff, stats, sums, dx, (bf16*)dxb, ws, B, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_tm_apply_kernel");
+  return launch_grad_sums(ws, BS_Q_TM, dwmc, dls, B, C, st);
+}

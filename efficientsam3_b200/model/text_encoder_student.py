@@ -11,6 +11,8 @@ i.e. frozen BN as set_bn_state / TRAIN.EVAL_BN_WHEN_TRAINING leaves it) with gra
 node (TextStudentTrainFunction) whose backward runs the native kernels (backbones/mobile_clip.py TextStudentTrainGraph).  `encoder.projection_layer` is not used here (the reference calls the encoder with return_all_tokens=True):
 it gets no gradient, so optimisers skip it (build stage1.optim.FlatAdamW with exclude=TextStudentEncoder.UNUSED_PARAMETERS).
 A train-mode module under torch.no_grad() runs the eval path: the base students have no train-time behaviour besides gradients.
+MobileCLIP-S0 after enable_batch_stat_bn() with its BatchNorms in train mode normalises with batch statistics instead, with grad
+or under torch.no_grad(), and updates the running buffers on every forward (RepMixerBatchStatUnit).
 """
 from __future__ import annotations
 
@@ -67,8 +69,23 @@ class TextStudentEncoder(nn.Module, NativePlanMixin):
         with torch.no_grad():
             return self._forward_eval(text, dev)
 
+    def enable_batch_stat_bn(self, enabled: bool = True):
+        """Opt in to batch-statistics BatchNorm in MobileCLIP-S0's RepMixerBlocks: with every such BN in train mode, each forward
+        (grad enabled or not) normalises with the batch's mean / variance over all B*L tokens and updates running_mean /
+        running_var / num_batches_tracked, as nn.BatchNorm2d trains.  A caption's output then depends on its batch.  With the BNs
+        in .eval() the frozen path runs unchanged.  A plain attribute of the encoder (not in the state_dict); no effect on the
+        TransformerEncoder-only students.  Returns self."""
+        self.encoder.batch_stat_bn = bool(enabled)
+        return self
+
+    def _check_batch(self, ids):
+        if self.encoder.batch_stat_active() and ids.shape[0] * ids.shape[1] < 2:
+            raise ValueError("TextStudentEncoder: batch-statistics BatchNorm expects more than 1 value per channel when training "
+                             f"(B*L = {ids.shape[0] * ids.shape[1]})")
+
     def _forward_eval(self, text, dev):
         ids = self.tokenize(text)
+        self._check_batch(ids)
         mask = (ids != 0).bool().ne(1)                       # True = padding (text_encoder_student.py:56)
         B, L = ids.shape
         emb = self.encoder._embed(ids)                       # [B, L, dim]: also the trunk's input stream
@@ -87,6 +104,7 @@ class TextStudentEncoder(nn.Module, NativePlanMixin):
         if ids.shape[1] > ops.TEXT_ATTN_BWD_MAX_L:
             raise ValueError(f"TextStudentEncoder: training takes 1..{ops.TEXT_ATTN_BWD_MAX_L} tokens per caption, got "
                              f"{ids.shape[1]}")
+        self._check_batch(ids)
         mask = (ids != 0).bool().ne(1)
         memory, emb = TextStudentTrainFunction.apply(self, ids, *self.trainable_parameters())
         return mask.to(dev), memory.transpose(0, 1), emb.transpose(0, 1)

@@ -613,6 +613,72 @@ def repmixer_tm_bwd(x, e, taps, bnp, B, L, dtaps=None, dls=None, dbn=(None,) * 6
     return dx, dxb
 
 
+# ------------------------------------------------------------------------------------ RepMixerBlock, batch-statistics BN (repmixer_bn_train.cu)
+KERNELS_PER_CALL.update({"es3_repmixer_bn_fwd": 5, "es3_repmixer_bn_ffn_bwd": 4, "es3_repmixer_bn_tm_bwd": 4})
+
+
+def _repmixer_bn_args(name, rows, B, L, taps, aff, stats=None):
+    """_repmixer_bwd_args plus B*L >= 2 (a batch statistic needs more than one value per channel, as nn.BatchNorm2d requires);
+    taps [2, 11, C], aff [9, C], stats [8, C] fp32 contiguous."""
+    if B * L < 2:
+        raise ValueError(f"{name}: batch-statistics BatchNorm needs more than 1 value per channel (B*L = {B * L})")
+    C = rows[0].shape[-1]
+    params = [(taps, (2, 11, C)), (aff, (9, C))] + ([(stats, (8, C))] if stats is not None else [])
+    return _repmixer_bwd_args(name, rows, B, L, params)
+
+
+def repmixer_bn_fwd(x, B, L, taps, aff, bns):
+    """RepMixerBlock prologue with batch-statistics BatchNorm on x [B*L, C] fp32.  taps [2, 11, C] = raw w_mc, w_f; aff [9, C] =
+    ls_tm, (gamma, beta) of BN_ms, BN_mc, BN_ns, BN_f; bns = those four nn.BatchNorm2d, whose running_mean / running_var /
+    num_batches_tracked are updated in place on the device.  Returns (x1 fp32, u bf16, fold [24, C] = wm, bm, wf, bf,
+    stats [8, C] = (batch mean, invstd) of the four BNs)."""
+    C = _repmixer_bn_args("repmixer_bn_fwd", (x,), B, L, taps, aff)
+    run = []
+    for bn in bns:
+        for t in (bn.running_mean, bn.running_var):
+            _chk(t, torch.float32, "running statistics")
+            if not (t.is_contiguous() and t.numel() == C):
+                raise ValueError(f"repmixer_bn_fwd: expected contiguous fp32 running statistics of {C} channels")
+        _chk(bn.num_batches_tracked, torch.int64, "num_batches_tracked")
+        run += [bn.running_mean.data_ptr(), bn.running_var.data_ptr(), bn.num_batches_tracked.data_ptr()]
+    x1 = torch.empty_like(x)
+    u = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16)
+    fold = torch.empty((24, C), device=x.device, dtype=torch.float32)
+    stats = torch.empty((8, C), device=x.device, dtype=torch.float32)
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
+    _call("es3_repmixer_bn_fwd", "repmixer_bn_fwd", _nb(x, x, x1, u, x), 3 * 4 * 11 * B * L * C, x.data_ptr(), x1.data_ptr(),
+          u.data_ptr(), taps.data_ptr(), aff.data_ptr(), *run, *[float(bn.eps) for bn in bns],
+          *[float(bn.momentum) for bn in bns], fold.data_ptr(), stats.data_ptr(), ws.data_ptr(), B, L, C, _stream())
+    return x1, u, fold, stats
+
+
+def repmixer_bn_ffn_bwd(x1, du, g, taps, aff, stats, B, L, dtaps=None, dgamma=None, dbeta=None):
+    """ConvFFN.conv + BN_f backward with batch statistics (stats from repmixer_bn_fwd): returns e = g + dw^T(df; w_f) fp32;
+    dtaps [C,1,1,11], dgamma, dbeta [C] accumulated."""
+    C = _repmixer_bn_args("repmixer_bn_ffn_bwd", (x1, du, g), B, L, taps, aff, stats)
+    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dgamma, C, "dgamma"), _grad_dst(dbeta, C, "dbeta")]
+    e = torch.empty_like(x1)
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x1.device)
+    _call("es3_repmixer_bn_ffn_bwd", "repmixer_bn_ffn_bwd", _nb(x1, du, x1, du, g, e), 8 * 11 * x1.numel(), x1.data_ptr(),
+          du.data_ptr(), g.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), e.data_ptr(), ws.data_ptr(), *ptrs,
+          B, L, C, _stream())
+    return e
+
+
+def repmixer_bn_tm_bwd(x, e, taps, aff, stats, B, L, dtaps=None, dls=None, dbn=(None,) * 6, want_bf16=False):
+    """RepMixer token-mixer backward with batch statistics: returns (dx fp32, bf16 copy | None); dtaps [C,1,1,11], dls [C,1,1]
+    and dbn = (dgamma, dbeta) x (ms, mc, ns) accumulated."""
+    C = _repmixer_bn_args("repmixer_bn_tm_bwd", (x, e), B, L, taps, aff, stats)
+    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dls, C, "dls")] + [_grad_dst(t, C, "dbn") for t in dbn]
+    dx = torch.empty_like(x)
+    dxb = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
+    _call("es3_repmixer_bn_tm_bwd", "repmixer_bn_tm_bwd", _nb(x, e, x, e, dx, dxb), 10 * 11 * x.numel(), x.data_ptr(),
+          e.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), dx.data_ptr(), _ptr(dxb), ws.data_ptr(), *ptrs,
+          B, L, C, _stream())
+    return dx, dxb
+
+
 # ------------------------------------------------------------------------------------ text-student backward (text_bwd.cu)
 TEXT_ATTN_BWD_MAX_L = 128
 KERNELS_PER_CALL.update({"es3_layernorm_bwd_f32": 2, "es3_text_kd_loss_fwd": 2, "es3_text_consistency_fwd": 2,

@@ -96,8 +96,10 @@ def train_text_one_epoch(config, model, data_loader, optimizer, epoch, lr_at=Non
     never sees a gradient for encoder.projection_layer).  Reads DISTILL.NUM_EMBED / EMBED_DIM (the stored embeddings' shape),
     MASK_PAD_TOKENS, COSINE and CONSISTENCY_LOSS; TRAIN.ACCUMULATION_STEPS / CLIP_GRAD and the cosine schedule as
     train_one_epoch does.  With TRAIN.EVAL_BN_WHEN_TRAINING (read with a default of False) every BatchNorm goes back to eval mode
-    after model.train(), as set_bn_state does: MobileCLIP-S0 trains natively only with frozen BatchNorm.  The reference's text
-    trainer leaves that call commented out (train_text_encoder_stage1.py:173); its text configs all set the key False.
+    after model.train(), as set_bn_state does, and MobileCLIP-S0 trains with frozen BatchNorm.  Without it, S0 trains with
+    batch-statistics BatchNorm once the model opted in (TextStudentEncoder.enable_batch_stat_bn), as the reference's text configs
+    run it; otherwise it raises.  The reference's text trainer leaves that call commented out (train_text_encoder_stage1.py:173);
+    its text configs all set the key False.
     Returns the list of per-iteration losses (device scalars)."""
     from .losses import text_kd_train_step
     model.train()

@@ -258,6 +258,27 @@ int es3_repmixer_tm_bwd(const float* x, const float* e, const float* wmc, const 
                         float* dls, float* dg_ms, float* db_ms, float* dg_mc, float* db_mc, float* dg_ns, float* db_ns, int B, int L,
                         int C, void* stream);
 
+/* MobileCLIP-S0's RepMixerBlock with batch-statistics BatchNorm (repmixer_bn_train.cu), 1 <= L <= 128, C % 32 == 0, B*L >= 2; one
+ * CTA per (sequence, 32 channels).  taps [2][11][C] fp32 = the raw depthwise weights of mixer.rbr_conv.0.conv and convffn.conv.conv;
+ * aff [9][C] = ls_tm, then (gamma, beta) of BN_ms (mixer.rbr_skip), BN_mc (mixer.rbr_conv.0.bn), BN_ns (norm.rbr_skip), BN_f
+ * (convffn.conv.bn); stats [8][C] = (batch mean, invstd) of the same four.  ws: es3_repmixer_bn_ws_floats(B, C).
+ * es3_repmixer_bn_fwd: mean / biased variance over the B*L tokens (fixed-order, fp64 combination), running buffers updated in place
+ * with the unbiased variance and momentum, num_batches_tracked += 1; fold [24][C] = (wm, bm, wf, bf) as the eval fold writes them,
+ * then es3_repmixer_bf16 on them (x1 fp32, u bf16).  Five kernels.
+ * es3_repmixer_bn_ffn_bwd: e = g + dw^T(df; w_f), df = the batch-statistics BN_f input gradient; dwf, dgamma, dbeta += theirs.
+ * es3_repmixer_bn_tm_bwd: the token mixer's dx fp32 (+ bf16 copy dxb); dwmc, dls and the three BNs' gamma / beta += theirs.
+ * Each backward is a sums pass, a fixed-order reduction, an apply pass and the gradient sums (four kernels); null gradients skip. */
+long long es3_repmixer_bn_ws_floats(int B, int C);
+int es3_repmixer_bn_fwd(const float* x, float* x1, void* u, const float* taps, const float* aff, float* rm_ms, float* rv_ms,
+                        long long* nbt_ms, float* rm_mc, float* rv_mc, long long* nbt_mc, float* rm_ns, float* rv_ns, long long* nbt_ns,
+                        float* rm_f, float* rv_f, long long* nbt_f, float eps_ms, float eps_mc, float eps_ns, float eps_f, float mom_ms,
+                        float mom_mc, float mom_ns, float mom_f, float* fold, float* stats, float* ws, int B, int L, int C, void* stream);
+int es3_repmixer_bn_ffn_bwd(const float* x1, const float* du, const float* g, const float* taps, const float* aff, const float* stats,
+                            float* e, float* ws, float* dwf, float* dgamma, float* dbeta, int B, int L, int C, void* stream);
+int es3_repmixer_bn_tm_bwd(const float* x, const float* e, const float* taps, const float* aff, const float* stats, float* dx, void* dxb,
+                           float* ws, float* dwmc, float* dls, float* dg_ms, float* db_ms, float* dg_mc, float* db_mc, float* dg_ns,
+                           float* db_ns, int B, int L, int C, void* stream);
+
 /* ------------------------------------------------------------------------------------------ SAM heads */
 /* PositionEmbeddingRandom over an h x w grid -> [h*w, 2F] fp32 (PromptEncoder.get_dense_pe, prompt_encoder.py:61-69). */
 int es3_dense_pe(const float* gauss, int F, int h, int w, float* out, void* stream);

@@ -12,7 +12,8 @@ three forwards -> global-norm clip 5.0 -> AdamW.  Both arms tokenise on the host
 seeded word sequences (3-14 words) over the words of the test strings, tokenised with the CLIP merge subset the tests rebuild
 (tests/golden/text_bpe_subset.json); teacher embeddings are seeded random fp16 values upcast to fp32, as stored.
 MobileCLIP-S0 runs with every BatchNorm frozen in .eval() (TRAIN.EVAL_BN_WHEN_TRAINING: running statistics, as the oracle's BN
-in both eager arms).  Algorithmic FLOPs per step (train_flops): three forwards (oracle.text.flops_mobileclip) and three backwards, each GEMM's backward
+in both eager arms); its *_bnstat_* rows train with batch-statistics BatchNorm (enable_batch_stat_bn, as the shipped S0 text configs
+run), and their eager arms run the batch-statistics oracle (tests/oracle_text_bn.py), which updates running buffers too.  Algorithmic FLOPs per step (train_flops): three forwards (oracle.text.flops_mobileclip) and three backwards, each GEMM's backward
 2x its forward, the attention backward 10 B L^2 C per layer (S recomputed, dP, dV, dQ, dK) against the forward's 4 B L^2 C.
 """
 from __future__ import annotations
@@ -71,22 +72,28 @@ def per_step_ms(fn, steps, warmup):
     return statistics.median(times), q[0], q[-1]
 
 
-def eager_arm(sd_dev, tok, ctx, caps, teacher, cfg, amp, trainable=None):
+def eager_arm(sd_dev, tok, ctx, caps, teacher, cfg, amp, trainable=None, bn_stat=False):
     """The oracle graph trained as the reference's loop does (train_text_encoder_stage1.py:221-288), consistency block twice.
-    trainable: the parameter names (default: every state_dict entry; BatchNorm buffers are not parameters)."""
+    trainable: the parameter names (default: every state_dict entry; BatchNorm buffers are not parameters).  bn_stat: the
+    RepMixerBlocks' BatchNorms in train mode (batch statistics, running buffers updated)."""
     from efficientsam3_b200.stage1.losses import permute_words
     from oracle import text as OT
+    from oracle_text_bn import running_clones, text_student_bn
     params = {k: v.clone().requires_grad_(True) for k, v in sd_dev.items()
               if k != "encoder.projection_layer" and (trainable is None or k in trainable)}
     sd = dict(sd_dev, **params)
     opt = torch.optim.AdamW(list(params.values()), lr=1e-4, weight_decay=0.05)
     scaler = torch.amp.GradScaler("cuda", enabled=amp)
     dev = teacher.device
+    run = running_clones(sd_dev) if bn_stat else None
+
+    def student(ids):
+        return text_student_bn(sd, ids, cfg, run) if bn_stat else OT.text_student(sd, ids, cfg)
 
     def step():
         ids = tok(caps, context_length=ctx).to(dev, non_blocking=True)
         with torch.autocast("cuda", dtype=torch.float16, enabled=amp):
-            preds = OT.text_student(sd, ids, cfg)[1].transpose(0, 1)
+            preds = student(ids)[1].transpose(0, 1)
             valid = (ids != 0).float()
             sim = F.cosine_similarity(preds, teacher, dim=2)
             n = valid.sum(1).clamp(min=1.0)
@@ -94,7 +101,7 @@ def eager_arm(sd_dev, tok, ctx, caps, teacher, cfg, amp, trainable=None):
             loss = loss + COSINE * (((1.0 - sim) * valid).sum(1) / n).mean()
             for _ in range(2):
                 pids = tok([permute_words(c) for c in caps], context_length=ctx).to(dev, non_blocking=True)
-                q = OT.text_student(sd, pids, cfg)[1].transpose(0, 1)
+                q = student(pids)[1].transpose(0, 1)
                 loss = loss + CONSISTENCY * F.mse_loss(preds.mean(dim=1), q.mean(dim=1))
         scaler.scale(loss).backward()
         scaler.unscale_(opt)
@@ -130,14 +137,19 @@ def main():
     for tag, backbone, B, L in (("mobileclip_s1_b64_ctx32", "MobileCLIP-S1", 64, 32), ("mobileclip_s1_b64_ctx16", "MobileCLIP-S1", 64, 16),
                                 ("mobileclip2_l_b32_ctx32", "MobileCLIP2-L", 32, 32), ("mobileclip2_l_b32_ctx16", "MobileCLIP2-L", 32, 16),
                                 ("mobileclip_b_b64_ctx32", "MobileCLIP-B", 64, 32),
-                                ("mobileclip_s0_b64_ctx32", "MobileCLIP-S0", 64, 32), ("mobileclip_s0_b64_ctx16", "MobileCLIP-S0", 64, 16)):
+                                ("mobileclip_s0_b64_ctx32", "MobileCLIP-S0", 64, 32), ("mobileclip_s0_b64_ctx16", "MobileCLIP-S0", 64, 16),
+                                ("mobileclip_s0_bnstat_b64_ctx32", "MobileCLIP-S0", 64, 32),
+                                ("mobileclip_s0_bnstat_b64_ctx16", "MobileCLIP-S0", 64, 16)):
         m = build_text_student_model(NS(MODEL=NS(BACKBONE=backbone, BPE_PATH=BPE), DISTILL=NS(EMBED_DIM=256, CONTEXT_LENGTH=L)))
         sd = fill_state_dict(m.state_dict(), 1)
         m.load_state_dict(sd)
         m = m.to(dev).train()
         enc = m.encoder
         mct = enc.transformer[0].__class__.__name__ == "RepMixerBlock"
-        if mct:       # S0 trains with frozen BatchNorm (TRAIN.EVAL_BN_WHEN_TRAINING); the oracle's BN uses running statistics too
+        bn_stat = "_bnstat_" in tag
+        if bn_stat:   # batch-statistics BatchNorm, as the shipped S0 text configs train (EVAL_BN_WHEN_TRAINING False)
+            m.enable_batch_stat_bn()
+        elif mct:     # S0 trains with frozen BatchNorm (TRAIN.EVAL_BN_WHEN_TRAINING); the oracle's BN uses running statistics too
             for mod in m.modules():
                 if isinstance(mod, torch.nn.modules.batchnorm._BatchNorm):
                     mod.eval()
@@ -161,13 +173,13 @@ def main():
         ms, ms_lo, ms_hi = per_step_ms(native, args.steps, args.warmup)
         sd_dev = {k: v.to(dev) for k, v in sd.items()}
         names = {n for n, _ in m.named_parameters()}
-        ms16, ms16_lo, ms16_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, True, names), args.steps,
+        ms16, ms16_lo, ms16_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, True, names, bn_stat), args.steps,
                                              args.warmup)
-        ms32, ms32_lo, ms32_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, False, names), args.steps,
+        ms32, ms32_lo, ms32_hi = per_step_ms(eager_arm(sd_dev, m.tokenizer, L, caps, teacher, cfg, False, names, bn_stat), args.steps,
                                              args.warmup)
         flops = train_flops(cfg, B, L, 256)
         r3 = lambda *v: [round(x, 3) for x in v]  # noqa: E731
-        res[tag] = dict(batch=B, ctx=L, **(dict(frozen_bn=True) if mct else {}), native_ms=round(ms, 3), native_p10_p90_ms=r3(ms_lo, ms_hi), launches_per_step=launches,
+        res[tag] = dict(batch=B, ctx=L, **(dict(frozen_bn=not bn_stat) if mct else {}), native_ms=round(ms, 3), native_p10_p90_ms=r3(ms_lo, ms_hi), launches_per_step=launches,
                         gflop_per_step=round(flops / 1e9, 1), native_tflops=round(flops / ms / 1e9, 2),
                         eager_fp16_autocast_ms=round(ms16, 3), eager_fp16_autocast_p10_p90_ms=r3(ms16_lo, ms16_hi),
                         eager_fp32_ms=round(ms32, 3), eager_fp32_p10_p90_ms=r3(ms32_lo, ms32_hi),

@@ -96,6 +96,17 @@ SIGNATURES: dict[str, list] = {
     "es3_affine_act": [_vp, _vp, _vp, _i, _vp, _vp, _ll, _i, _vp],
     "es3_bn_act_bwd_reduce": [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _ll, _i, _vp, _vp, _vp, _vp, _vp],
     "es3_bn_act_bwd_apply": [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ll, _i, _vp],
+    # synchronised BatchNorm (bn_sync.cu)
+    "es3_bn_stats_partial": [_vp, _ll, _i, _vp, _vp, _vp],
+    "es3_bn_stats_combine": [_vp, _i, _i, _f, _f] + [_vp] * 11,
+    "es3_bn_act_bwd_partial": [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ll, _i, _vp, _vp, _vp, _vp, _vp],
+    "es3_bn_bwd_coef": [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp],
+    "es3_repmixer_bn_stats_partial": [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp],
+    "es3_repmixer_bn_finalize_sync": [_vp, _i, _i] + [_vp] * 14 + [_f] * 8 + [_vp] * 3 + [_i, _vp],
+    "es3_repmixer_bn_ffn_sums": [_vp] * 8 + [_i, _i, _i, _vp],
+    "es3_repmixer_bn_ffn_apply": [_vp] * 7 + [_i] + [_vp] * 4 + [_i, _i, _i, _vp],
+    "es3_repmixer_bn_tm_sums": [_vp] * 13 + [_i, _i, _i, _vp],
+    "es3_repmixer_bn_tm_apply": [_vp] * 6 + [_i] + [_vp] * 6 + [_i, _i, _i, _vp],
     "es3_add_bf16": [_vp, _ll, _vp, _ll, _vp, _ll, _ll, _i, _vp],
     "es3_wgrad_pw": [_vp, _ll, _vp, _ll, _ll, _i, _i, _i, _i, _i, _i, _vp, _vp, _ll, _ll, _vp],
     "es3_transpose_pad_bf16": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp],

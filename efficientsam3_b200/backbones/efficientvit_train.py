@@ -23,7 +23,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, sync_bn
 from ..nn_utils import cached_pack, dw_weight, dw_weight_rot, pw_weight, pw_weight_t
 from .efficientvit import (ConvLayer, DSConv, EfficientViTBlock, LiteMLA, MBConv, ResidualBlock)
 
@@ -85,14 +85,14 @@ class ConvUnit:
         z = self._raw(x)
         if self.plain:
             assert residual is None
-            self.saved = (x, None, None, None, None, None, "none")
+            self.saved = (x, None, None, None, None, None, "none", None)
             return z
         norm = self.norm
+        sync = None
         if norm is None:
             scale, shift, mean, invstd, mode = None, self.conv.bias.detach().float().contiguous(), None, None, "none"
-        elif norm.training:
-            mean, invstd, scale, shift = ops.bn_stats(z, norm.weight.detach(), norm.bias.detach(), norm.eps, norm.momentum,
-                                                      norm.running_mean, norm.running_var, norm.num_batches_tracked)
+        elif norm.training:   # per-rank statistics, or synchronised over the process group of an nn.SyncBatchNorm (sync_bn.py)
+            mean, invstd, scale, shift, sync = sync_bn.batch_stats(norm, z)
             mode = "batch"
         else:   # frozen BN inside a training model: O(C) vector prep on the running statistics
             mean = norm.running_mean.detach().float().contiguous()
@@ -101,14 +101,14 @@ class ConvUnit:
             shift = (norm.bias.detach().float() - mean * scale).contiguous()
             mode = "eval"
         a = ops.affine_act(z, scale, shift, self.act, residual)
-        self.saved = (x, z, scale, shift, mean, invstd, mode)
+        self.saved = (x, z, scale, shift, mean, invstd, mode, sync)
         return a
 
     # ---- backward -----------------------------------------------------------------------------------------------------
     def backward(self, da, grads, need_dx=True, dx_residual=None):
         """da: gradient of the unit's output (bf16, NHWC).  dx_residual: gradient arriving at x over a skip connection,
         added to the returned dx.  Returns dx (None for the stem / need_dx=False)."""
-        x, z, scale, shift, mean, invstd, mode = self.saved
+        x, z, scale, shift, mean, invstd, mode, sync = self.saved
         self.saved = None
         conv, norm = self.conv, self.norm
         if self.plain:
@@ -116,7 +116,7 @@ class ConvUnit:
         else:
             dgamma = _grad_of(grads, norm.weight) if norm is not None else None
             dbeta = _grad_of(grads, norm.bias) if norm is not None else _grad_of(grads, conv.bias)
-            dz = ops.bn_act_bwd(da.contiguous(), z, scale, shift, self.act, mode, mean, invstd, dgamma, dbeta)
+            dz = sync_bn.bn_act_bwd(da.contiguous(), z, scale, shift, self.act, mode, mean, invstd, dgamma, dbeta, sync)
         gw = _grad_of(grads, conv.weight)
         if self.kind == "pw":
             B, H, W, K = x.shape

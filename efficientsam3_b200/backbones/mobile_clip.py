@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .. import ops
+from .. import ops, sync_bn
 from ..nn_utils import NativePlanMixin, bn_scale_bias, cached_pack
 
 
@@ -264,10 +264,27 @@ def repmixer_bn_pack(blk: RepMixerBlock):
 
 
 def repmixer_bn_forward(blk: RepMixerBlock, x, B, L):
-    """The block's prologue with batch-statistics BatchNorm (updates its running buffers): (x1 fp32, u bf16, stats [8, C], pack)."""
+    """The block's prologue with batch-statistics BatchNorm (updates its running buffers): (x1 fp32, u bf16, stats [8, C], pack,
+    sync).  sync is None for per-rank statistics; when the block's SyncBatchNorms span several ranks (sync_bn.repmixer_sync_group)
+    the statistics are taken over every rank -- es3_repmixer_bn_fwd split at its two finalize points, each rank's (count, mean, M2)
+    all-gathered -- and sync = (exchange group, the group's token count) for the backward."""
     p = repmixer_bn_pack(blk)
-    x1, u, _, stats = ops.repmixer_bn_fwd(x, B, L, p["taps"], p["aff"], repmixer_bns(blk))
-    return x1, u, stats, p
+    bns = repmixer_bns(blk)
+    group = sync_bn.repmixer_sync_group(bns)
+    if group is None:
+        x1, u, _, stats = ops.repmixer_bn_fwd(x, B, L, p["taps"], p["aff"], bns)
+        return x1, u, stats, p, None
+    group = sync_bn.exchange_group(group, x.is_cuda)
+    C = x.shape[1]
+    fold = torch.empty((24, C), device=x.device, dtype=torch.float32)
+    stats = torch.empty((8, C), device=x.device, dtype=torch.float32)
+    taps, aff = p["taps"], p["aff"]
+    parts = sync_bn.all_gather_partials(ops.repmixer_bn_stats_partial(x, B, L, taps, fold, 0), group)     # x and c = dw(x)
+    total = ops.repmixer_bn_finalize_sync(parts, 0, taps, aff, bns, fold, stats)
+    parts = sync_bn.all_gather_partials(ops.repmixer_bn_stats_partial(x, B, L, taps, fold, 1), group)     # f = dw(x1)
+    ops.repmixer_bn_finalize_sync(parts, 1, taps, aff, bns, fold, stats)
+    x1, u = ops.repmixer(x, B, L, fold[:11], fold[11], fold[12:23], fold[23])
+    return x1, u, stats, p, (group, total)
 
 
 def invalidate_running_folds(enc: "MobileCLIPTextTransformer"):
@@ -286,7 +303,7 @@ def run_layers(layers, x, B, L, causal, bn_blocks=None):
     for i, lp in enumerate(layers):
         if lp["kind"] == "repmixer":
             if bn_blocks is not None:
-                x1, u, _, _ = repmixer_bn_forward(bn_blocks[i], x, B, L)
+                x1, u, _, _, _ = repmixer_bn_forward(bn_blocks[i], x, B, L)
             else:
                 x1, u = ops.repmixer(x, B, L, lp["wm"], lp["bm"], lp["wf"], lp["bf"])
             h = ops.gemm(u, lp["fc1"][0], bias=lp["fc1"][1], act="gelu")
@@ -372,6 +389,10 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
         rejects a mixed train / eval state before this is consulted)."""
         return self.batch_stat_bn and any(m.training for b in self.transformer if isinstance(b, RepMixerBlock)
                                           for m in repmixer_bns(b))
+
+    def batch_stat_synced(self) -> bool:
+        """True when the RepMixerBlocks' batch statistics are taken over several ranks (SyncBatchNorm, sync_bn.sync_group)."""
+        return any(sync_bn.repmixer_sync_group(repmixer_bns(b)) is not None for b in self.transformer if isinstance(b, RepMixerBlock))
 
     def resize_pos_embed(self, new_length: int):
         """mobile_clip.py:709-724: truncates the table (a new Parameter) when new_length is shorter; never grows it."""
@@ -478,8 +499,9 @@ def _grad_of(grads, p):
 def check_trainable(module: nn.Module, enc: "MobileCLIPTextTransformer", what: str):
     """The raise paths of the training graph: S0-style RepMixerBlocks with a BatchNorm in train mode unless batch statistics were
     enabled (then: a mixed train / eval state, momentum=None, track_running_stats=False), strict precision, CPU modules,
-    dropout > 0."""
-    bns = [m for b in enc.transformer if isinstance(b, RepMixerBlock) for m in b.modules() if isinstance(m, nn.BatchNorm2d)]
+    dropout > 0.  nn.SyncBatchNorm (convert_sync_batchnorm) is a _BatchNorm but not a BatchNorm2d: both follow the same rules."""
+    bns = [m for b in enc.transformer if isinstance(b, RepMixerBlock) for m in b.modules()
+           if isinstance(m, nn.modules.batchnorm._BatchNorm)]
     if any(m.training for m in bns):
         if not enc.batch_stat_bn:
             raise NotImplementedError(f"{what}: the RepMixerBlocks of MobileCLIP-S0 train with frozen BatchNorm (running "
@@ -495,6 +517,9 @@ def check_trainable(module: nn.Module, enc: "MobileCLIPTextTransformer", what: s
                                           "batch-statistics BatchNorm")
             if not m.track_running_stats or m.running_mean is None:
                 raise NotImplementedError(f"{what}: batch-statistics BatchNorm is built with track_running_stats=True only")
+        for b in enc.transformer:
+            if isinstance(b, RepMixerBlock):
+                sync_bn.repmixer_sync_group(repmixer_bns(b))     # raises when a block's BNs disagree on their process group
     if ops.precision() == "strict":
         raise NotImplementedError(f"{what}: the strict (fp32) precision mode is not built for the text encoders")
     for m in module.modules():
@@ -695,15 +720,15 @@ class RepMixerBatchStatUnit(RepMixerUnit):
         self.enc = enc
 
     def forward(self, x, B, L):
-        x1, u, stats, p = repmixer_bn_forward(self.blk, x, B, L)
+        x1, u, stats, p, sync = repmixer_bn_forward(self.blk, x, B, L)
         invalidate_running_folds(self.enc)
         h = self.fc1.forward(u)
         x2 = ops.gemm(h, self.fc2._w(), scale=p["lsb"], bias=p["b2s"], residual=x1, out_dtype=torch.float32)
-        self.saved = (x, x1, h, p, stats, B, L)
+        self.saved = (x, x1, h, p, stats, sync, B, L)
         return x2
 
     def backward(self, g, gb, grads, want_bf16=True):
-        x, x1, h, p, stats, B, L = self.saved
+        x, x1, h, p, stats, sync, B, L = self.saved
         self.saved = None
         tm, ffn = self.tm, self.ffn
         y = ops.gemm(h, self.fc2._w(), bias=p["b2"], out_dtype=torch.float32)
@@ -714,12 +739,23 @@ class RepMixerBatchStatUnit(RepMixerUnit):
             ops.wgrad_pw(dy, h, gw2)
         du = self.fc1.backward(ops.gemm(dy, self.fc2._wt()), grads, out_dtype=torch.float32)
         bnf = ffn.conv.bn
-        e = ops.repmixer_bn_ffn_bwd(x1, du, g, p["taps"], p["aff"], stats, B, L, dtaps=_grad_of(grads, ffn.conv.conv.weight),
-                                    dgamma=_grad_of(grads, bnf.weight), dbeta=_grad_of(grads, bnf.bias))
         bns = repmixer_bns(self.blk)[:3]
-        return ops.repmixer_bn_tm_bwd(x, e, p["taps"], p["aff"], stats, B, L,
-                                      dtaps=_grad_of(grads, tm.mixer.rbr_conv[0].conv.weight), dls=_grad_of(grads, tm.layer_scale),
-                                      dbn=[_grad_of(grads, t) for bn in bns for t in (bn.weight, bn.bias)], want_bf16=want_bf16)
+        dbn = [_grad_of(grads, t) for bn in bns for t in (bn.weight, bn.bias)]
+        d_ftaps, d_mtaps = _grad_of(grads, ffn.conv.conv.weight), _grad_of(grads, tm.mixer.rbr_conv[0].conv.weight)
+        if sync is None:
+            e = ops.repmixer_bn_ffn_bwd(x1, du, g, p["taps"], p["aff"], stats, B, L, dtaps=d_ftaps, dgamma=_grad_of(grads, bnf.weight),
+                                        dbeta=_grad_of(grads, bnf.bias))
+            return ops.repmixer_bn_tm_bwd(x, e, p["taps"], p["aff"], stats, B, L, dtaps=d_mtaps, dls=_grad_of(grads, tm.layer_scale),
+                                          dbn=dbn, want_bf16=want_bf16)
+        # synchronised: each BN sum is all-gathered and added in rank order; the BNs' gamma / beta gradients stay this rank's own
+        group, total = sync
+        sums = ops.repmixer_bn_ffn_sums(x1, du, p["taps"], stats, B, L, p["aff"], dgamma=_grad_of(grads, bnf.weight),
+                                        dbeta=_grad_of(grads, bnf.bias))
+        e = ops.repmixer_bn_ffn_apply(x1, du, g, p["taps"], p["aff"], stats, sync_bn.all_gather_partials(sums, group), total, B, L,
+                                      dtaps=d_ftaps)
+        sums = ops.repmixer_bn_tm_sums(x, e, p["taps"], p["aff"], stats, B, L, dbn=dbn)
+        return ops.repmixer_bn_tm_apply(x, e, p["taps"], p["aff"], stats, sync_bn.all_gather_partials(sums, group), total, B, L,
+                                        dtaps=d_mtaps, dls=_grad_of(grads, tm.layer_scale), want_bf16=want_bf16)
 
 
 class TextEmbedUnit:

@@ -24,7 +24,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, sync_bn
 from ..nn_utils import dw_weight
 from .efficientvit_train import ConvUnit, _grad_of
 from .repvit import Conv2d_BN, RepViTBlock, SqueezeExcite
@@ -37,17 +37,17 @@ def _cu(cb: Conv2d_BN, act, kind) -> ConvUnit:
 
 
 def _norm_params(norm: nn.BatchNorm2d, z):
-    """(mean, invstd, scale, shift, mode) of a BatchNorm2d over z: batch statistics (+ running-stat update) in .train(),
-    running statistics when the module was frozen with .eval() (set_bn_state)."""
+    """(mean, invstd, scale, shift, mode, sync) of a BatchNorm2d over z: batch statistics (+ running-stat update) in .train(),
+    synchronised over the process group of an nn.SyncBatchNorm (sync: see sync_bn.batch_stats, None otherwise); running
+    statistics when the module was frozen with .eval() (set_bn_state)."""
     if norm.training:
-        mean, invstd, scale, shift = ops.bn_stats(z, norm.weight.detach(), norm.bias.detach(), norm.eps, norm.momentum,
-                                                  norm.running_mean, norm.running_var, norm.num_batches_tracked)
-        return mean, invstd, scale, shift, "batch"
+        mean, invstd, scale, shift, sync = sync_bn.batch_stats(norm, z)
+        return mean, invstd, scale, shift, "batch", sync
     mean = norm.running_mean.detach().float().contiguous()
     invstd = torch.rsqrt(norm.running_var.detach().float() + norm.eps).contiguous()
     scale = (norm.weight.detach().float() * invstd).contiguous()
     shift = (norm.bias.detach().float() - mean * scale).contiguous()
-    return mean, invstd, scale, shift, "eval"
+    return mean, invstd, scale, shift, "eval", None
 
 
 def _colsum_grads(d, z, dprod, dsum):
@@ -138,25 +138,26 @@ class RepVGGDWUnit:
         C = x.shape[-1]
         w3 = dw_weight(rv.conv.c, None)                                          # [9, C] fp32
         z1 = ops.dwconv(x, w3, None, 3, 1, None)
-        mean1, invstd1, scale1, shift1, mode1 = _norm_params(rv.conv.bn, z1)
+        n1 = _norm_params(rv.conv.bn, z1)
+        mean1, invstd1, scale1, shift1, mode1, sync1 = n1
         sb = (rv.conv1.weight.detach().float().reshape(C) + 1.0).contiguous()    # dw1x1 weight + the identity branch
         tb = (shift1 + rv.conv1.bias.detach().float()).contiguous()
         tmp = ops.affine_act(x, sb, tb, None)
         u = ops.affine_act(z1, scale1, None, None, residual=tmp)
-        mean_o, invstd_o, scale_o, shift_o, mode_o = _norm_params(rv.bn, u)
-        self.saved = (x, z1, u, w3, sb, (mean1, invstd1, scale1, shift1, mode1), (mean_o, invstd_o, scale_o, shift_o, mode_o))
-        return ops.affine_act(u, scale_o, shift_o, None)
+        no = _norm_params(rv.bn, u)
+        self.saved = (x, z1, u, w3, sb, n1, no)
+        return ops.affine_act(u, no[2], no[3], None)
 
     def backward(self, dy, grads):
         rv = self.rv
         x, z1, u, w3, sb, n1, no = self.saved
         self.saved = None
-        mean1, invstd1, scale1, shift1, mode1 = n1
-        mean_o, invstd_o, scale_o, shift_o, mode_o = no
-        du = ops.bn_act_bwd(dy.contiguous(), u, scale_o, shift_o, None, mode_o, mean_o, invstd_o,
-                            _grad_of(grads, rv.bn.weight), _grad_of(grads, rv.bn.bias))
-        dz1 = ops.bn_act_bwd(du, z1, scale1, shift1, None, mode1, mean1, invstd1,
-                             _grad_of(grads, rv.conv.bn.weight), _grad_of(grads, rv.conv.bn.bias))
+        mean1, invstd1, scale1, shift1, mode1, sync1 = n1
+        mean_o, invstd_o, scale_o, shift_o, mode_o, sync_o = no
+        du = sync_bn.bn_act_bwd(dy.contiguous(), u, scale_o, shift_o, None, mode_o, mean_o, invstd_o,
+                                _grad_of(grads, rv.bn.weight), _grad_of(grads, rv.bn.bias), sync_o)
+        dz1 = sync_bn.bn_act_bwd(du, z1, scale1, shift1, None, mode1, mean1, invstd1,
+                                 _grad_of(grads, rv.conv.bn.weight), _grad_of(grads, rv.conv.bn.bias), sync1)
         g_w1, g_b1 = _grad_of(grads, rv.conv1.weight), _grad_of(grads, rv.conv1.bias)
         if g_w1 is not None or g_b1 is not None:
             _colsum_grads(du, x, g_w1.view(-1) if g_w1 is not None else None, g_b1)
@@ -233,9 +234,10 @@ class PaddedStemUnit:
         w27[:, :c] = conv.weight.detach().float().reshape(c, 27).t()
         z = ops.stem_conv3x3_s2(x, w27, None, None)                              # [B,Ho,Wo,P], extra channels = 0
         gamma, beta = self._pad(bn.weight, 1.0), self._pad(bn.bias, 0.0)
+        sync = None
         if bn.training:
             rm, rv = self._pad(bn.running_mean, 0.0), self._pad(bn.running_var, 1.0)
-            mean, invstd, scale, shift = ops.bn_stats(z, gamma, beta, bn.eps, bn.momentum, rm, rv, bn.num_batches_tracked)
+            mean, invstd, scale, shift, sync = sync_bn.batch_stats(bn, z, gamma, beta, rm, rv)
             bn.running_mean.copy_(rm[:c])
             bn.running_var.copy_(rv[:c])
             mode = "batch"
@@ -245,16 +247,16 @@ class PaddedStemUnit:
             scale = (gamma * invstd).contiguous()
             shift = (beta - mean * scale).contiguous()
             mode = "eval"
-        self.saved = (x, z, scale, shift, mean, invstd, mode)
+        self.saved = (x, z, scale, shift, mean, invstd, mode, sync)
         return ops.affine_act(z, scale, shift, "gelu")
 
     def backward(self, da, grads):
-        x, z, scale, shift, mean, invstd, mode = self.saved
+        x, z, scale, shift, mean, invstd, mode, sync = self.saved
         self.saved = None
         conv, bn, c, p = self.conv, self.bn, self.c, self.p
         dev = z.device
         dg, db = torch.zeros(p, device=dev, dtype=torch.float32), torch.zeros(p, device=dev, dtype=torch.float32)
-        dz = ops.bn_act_bwd(da.contiguous(), z, scale, shift, "gelu", mode, mean, invstd, dg, db)
+        dz = sync_bn.bn_act_bwd(da.contiguous(), z, scale, shift, "gelu", mode, mean, invstd, dg, db, sync)
         g_w, g_b = _grad_of(grads, bn.weight), _grad_of(grads, bn.bias)
         if g_w is not None:
             g_w += dg[:c]
@@ -307,18 +309,19 @@ class PatchEmbedUnit:
         w9[:, :, :cin] = conv.weight.detach().permute(2, 3, 0, 1).reshape(9, cout, cin).to(torch.bfloat16)
         ones = torch.ones(cout, device=a0.device, dtype=torch.float32)
         z = ops.conv3x3_s2_narrow(a0, w9, ones, torch.zeros_like(ones), None)    # raw conv
-        mean, invstd, scale, shift, mode = _norm_params(bn, z)
-        self.saved = (a0, z, w9, (mean, invstd, scale, shift, mode))
+        mean, invstd, scale, shift, mode, sync = _norm_params(bn, z)
+        self.saved = (a0, z, w9, (mean, invstd, scale, shift, mode, sync))
         return ops.affine_act(z, scale, shift, None)
 
     def backward(self, dy, grads):
-        a0, z, w9, (mean, invstd, scale, shift, mode) = self.saved
+        a0, z, w9, (mean, invstd, scale, shift, mode, sync) = self.saved
         self.saved = None
         conv, bn = self.cb1.c, self.cb1.bn
         cout, cin_true = conv.out_channels, conv.in_channels
         B, H, W, cin = a0.shape                                                  # cin = padded width of the staged input
         Ho, Wo = H // 2, W // 2
-        dz = ops.bn_act_bwd(dy.contiguous(), z, scale, shift, None, mode, mean, invstd, _grad_of(grads, bn.weight), _grad_of(grads, bn.bias))
+        dz = sync_bn.bn_act_bwd(dy.contiguous(), z, scale, shift, None, mode, mean, invstd, _grad_of(grads, bn.weight),
+                                _grad_of(grads, bn.bias), sync)
         dz2 = dz.view(-1, cout)
         # weight gradient: tap (ky, kx) reads phase (py, px) of a0 at a stride-1 shift
         gw_true = _grad_of(grads, conv.weight)

@@ -154,17 +154,10 @@ __device__ float bn_update(const BnRun& r, int ch, double mean, double var, doub
   return (float)(1.0 / sqrt(var + (double)r.eps));
 }
 
-// One thread per channel.  MODE 0: BN_ms, BN_ns (statistics of x) and BN_mc (of c); writes wm, bm.  MODE 1: BN_f; writes wf, bf.
-template <int MODE>
-__global__ void repmixer_bn_finalize_kernel(const float* __restrict__ part, int B, int L, int C, BnFinalize f) {
-  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-  if (ch >= C) return;
-  const double M = (double)B * L;
+// BN_ms, BN_ns (statistics of x: mx, vx) and BN_mc (of c: mc, vc) over M values: running buffers, stats, folded wm, bm.
+__device__ void finalize_xc(const BnFinalize& f, int ch, int C, double mx, double vx, double mc, double vc, double M) {
   const float* aff = f.aff;
-  if constexpr (MODE == 0) {
-    double mx, vx, mc, vc;
-    combine(part, BS_Q_XC, 0, B, L, C, ch, mx, vx);
-    combine(part, BS_Q_XC, 3, B, L, C, ch, mc, vc);
+  {
     const float i_ms = bn_update(f.bn[0], ch, mx, vx, M), i_mc = bn_update(f.bn[1], ch, mc, vc, M);
     const float i_ns = bn_update(f.bn[2], ch, mx, vx, M);
     const float fmx = (float)mx, fmc = (float)mc;
@@ -184,9 +177,13 @@ __global__ void repmixer_bn_finalize_kernel(const float* __restrict__ part, int 
       f.fold[k * C + ch] = wk;
     }
     f.fold[BS_KS * C + ch] = ls * (b_ms + b_mc - b_ns);
-  } else {
-    double mf, vf;
-    combine(part, BS_Q_F, 0, B, L, C, ch, mf, vf);
+  }
+}
+
+// BN_f (statistics of f: mf, vf) over M values: running buffers, stats, folded wf, bf.
+__device__ void finalize_f(const BnFinalize& f, int ch, int C, double mf, double vf, double M) {
+  const float* aff = f.aff;
+  {
     const float i_f = bn_update(f.bn[3], ch, mf, vf, M), fmf = (float)mf;
     f.stats[S_M_F * C + ch] = fmf;
     f.stats[S_I_F * C + ch] = i_f;
@@ -195,6 +192,77 @@ __global__ void repmixer_bn_finalize_kernel(const float* __restrict__ part, int 
     for (int k = 0; k < BS_KS; ++k) f.fold[(BS_KS + 1 + k) * C + ch] = f.taps[(BS_KS + k) * C + ch] * s_f;
     f.fold[(2 * BS_KS + 1) * C + ch] = aff[A_B_F * C + ch] - fmf * s_f;
   }
+}
+
+// One thread per channel.  MODE 0: BN_ms, BN_ns (statistics of x) and BN_mc (of c); writes wm, bm.  MODE 1: BN_f; writes wf, bf.
+template <int MODE>
+__global__ void repmixer_bn_finalize_kernel(const float* __restrict__ part, int B, int L, int C, BnFinalize f) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= C) return;
+  const double M = (double)B * L;
+  if constexpr (MODE == 0) {
+    double mx, vx, mc, vc;
+    combine(part, BS_Q_XC, 0, B, L, C, ch, mx, vx);
+    combine(part, BS_Q_XC, 3, B, L, C, ch, mc, vc);
+    finalize_xc(f, ch, C, mx, vx, mc, vc, M);
+  } else {
+    double mf, vf;
+    combine(part, BS_Q_F, 0, B, L, C, ch, mf, vf);
+    finalize_f(f, ch, C, mf, vf, M);
+  }
+}
+
+// Synchronised BatchNorm (SyncBatchNorm over several ranks).  This rank's (count, mean, M2) of each value, fp64 out [NV][3][C]
+// (MODE 0: x, c; MODE 1: f), from the per-sequence partials of repmixer_bn_stats_kernel<MODE>.
+template <int MODE>
+__global__ void repmixer_bn_local_kernel(const float* __restrict__ part, int B, int L, int C, double* __restrict__ out) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= C) return;
+  constexpr int NV = MODE == 0 ? 2 : 1, Q = MODE == 0 ? BS_Q_XC : BS_Q_F;
+  const double M = (double)B * L;
+#pragma unroll
+  for (int v = 0; v < NV; ++v) {
+    double mean, var;
+    combine(part, Q, 3 * v, B, L, C, ch, mean, var);
+    out[(v * 3) * C + ch] = M;
+    out[(v * 3 + 1) * C + ch] = mean;
+    out[(v * 3 + 2) * C + ch] = var * M;
+  }
+}
+
+// Chan's combination of value v over the W ranks' [W][NV][3][C] partials, in rank order.
+__device__ void chan_ranks(const double* __restrict__ parts, int W, int NV, int v, int C, int ch, double& n, double& mean, double& var) {
+  n = 0.0; mean = 0.0;
+  double m2 = 0.0;
+  for (int w = 0; w < W; ++w) {
+    const double* p = parts + ((long long)w * NV + v) * 3 * C + ch;
+    const double nb = p[0];
+    if (nb <= 0.0) continue;
+    const double nn = n + nb, d = p[C] - mean;
+    mean += d * (nb / nn);
+    m2 += p[2 * C] + d * d * (n * nb / nn);
+    n = nn;
+  }
+  var = n > 0.0 ? fmax(m2 / n, 0.0) : 0.0;
+}
+
+// The finalize of repmixer_bn_finalize_kernel<MODE> on every rank's partials; total [1] = the count over the group.
+template <int MODE>
+__global__ void repmixer_bn_finalize_sync_kernel(const double* __restrict__ parts, int W, int C, BnFinalize f, double* __restrict__ total) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= C) return;
+  double n;
+  if constexpr (MODE == 0) {
+    double mx, vx, mc, vc;
+    chan_ranks(parts, W, 2, 0, C, ch, n, mx, vx);
+    chan_ranks(parts, W, 2, 1, C, ch, n, mc, vc);
+    finalize_xc(f, ch, C, mx, vx, mc, vc, n);
+  } else {
+    double mf, vf;
+    chan_ranks(parts, W, 1, 0, C, ch, n, mf, vf);
+    finalize_f(f, ch, C, mf, vf, n);
+  }
+  if (ch == 0 && total != nullptr) total[0] = n;
 }
 
 // ConvFFN sums pass: sum du and sum du fhat (BN_f's beta / gamma gradients), fhat = (dw(x1; w_f) - mean_f) invstd_f.
@@ -224,8 +292,9 @@ __global__ void __launch_bounds__(BS_THREADS) repmixer_bn_ffn_sums_kernel(const 
 __global__ void __launch_bounds__(BS_THREADS) repmixer_bn_ffn_apply_kernel(const float* __restrict__ x1, const float* __restrict__ du,
                                                                            const float* __restrict__ g, const float* __restrict__ taps,
                                                                            const float* __restrict__ aff, const float* __restrict__ stats,
-                                                                           const float* __restrict__ sums, float* __restrict__ e,
-                                                                           float* __restrict__ part, int B, int L, int C) {
+                                                                           const float* __restrict__ sums, const double* __restrict__ total,
+                                                                           float* __restrict__ e, float* __restrict__ part, int B, int L,
+                                                                           int C) {
   __shared__ float sx1[BS_PAD * BS_CH];
   __shared__ float sdf[BS_PAD * BS_CH];
   const int c = threadIdx.x % BS_CH, r0 = threadIdx.x / BS_CH;
@@ -238,7 +307,8 @@ __global__ void __launch_bounds__(BS_THREADS) repmixer_bn_ffn_apply_kernel(const
 #pragma unroll
   for (int k = 0; k < BS_KS; ++k) w[k] = taps[(BS_KS + k) * C + ch];
   const float mf = stats[S_M_F * C + ch], inv = stats[S_I_F * C + ch], s_f = aff[A_G_F * C + ch] * inv;
-  const float rM = 1.f / ((float)B * (float)L), m0 = sums[ch] * rM, m1 = sums[C + ch] * rM;
+  // total: the count over every rank when synchronised, else this batch's B L
+  const float rM = total ? (float)(1.0 / total[0]) : 1.f / ((float)B * (float)L), m0 = sums[ch] * rM, m1 = sums[C + ch] * rM;
   float v[BS_Q_FFN];
 #pragma unroll
   for (int q = 0; q < BS_Q_FFN; ++q) v[q] = 0.f;
@@ -292,7 +362,8 @@ __global__ void __launch_bounds__(BS_THREADS) repmixer_bn_tm_sums_kernel(const f
 __global__ void __launch_bounds__(BS_THREADS) repmixer_bn_tm_apply_kernel(const float* __restrict__ x, const float* __restrict__ e,
                                                                           const float* __restrict__ taps, const float* __restrict__ aff,
                                                                           const float* __restrict__ stats, const float* __restrict__ sums,
-                                                                          float* __restrict__ dx, bf16* __restrict__ dxb,
+                                                                          const double* __restrict__ total, float* __restrict__ dx,
+                                                                          bf16* __restrict__ dxb,
                                                                           float* __restrict__ part, int B, int L, int C) {
   __shared__ float sx[BS_PAD * BS_CH];
   __shared__ float sdc[BS_PAD * BS_CH];
@@ -310,7 +381,8 @@ __global__ void __launch_bounds__(BS_THREADS) repmixer_bn_tm_apply_kernel(const 
   const float g_ms = aff[A_G_MS * C + ch], g_mc = aff[A_G_MC * C + ch], g_ns = aff[A_G_NS * C + ch];
   const float s_ms = g_ms * i_ms, s_mc = g_mc * i_mc, s_ns = g_ns * i_ns;
   const float br = aff[A_B_MS * C + ch] + aff[A_B_MC * C + ch] - aff[A_B_NS * C + ch];
-  const float rM = 1.f / ((float)B * (float)L), m0 = sums[ch] * rM, m1 = sums[C + ch] * rM, m2 = sums[2 * C + ch] * rM;
+  const float rM = total ? (float)(1.0 / total[0]) : 1.f / ((float)B * (float)L);
+  const float m0 = sums[ch] * rM, m1 = sums[C + ch] * rM, m2 = sums[2 * C + ch] * rM;
   const float k_ms = s_ms * i_ms * i_ms * m2, k_ns = s_ns * i_ns * i_ns * m2;     // xhat i S2 / M, per unit (x - mean)
   float v[BS_Q_TM];
 #pragma unroll
@@ -470,7 +542,7 @@ extern "C" int es3_repmixer_bn_ffn_bwd(const float* x1, const float* du, const f
   db.add(1, dgamma);
   repmixer_bn_sums_kernel<2><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, C, sums, db.d);
   ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<ffn>");
-  repmixer_bn_ffn_apply_kernel<<<grid, BS_THREADS, 0, st>>>(x1, du, g, taps, aff, stats, sums, e, ws, B, L, C);
+  repmixer_bn_ffn_apply_kernel<<<grid, BS_THREADS, 0, st>>>(x1, du, g, taps, aff, stats, sums, nullptr, e, ws, B, L, C);
   ES3_LAUNCH_CHECK("repmixer_bn_ffn_apply_kernel");
   return launch_grad_sums(ws, BS_Q_FFN, dwf, nullptr, B, C, st);
 }
@@ -495,7 +567,127 @@ extern "C" int es3_repmixer_bn_tm_bwd(const float* x, const float* e, const floa
   db.add(2, dg_ns, -1.f, stats + S_I_NS * C);
   repmixer_bn_sums_kernel<3><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, C, sums, db.d);
   ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<tm>");
-  repmixer_bn_tm_apply_kernel<<<grid, BS_THREADS, 0, st>>>(x, e, taps, aff, stats, sums, dx, (bf16*)dxb, ws, B, L, C);
+  repmixer_bn_tm_apply_kernel<<<grid, BS_THREADS, 0, st>>>(x, e, taps, aff, stats, sums, nullptr, dx, (bf16*)dxb, ws, B, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_tm_apply_kernel");
+  return launch_grad_sums(ws, BS_Q_TM, dwmc, dls, B, C, st);
+}
+
+// ------------------------------------------------------------------------------------------ synchronised BatchNorm
+// nn.SyncBatchNorm over several ranks: the forward above split at its two finalize points, the backward at its two sums.  Every
+// rank all-gathers the partials (fp64 (count, mean, M2) forward, fp32 sums backward) and combines them in rank order, so the
+// statistics and running buffers are bit-identical on every rank.  One rank's batch may hold a single token: only the count over the
+// group matters, and with two or more ranks it is >= 2.
+#define BS_CHECK_SHAPE_SYNC(fn)                                                                                                \
+  ES3_REQUIRE(L >= 1 && L <= BS_MAXL, fn ": sequence length %d outside 1..%d (the sequence is kept in shared memory)", L,  \
+              BS_MAXL);                                                                                                        \
+  ES3_REQUIRE(B >= 1 && C >= BS_CH && C % BS_CH == 0, fn ": need B >= 1 and C %% %d == 0 (B=%d C=%d)", BS_CH, B, C)
+
+/* mode 0: part [2][3][C] = (count, mean, M2) of x and c = dw(x; w_mc); mode 1: part [1][3][C] of f = dw(x1; w_f), x1 from
+ * fold's wm, bm (es3_repmixer_bn_finalize_sync mode 0).  ws: es3_repmixer_bn_ws_floats(B, C). */
+extern "C" int es3_repmixer_bn_stats_partial(const float* x, const float* taps, const float* fold, int mode, float* ws, double* part,
+                                             int B, int L, int C, void* stream) {
+  BS_CHECK_SHAPE_SYNC("es3_repmixer_bn_stats_partial");
+  ES3_REQUIRE(mode == 0 || mode == 1, "es3_repmixer_bn_stats_partial: mode %d", mode);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid(C / BS_CH, B);
+  if (mode == 0) {
+    repmixer_bn_stats_kernel<0><<<grid, BS_THREADS, 0, st>>>(x, taps, fold, ws, L, C);
+    ES3_LAUNCH_CHECK("repmixer_bn_stats_kernel<xc>");
+    repmixer_bn_local_kernel<0><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, L, C, part);
+  } else {
+    repmixer_bn_stats_kernel<1><<<grid, BS_THREADS, 0, st>>>(x, taps, fold, ws, L, C);
+    ES3_LAUNCH_CHECK("repmixer_bn_stats_kernel<f>");
+    repmixer_bn_local_kernel<1><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, L, C, part);
+  }
+  ES3_LAUNCH_CHECK("repmixer_bn_local_kernel");
+  return 0;
+}
+
+/* parts [W][2 | 1][3][C] (every rank's es3_repmixer_bn_stats_partial, rank order) -> as es3_repmixer_bn_fwd's finalize mode 0 | 1:
+ * running buffers over the total count, num_batches_tracked, stats and fold rows; total [1] = the count over the group. */
+extern "C" int es3_repmixer_bn_finalize_sync(const double* parts, int W, int mode, const float* taps, const float* aff, float* rm_ms,
+                                             float* rv_ms, long long* nbt_ms, float* rm_mc, float* rv_mc, long long* nbt_mc, float* rm_ns,
+                                             float* rv_ns, long long* nbt_ns, float* rm_f, float* rv_f, long long* nbt_f, float eps_ms,
+                                             float eps_mc, float eps_ns, float eps_f, float mom_ms, float mom_mc, float mom_ns,
+                                             float mom_f, float* fold, float* stats, double* total, int C, void* stream) {
+  ES3_REQUIRE(W >= 1 && C >= BS_CH && C % BS_CH == 0, "es3_repmixer_bn_finalize_sync: need W >= 1 and C %% %d == 0", BS_CH);
+  ES3_REQUIRE(mode == 0 || mode == 1, "es3_repmixer_bn_finalize_sync: mode %d", mode);
+  cudaStream_t st = (cudaStream_t)stream;
+  BnFinalize f;
+  f.bn[0] = BnRun{rm_ms, rv_ms, nbt_ms, eps_ms, mom_ms};
+  f.bn[1] = BnRun{rm_mc, rv_mc, nbt_mc, eps_mc, mom_mc};
+  f.bn[2] = BnRun{rm_ns, rv_ns, nbt_ns, eps_ns, mom_ns};
+  f.bn[3] = BnRun{rm_f, rv_f, nbt_f, eps_f, mom_f};
+  f.taps = taps; f.aff = aff; f.fold = fold; f.stats = stats;
+  if (mode == 0)
+    repmixer_bn_finalize_sync_kernel<0><<<ceil_div(C, 128), 128, 0, st>>>(parts, W, C, f, total);
+  else
+    repmixer_bn_finalize_sync_kernel<1><<<ceil_div(C, 128), 128, 0, st>>>(parts, W, C, f, total);
+  ES3_LAUNCH_CHECK("repmixer_bn_finalize_sync_kernel");
+  return 0;
+}
+
+/* ConvFFN backward, first half: this rank's sums [2][C] (sum du, sum du fhat) and its BN_f dgamma / dbeta (+=, may be null). */
+extern "C" int es3_repmixer_bn_ffn_sums(const float* x1, const float* du, const float* taps, const float* stats, float* ws, float* sums,
+                                        float* dgamma, float* dbeta, int B, int L, int C, void* stream) {
+  BS_CHECK_SHAPE_SYNC("es3_repmixer_bn_ffn_sums");
+  cudaStream_t st = (cudaStream_t)stream;
+  repmixer_bn_ffn_sums_kernel<<<dim3(C / BS_CH, B), BS_THREADS, 0, st>>>(x1, du, taps, stats, ws, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_ffn_sums_kernel");
+  DstBuilder db;
+  db.add(0, dbeta);
+  db.add(1, dgamma);
+  repmixer_bn_sums_kernel<2><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, C, sums, db.d);
+  ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<ffn>");
+  return 0;
+}
+
+/* ConvFFN backward, second half: parts [W][2][C] (every rank's sums, rank order) and the total count -> e, dwf (+=). */
+extern "C" int es3_repmixer_bn_ffn_apply(const float* x1, const float* du, const float* g, const float* taps, const float* aff,
+                                         const float* stats, const float* parts, int W, const double* total, float* e, float* ws,
+                                         float* dwf, int B, int L, int C, void* stream) {
+  BS_CHECK_SHAPE_SYNC("es3_repmixer_bn_ffn_apply");
+  ES3_REQUIRE(W >= 1 && parts && total, "es3_repmixer_bn_ffn_apply: need W >= 1, parts and total");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* sums = ws + (long long)B * BS_Q_MAX * C;
+  repmixer_bn_sums_kernel<2><<<ceil_div(C, 128), 128, 0, st>>>(parts, W, C, sums, DstBuilder().d);
+  ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<ffn ranks>");
+  repmixer_bn_ffn_apply_kernel<<<dim3(C / BS_CH, B), BS_THREADS, 0, st>>>(x1, du, g, taps, aff, stats, sums, total, e, ws, B, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_ffn_apply_kernel");
+  return launch_grad_sums(ws, BS_Q_FFN, dwf, nullptr, B, C, st);
+}
+
+/* Token-mixer backward, first half: this rank's sums [3][C] and the gamma / beta gradients of BN_ms, BN_mc, BN_ns (+=, may be null). */
+extern "C" int es3_repmixer_bn_tm_sums(const float* x, const float* e, const float* taps, const float* aff, const float* stats, float* ws,
+                                       float* sums, float* dg_ms, float* db_ms, float* dg_mc, float* db_mc, float* dg_ns, float* db_ns,
+                                       int B, int L, int C, void* stream) {
+  BS_CHECK_SHAPE_SYNC("es3_repmixer_bn_tm_sums");
+  cudaStream_t st = (cudaStream_t)stream;
+  repmixer_bn_tm_sums_kernel<<<dim3(C / BS_CH, B), BS_THREADS, 0, st>>>(x, e, taps, aff, stats, ws, L, C);
+  ES3_LAUNCH_CHECK("repmixer_bn_tm_sums_kernel");
+  DstBuilder db;
+  db.add(0, db_ms);
+  db.add(0, db_mc);
+  db.add(0, db_ns, -1.f);
+  db.add(1, dg_mc);
+  db.add(2, dg_ms, 1.f, stats + S_I_MS * C);
+  db.add(2, dg_ns, -1.f, stats + S_I_NS * C);
+  repmixer_bn_sums_kernel<3><<<ceil_div(C, 128), 128, 0, st>>>(ws, B, C, sums, db.d);
+  ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<tm>");
+  return 0;
+}
+
+/* Token-mixer backward, second half: parts [W][3][C] and the total count -> dx (+ bf16 copy dxb, may be null), dwmc, dls (+=). */
+extern "C" int es3_repmixer_bn_tm_apply(const float* x, const float* e, const float* taps, const float* aff, const float* stats,
+                                        const float* parts, int W, const double* total, float* dx, void* dxb, float* ws, float* dwmc,
+                                        float* dls, int B, int L, int C, void* stream) {
+  BS_CHECK_SHAPE_SYNC("es3_repmixer_bn_tm_apply");
+  ES3_REQUIRE(W >= 1 && parts && total, "es3_repmixer_bn_tm_apply: need W >= 1, parts and total");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* sums = ws + (long long)B * BS_Q_MAX * C;
+  repmixer_bn_sums_kernel<3><<<ceil_div(C, 128), 128, 0, st>>>(parts, W, C, sums, DstBuilder().d);
+  ES3_LAUNCH_CHECK("repmixer_bn_sums_kernel<tm ranks>");
+  repmixer_bn_tm_apply_kernel<<<dim3(C / BS_CH, B), BS_THREADS, 0, st>>>(x, e, taps, aff, stats, sums, total, dx, (bf16*)dxb, ws, B, L, C);
   ES3_LAUNCH_CHECK("repmixer_bn_tm_apply_kernel");
   return launch_grad_sums(ws, BS_Q_TM, dwmc, dls, B, C, st);
 }

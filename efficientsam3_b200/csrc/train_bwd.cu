@@ -20,7 +20,7 @@
 //
 // Gradients of activations are bf16 (the reference's AMP path keeps them fp16), parameter gradients fp32 and ACCUMULATED
 // (+=) into their destination, all reductions are two-stage with a fixed order: no atomics, bit-reproducible.
-#include "common.cuh"
+#include "col_reduce.cuh"
 
 namespace es3 {
 namespace {
@@ -238,29 +238,7 @@ __global__ void __launch_bounds__(CR_THREADS, 3) col_reduce_ring_kernel(const bf
   }
 }
 
-// Second stage of the column reductions.  block 256 = 8 channels x 32 lanes: lane l adds partials l, l + 32, ... (double),
-// the 32 lanes are then summed in a fixed order.  (One thread per channel walking all <= 1184 partials serially cost
-// 35 + 54 launches per step.)
-__device__ __forceinline__ bool sum_block_partials(const float* __restrict__ part, int nblk, int C, double& s, double& q, int& c_out) {
-  __shared__ double r0[32][9], r1[32][9];
-  const int cl = threadIdx.x & 7, lane = threadIdx.x >> 3;
-  const int c = blockIdx.x * 8 + cl;
-  double a = 0.0, b = 0.0;
-  if (c < C) {
-    for (int blk = lane; blk < nblk; blk += 32) {
-      a += (double)part[((long long)blk * 2) * C + c];
-      b += (double)part[((long long)blk * 2 + 1) * C + c];
-    }
-  }
-  r0[lane][cl] = a;
-  r1[lane][cl] = b;
-  __syncthreads();
-  c_out = c;
-  if (lane != 0 || c >= C) return false;
-  s = 0.0; q = 0.0;
-  for (int l = 0; l < 32; ++l) { s += r0[l][cl]; q += r1[l][cl]; }
-  return true;
-}
+// Second stage of the column reductions: sum_block_partials (col_reduce.cuh).
 
 // batch statistics, folded (scale, shift) for the normalise pass, running-stat update (nn.BatchNorm2d: momentum on the
 // UNBIASED variance).  grid ceil(C / 8), block 256.
@@ -1408,22 +1386,49 @@ static int elementwise_geometry(long long M, int C, int* CVB, int* nblk, long lo
   return 0;
 }
 
+int es3::col_reduce_partials(bool stats, int act, const void* z, const void* da, const float* scale, const float* shift,
+                              long long M, int C, float* ws, int* nblk_out, cudaStream_t st) {
+  int CVB, nblk, gy;
+  long long rpb;
+  col_reduce_geometry(M, C, &CVB, &nblk, &rpb, &gy);
+  *nblk_out = nblk;
+  const bool ring = col_reduce_use_ring();
+  if (stats) {
+    if (ring) {
+      constexpr int RING = CRR_STAGES * 1 * CR_THREADS * 16;
+      col_reduce_ring_kernel<ACT_NONE, true><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, nullptr, nullptr, nullptr, M, C, CVB, rpb, ws);
+    } else {
+      col_reduce_kernel<ACT_NONE, true><<<dim3(nblk, gy), CR_THREADS, 0, st>>>((const bf16*)z, nullptr, nullptr, nullptr, M, C, CVB, rpb, ws);
+    }
+    ES3_LAUNCH_CHECK("col_reduce_kernel<stats>");
+    return 0;
+  }
+  ES3_DISPATCH_ACT_BWD(act, A, {
+    if (ring) {
+      constexpr int RING = CRR_STAGES * 2 * CR_THREADS * 16;                     // 48 KB: needs the opt-in above the default 48 KB with `red`
+      static bool configured = false;
+      if (!configured) {
+        ES3_CHECK_CUDA(cudaFuncSetAttribute(col_reduce_ring_kernel<A, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RING));
+        configured = true;
+      }
+      col_reduce_ring_kernel<A, false><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, (const bf16*)da, scale, shift, M, C, CVB, rpb, ws);
+    } else {
+      col_reduce_kernel<A, false><<<dim3(nblk, gy), CR_THREADS, 0, st>>>((const bf16*)z, (const bf16*)da, scale, shift, M, C, CVB, rpb, ws);
+    }
+  })
+  ES3_LAUNCH_CHECK("col_reduce_kernel<bwd>");
+  return 0;
+}
+
 extern "C" int es3_bn_stats(const void* z, long long M, int C, float eps, float momentum, const float* gamma, const float* beta,
                             float* ws, float* mean, float* invstd, float* scale, float* shift, float* running_mean,
                             float* running_var, long long* num_batches_tracked, void* stream) {
   ES3_REQUIRE(M > 0 && C > 0 && C % 8 == 0, "es3_bn_stats: need M > 0 and C %% 8 == 0 (M=%lld C=%d)", M, C);
   ES3_REQUIRE(((uintptr_t)z & 15) == 0, "es3_bn_stats: z must be 16-byte aligned");
-  int CVB, nblk, gy;
-  long long rpb;
-  col_reduce_geometry(M, C, &CVB, &nblk, &rpb, &gy);
   cudaStream_t st = (cudaStream_t)stream;
-  if (col_reduce_use_ring()) {
-    constexpr int RING = CRR_STAGES * 1 * CR_THREADS * 16;
-    col_reduce_ring_kernel<ACT_NONE, true><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, nullptr, nullptr, nullptr, M, C, CVB, rpb, ws);
-  } else {
-    col_reduce_kernel<ACT_NONE, true><<<dim3(nblk, gy), CR_THREADS, 0, st>>>((const bf16*)z, nullptr, nullptr, nullptr, M, C, CVB, rpb, ws);
-  }
-  ES3_LAUNCH_CHECK("col_reduce_kernel<stats>");
+  int nblk;
+  const int rc = col_reduce_partials(true, ACT_NONE, z, nullptr, nullptr, nullptr, M, C, ws, &nblk, st);
+  if (rc) return rc;
   bn_stats_finalize_kernel<<<ceil_div(C, 8), 256, 0, st>>>((const bf16*)z, ws, nblk, C, M, eps, momentum, gamma, beta, mean, invstd, scale, shift,
                                                             running_mean, running_var, num_batches_tracked);
   ES3_LAUNCH_CHECK("bn_stats_finalize_kernel");
@@ -1450,25 +1455,10 @@ extern "C" int es3_bn_act_bwd_reduce(const void* da, const void* z, const float*
   ES3_REQUIRE(M > 0 && C > 0 && C % 8 == 0, "es3_bn_act_bwd_reduce: need C %% 8 == 0 (C=%d)", C);
   ES3_REQUIRE(mode >= 0 && mode <= 2, "es3_bn_act_bwd_reduce: mode %d", mode);
   ES3_REQUIRE(mode == 0 || (mean && invstd), "es3_bn_act_bwd_reduce: BN modes need mean / invstd");
-  int CVB, nblk, gy;
-  long long rpb;
-  col_reduce_geometry(M, C, &CVB, &nblk, &rpb, &gy);
   cudaStream_t st = (cudaStream_t)stream;
-  const bool ring = col_reduce_use_ring();
-  ES3_DISPATCH_ACT_BWD(act, A, {
-    if (ring) {
-      constexpr int RING = CRR_STAGES * 2 * CR_THREADS * 16;                     // 48 KB: needs the opt-in above the default 48 KB with `red`
-      static bool configured = false;
-      if (!configured) {
-        ES3_CHECK_CUDA(cudaFuncSetAttribute(col_reduce_ring_kernel<A, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RING));
-        configured = true;
-      }
-      col_reduce_ring_kernel<A, false><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, (const bf16*)da, scale, shift, M, C, CVB, rpb, ws);
-    } else {
-      col_reduce_kernel<A, false><<<dim3(nblk, gy), CR_THREADS, 0, st>>>((const bf16*)z, (const bf16*)da, scale, shift, M, C, CVB, rpb, ws);
-    }
-  })
-  ES3_LAUNCH_CHECK("col_reduce_kernel<bwd>");
+  int nblk;
+  const int rc = col_reduce_partials(false, act, z, da, scale, shift, M, C, ws, &nblk, st);
+  if (rc) return rc;
   bn_bwd_finalize_kernel<<<ceil_div(C, 8), 256, 0, st>>>(ws, nblk, C, M, mode, scale, mean, invstd, coef, dgamma, dbeta);
   ES3_LAUNCH_CHECK("bn_bwd_finalize_kernel");
   return 0;

@@ -79,7 +79,8 @@ class TextStudentEncoder(nn.Module, NativePlanMixin):
         return self
 
     def _check_batch(self, ids):
-        if self.encoder.batch_stat_active() and ids.shape[0] * ids.shape[1] < 2:
+        # synchronised over several ranks, the count is over the group (>= 2): one token per rank is fine, as in SyncBatchNorm
+        if self.encoder.batch_stat_active() and ids.shape[0] * ids.shape[1] < 2 and not self.encoder.batch_stat_synced():
             raise ValueError("TextStudentEncoder: batch-statistics BatchNorm expects more than 1 value per channel when training "
                              f"(B*L = {ids.shape[0] * ids.shape[1]})")
 

@@ -679,6 +679,123 @@ def repmixer_bn_tm_bwd(x, e, taps, aff, stats, B, L, dtaps=None, dls=None, dbn=(
     return dx, dxb
 
 
+# RepMixerBlock with synchronised BatchNorm: the forward split at its finalize points, the backward at its sums (the ranks
+# all-gather what the *_partial / *_sums calls return, sync_bn.repmixer_*).  A rank may hold B*L == 1: only the group's count
+# matters, and with two or more ranks it is >= 2.
+KERNELS_PER_CALL.update({"es3_repmixer_bn_stats_partial": 2, "es3_repmixer_bn_ffn_sums": 2, "es3_repmixer_bn_tm_sums": 2,
+                         "es3_repmixer_bn_ffn_apply": 3, "es3_repmixer_bn_tm_apply": 3})
+
+
+def _running_ptrs(bns, C, name):
+    run = []
+    for bn in bns:
+        for t in (bn.running_mean, bn.running_var):
+            _chk(t, torch.float32, "running statistics")
+            if not (t.is_contiguous() and t.numel() == C):
+                raise ValueError(f"{name}: expected contiguous fp32 running statistics of {C} channels")
+        _chk(bn.num_batches_tracked, torch.int64, "num_batches_tracked")
+        run += [bn.running_mean.data_ptr(), bn.running_var.data_ptr(), bn.num_batches_tracked.data_ptr()]
+    return run
+
+
+def repmixer_bn_stats_partial(x, B, L, taps, fold, mode):
+    """This rank's (count, mean, M2) fp64: mode 0 [2, 3, C] of x and c = dw(x; w_mc), mode 1 [1, 3, C] of f = dw(x1; w_f) with x1
+    from fold's wm, bm (repmixer_bn_finalize_sync mode 0).  fold [24, C] fp32 (mode 0 does not read it)."""
+    C = x.shape[-1]
+    _repmixer_bwd_args("repmixer_bn_stats_partial", (x,), B, L, [(taps, (2, 11, C)), (fold, (24, C))])
+    part = torch.empty((2 if mode == 0 else 1, 3, C), device=x.device, dtype=torch.float64)
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
+    _call("es3_repmixer_bn_stats_partial", "repmixer_bn_stats_partial", _nb(x), 2 * 11 * x.numel(), x.data_ptr(), taps.data_ptr(),
+          fold.data_ptr(), int(mode), ws.data_ptr(), part.data_ptr(), B, L, C, _stream())
+    return part
+
+
+def repmixer_bn_finalize_sync(parts, mode, taps, aff, bns, fold, stats):
+    """parts [W, 2 | 1, 3, C] fp64, every rank's repmixer_bn_stats_partial in rank order.  Writes the mode's rows of fold [24, C] and
+    stats [8, C] (as repmixer_bn_fwd returns them), updates the BNs' running buffers over the group's count; returns that count
+    (one-element fp64)."""
+    nv = 2 if mode == 0 else 1
+    _chk(parts, torch.float64, "parts")
+    C = fold.shape[-1]
+    if not (parts.is_contiguous() and parts.dim() == 4 and parts.shape[1:] == (nv, 3, C)):
+        raise ValueError(f"repmixer_bn_finalize_sync: expected contiguous fp64 parts [W, {nv}, 3, {C}], got {tuple(parts.shape)}")
+    for t, shape, n in ((taps, (2, 11, C), "taps"), (aff, (9, C), "aff"), (fold, (24, C), "fold"), (stats, (8, C), "stats")):
+        _chk(t, torch.float32, n)
+        if not (t.is_contiguous() and tuple(t.shape) == shape):
+            raise ValueError(f"repmixer_bn_finalize_sync: expected contiguous {n} {shape}, got {tuple(t.shape)}")
+    run = _running_ptrs(bns, C, "repmixer_bn_finalize_sync")
+    total = torch.empty(1, device=parts.device, dtype=torch.float64)
+    _call("es3_repmixer_bn_finalize_sync", "repmixer_bn_finalize_sync", _nb(parts), 40 * parts.numel(), parts.data_ptr(),
+          parts.shape[0], int(mode), taps.data_ptr(), aff.data_ptr(), *run, *[float(bn.eps) for bn in bns],
+          *[float(bn.momentum) for bn in bns], fold.data_ptr(), stats.data_ptr(), total.data_ptr(), C, _stream())
+    return total
+
+
+def _sync_parts(parts, Q, C, name):
+    _chk(parts, torch.float32, "parts")
+    if not (parts.is_contiguous() and parts.dim() == 3 and parts.shape[1:] == (Q, C)):
+        raise ValueError(f"{name}: expected contiguous fp32 parts [W, {Q}, {C}], got {tuple(parts.shape)}")
+
+
+def _sync_total(total, name):
+    _chk(total, torch.float64, "total")
+    if total.numel() != 1:
+        raise ValueError(f"{name}: total must be a one-element fp64 tensor")
+
+
+def repmixer_bn_ffn_sums(x1, du, taps, stats, B, L, aff, dgamma=None, dbeta=None):
+    """First half of repmixer_bn_ffn_bwd: this rank's sums fp32 [2, C]; BN_f's dgamma / dbeta accumulated (this rank's)."""
+    C = x1.shape[-1]
+    _repmixer_bwd_args("repmixer_bn_ffn_sums", (x1, du), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    ptrs = [_grad_dst(dgamma, C, "dgamma"), _grad_dst(dbeta, C, "dbeta")]
+    sums = torch.empty((2, C), device=x1.device, dtype=torch.float32)
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x1.device)
+    _call("es3_repmixer_bn_ffn_sums", "repmixer_bn_ffn_sums", _nb(x1, du), 3 * 11 * x1.numel(), x1.data_ptr(), du.data_ptr(),
+          taps.data_ptr(), stats.data_ptr(), ws.data_ptr(), sums.data_ptr(), *ptrs, B, L, C, _stream())
+    return sums
+
+
+def repmixer_bn_ffn_apply(x1, du, g, taps, aff, stats, parts, total, B, L, dtaps=None):
+    """Second half of repmixer_bn_ffn_bwd with every rank's sums parts [W, 2, C] (rank order) and the group's count: returns e."""
+    C = x1.shape[-1]
+    _repmixer_bwd_args("repmixer_bn_ffn_apply", (x1, du, g), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    _sync_parts(parts, 2, C, "repmixer_bn_ffn_apply")
+    _sync_total(total, "repmixer_bn_ffn_apply")
+    e = torch.empty_like(x1)
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x1.device)
+    _call("es3_repmixer_bn_ffn_apply", "repmixer_bn_ffn_apply", _nb(x1, du, g, e), 5 * 11 * x1.numel(), x1.data_ptr(), du.data_ptr(),
+          g.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), parts.data_ptr(), parts.shape[0], total.data_ptr(),
+          e.data_ptr(), ws.data_ptr(), _grad_dst(dtaps, 11 * C, "dtaps"), B, L, C, _stream())
+    return e
+
+
+def repmixer_bn_tm_sums(x, e, taps, aff, stats, B, L, dbn=(None,) * 6):
+    """First half of repmixer_bn_tm_bwd: this rank's sums fp32 [3, C]; dbn = (dgamma, dbeta) x (ms, mc, ns) accumulated."""
+    C = x.shape[-1]
+    _repmixer_bwd_args("repmixer_bn_tm_sums", (x, e), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    ptrs = [_grad_dst(t, C, "dbn") for t in dbn]
+    sums = torch.empty((3, C), device=x.device, dtype=torch.float32)
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
+    _call("es3_repmixer_bn_tm_sums", "repmixer_bn_tm_sums", _nb(x, e), 4 * 11 * x.numel(), x.data_ptr(), e.data_ptr(),
+          taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), ws.data_ptr(), sums.data_ptr(), *ptrs, B, L, C, _stream())
+    return sums
+
+
+def repmixer_bn_tm_apply(x, e, taps, aff, stats, parts, total, B, L, dtaps=None, dls=None, want_bf16=False):
+    """Second half of repmixer_bn_tm_bwd with every rank's sums parts [W, 3, C] and the group's count: (dx fp32, bf16 copy | None)."""
+    C = x.shape[-1]
+    _repmixer_bwd_args("repmixer_bn_tm_apply", (x, e), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    _sync_parts(parts, 3, C, "repmixer_bn_tm_apply")
+    _sync_total(total, "repmixer_bn_tm_apply")
+    dx = torch.empty_like(x)
+    dxb = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
+    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
+    _call("es3_repmixer_bn_tm_apply", "repmixer_bn_tm_apply", _nb(x, e, dx, dxb), 6 * 11 * x.numel(), x.data_ptr(), e.data_ptr(),
+          taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), parts.data_ptr(), parts.shape[0], total.data_ptr(), dx.data_ptr(),
+          _ptr(dxb), ws.data_ptr(), _grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dls, C, "dls"), B, L, C, _stream())
+    return dx, dxb
+
+
 # ------------------------------------------------------------------------------------ text-student backward (text_bwd.cu)
 TEXT_ATTN_BWD_MAX_L = 128
 KERNELS_PER_CALL.update({"es3_layernorm_bwd_f32": 2, "es3_text_kd_loss_fwd": 2, "es3_text_consistency_fwd": 2,
@@ -1222,10 +1339,113 @@ def bn_act_bwd(da, z, scale, shift, act, mode, mean=None, invstd=None, dgamma=No
           _ptr(dbeta), _stream())
     if not apply:
         return None
+    return bn_act_bwd_apply(da, z, scale, shift, act, coef)
+
+
+def bn_act_bwd_apply(da, z, scale, shift, act, coef):
+    """dz = coef[0] g + coef[1] z + coef[2], g = da act'(scale z + shift); da, z [..., C] bf16 contiguous, coef fp32 [3, C]."""
+    _chk(da, torch.bfloat16, "da"); _chk(z, torch.bfloat16, "z"); _chk(coef, torch.float32, "coef")
+    _ensure_init(z)
+    assert da.is_contiguous() and z.is_contiguous() and da.shape == z.shape
+    C = z.shape[-1]
+    assert coef.is_contiguous() and coef.shape == (3, C), coef.shape
     dz = torch.empty_like(z)
     _call("es3_bn_act_bwd_apply", "bn_act_bwd_apply", _nb(da, z, dz), 8 * z.numel(), da.data_ptr(), z.data_ptr(), _ptr(scale),
-          _ptr(shift), ACT[act], coef.data_ptr(), dz.data_ptr(), M, C, _stream())
+          _ptr(shift), ACT[act], coef.data_ptr(), dz.data_ptr(), z.numel() // C, C, _stream())
     return dz
+
+
+# ------------------------------------------------------------------------------------ synchronised BatchNorm (bn_sync.cu)
+KERNELS_PER_CALL.update({"es3_bn_stats_partial": 2, "es3_bn_act_bwd_partial": 2})
+
+
+def _vec_f32(t, C, name):
+    if t is None:
+        return
+    _chk(t, torch.float32, name)
+    if not (t.is_contiguous() and t.numel() == C):
+        raise ValueError(f"{name}: expected a contiguous fp32 vector of {C} channels, got {tuple(t.shape)}")
+
+
+def _rows_z(z, name="z"):
+    _chk(z, torch.bfloat16, name)
+    if not z.is_contiguous() or z.dim() < 2 or z.shape[-1] % 8 or z.numel() == 0:
+        raise ValueError(f"{name}: expected a non-empty contiguous bf16 [..., C] tensor with C % 8 == 0, got {tuple(z.shape)}")
+    C = z.shape[-1]
+    return z.numel() // C, C
+
+
+def _gathered(part, rows, name):
+    _chk(part, torch.float64, name)
+    if not (part.is_contiguous() and part.dim() == 3 and part.shape[0] >= 1 and part.shape[1] == rows and part.shape[2] % 8 == 0):
+        raise ValueError(f"{name}: expected a contiguous fp64 [W, {rows}, C] tensor with C % 8 == 0, got {tuple(part.shape)}")
+    return part.shape[0], part.shape[2]
+
+
+def bn_stats_partial(z):
+    """This rank's batch statistics of z [..., C] bf16: fp64 [3, C] = (count, mean, M2) per channel (es3_bn_stats_partial)."""
+    M, C = _rows_z(z)
+    _ensure_init(z)
+    ws = _f32ws(_lib.size("es3_col_reduce_ws_floats", M, C), z.device)
+    part = torch.empty((3, C), device=z.device, dtype=torch.float64)
+    _call("es3_bn_stats_partial", "bn_stats_partial", _nb(z), 3 * z.numel(), z.data_ptr(), M, C, ws.data_ptr(), part.data_ptr(), _stream())
+    return part
+
+
+def bn_stats_combine(parts, gamma, beta, eps, momentum, running_mean=None, running_var=None, num_batches_tracked=None):
+    """parts: fp64 [W, 3, C], every rank's bn_stats_partial in rank order.  Returns (mean, invstd, scale, shift) fp32 [C] as
+    bn_stats does, and the total row count as a one-element fp64 device tensor; updates the running buffers in place."""
+    W, C = _gathered(parts, 3, "parts")
+    _ensure_init(parts)
+    for t, n in ((gamma, "gamma"), (beta, "beta"), (running_mean, "running_mean"), (running_var, "running_var")):
+        _vec_f32(t, C, n)
+    if num_batches_tracked is not None and num_batches_tracked.dtype != torch.int64:
+        raise ValueError("num_batches_tracked: expected int64")
+    dev = parts.device
+    mean, invstd, scale, shift = (torch.empty(C, device=dev, dtype=torch.float32) for _ in range(4))
+    total = torch.empty(1, device=dev, dtype=torch.float64)
+    _call("es3_bn_stats_combine", "bn_stats_combine", _nb(parts), 10 * W * C, parts.data_ptr(), W, C, float(eps), float(momentum),
+          _ptr(gamma), _ptr(beta), mean.data_ptr(), invstd.data_ptr(), scale.data_ptr(), shift.data_ptr(), _ptr(running_mean),
+          _ptr(running_var), _ptr(num_batches_tracked), total.data_ptr(), _stream())
+    return mean, invstd, scale, shift, total
+
+
+def bn_act_bwd_partial(da, z, scale, shift, act, mean, invstd, dgamma=None, dbeta=None):
+    """This rank's sums of the batch-statistics BN backward: fp64 [2, C] = (sum g, sum g (z - mean)), g = da act'(scale z + shift).
+    dgamma / dbeta (fp32 [C], may be None) accumulate this rank's own gradients."""
+    M, C = _rows_z(z)
+    _chk(da, torch.bfloat16, "da")
+    if not (da.is_contiguous() and da.shape == z.shape):
+        raise ValueError(f"da: expected a contiguous tensor of z's shape {tuple(z.shape)}, got {tuple(da.shape)}")
+    if mean is None or invstd is None:
+        raise ValueError("bn_act_bwd_partial: mean and invstd are required")
+    for t, n in ((scale, "scale"), (shift, "shift"), (mean, "mean"), (invstd, "invstd"), (dgamma, "dgamma"), (dbeta, "dbeta")):
+        _vec_f32(t, C, n)
+    _ensure_init(z)
+    ws = _f32ws(_lib.size("es3_col_reduce_ws_floats", M, C), z.device)
+    part = torch.empty((2, C), device=z.device, dtype=torch.float64)
+    _call("es3_bn_act_bwd_partial", "bn_act_bwd_partial", _nb(da, z), 6 * z.numel(), da.data_ptr(), z.data_ptr(), _ptr(scale),
+          _ptr(shift), ACT[act], mean.data_ptr(), invstd.data_ptr(), M, C, ws.data_ptr(), part.data_ptr(), _ptr(dgamma), _ptr(dbeta),
+          _stream())
+    return part
+
+
+def bn_bwd_coef(parts, total, scale, mean, invstd):
+    """parts: fp64 [W, 2, C], every rank's bn_act_bwd_partial in rank order; total: the count bn_stats_combine returned.
+    Returns coef fp32 [3, C] for bn_act_bwd_apply."""
+    W, C = _gathered(parts, 2, "parts")
+    _chk(total, torch.float64, "total")
+    if total.numel() != 1:
+        raise ValueError("total: expected a one-element fp64 tensor")
+    if mean is None or invstd is None:
+        raise ValueError("bn_bwd_coef: mean and invstd are required")
+    for t, n in ((scale, "scale"), (mean, "mean"), (invstd, "invstd")):
+        _vec_f32(t, C, n)
+    _ensure_init(parts)
+    coef = torch.empty((3, C), device=parts.device, dtype=torch.float32)
+    _call("es3_bn_bwd_coef", "bn_bwd_coef", _nb(parts), 8 * W * C, parts.data_ptr(), W, C, total.data_ptr(), _ptr(scale),
+          mean.data_ptr(), invstd.data_ptr(), coef.data_ptr(), _stream())
+    return coef
 
 
 def add_bf16(a, b):

@@ -392,6 +392,44 @@ int es3_bn_act_bwd_reduce(const void* da, const void* z, const float* scale, con
                           float* dbeta, void* stream);
 int es3_bn_act_bwd_apply(const void* da, const void* z, const float* scale, const float* shift, int act, const float* coef,
                          void* dz, long long M, int C, void* stream);
+/* Synchronised BatchNorm (nn.SyncBatchNorm in train mode; bn_sync.cu): es3_bn_stats and the batch-statistics backward split where
+ * the ranks of a process group all-gather their partials.  Partials are fp64 and combined in rank order, so every rank computes
+ * bit-identical statistics.  ws: es3_col_reduce_ws_floats(M, C) floats.
+ *   es3_bn_stats_partial: part [3][C] = (count, mean, M2 = sum (z - mean)^2) of this rank's rows, pivot-shifted as es3_bn_stats.
+ *   es3_bn_stats_combine: part [W][3][C] -> mean, invstd, scale, shift as es3_bn_stats writes them, the running-stat update over the
+ *     total count, num_batches_tracked += 1 and total [1] = the total count (running_* / num_batches_tracked / total may be NULL).
+ *   es3_bn_act_bwd_partial: part [2][C] = (sum g, sum g (z - mean)) of this rank's rows, g = da act'(scale z + shift); adds this
+ *     rank's dgamma = invstd sum g (z - mean) and dbeta = sum g (either may be NULL).
+ *   es3_bn_bwd_coef: part [W][2][C] summed in rank order and the total count -> coef [3][C] for es3_bn_act_bwd_apply. */
+/* Synchronised BatchNorm in MobileCLIP-S0's RepMixerBlocks (repmixer_bn_train.cu): es3_repmixer_bn_fwd split at its two
+ * finalize points and the batch-statistics backward at its two sums, for the ranks to all-gather the partials in between. */
+int es3_repmixer_bn_stats_partial(const float* x, const float* taps, const float* fold, int mode, float* ws, double* part, int B, int L,
+                                  int C, void* stream);
+int es3_repmixer_bn_finalize_sync(const double* parts, int W, int mode, const float* taps, const float* aff, float* rm_ms, float* rv_ms,
+                                  long long* nbt_ms, float* rm_mc, float* rv_mc, long long* nbt_mc, float* rm_ns, float* rv_ns,
+                                  long long* nbt_ns, float* rm_f, float* rv_f, long long* nbt_f, float eps_ms, float eps_mc, float eps_ns,
+                                  float eps_f, float mom_ms, float mom_mc, float mom_ns, float mom_f, float* fold, float* stats,
+                                  double* total, int C, void* stream);
+int es3_repmixer_bn_ffn_sums(const float* x1, const float* du, const float* taps, const float* stats, float* ws, float* sums,
+                             float* dgamma, float* dbeta, int B, int L, int C, void* stream);
+int es3_repmixer_bn_ffn_apply(const float* x1, const float* du, const float* g, const float* taps, const float* aff, const float* stats,
+                              const float* parts, int W, const double* total, float* e, float* ws, float* dwf, int B, int L, int C,
+                              void* stream);
+int es3_repmixer_bn_tm_sums(const float* x, const float* e, const float* taps, const float* aff, const float* stats, float* ws,
+                            float* sums, float* dg_ms, float* db_ms, float* dg_mc, float* db_mc, float* dg_ns, float* db_ns, int B,
+                            int L, int C, void* stream);
+int es3_repmixer_bn_tm_apply(const float* x, const float* e, const float* taps, const float* aff, const float* stats,
+                             const float* parts, int W, const double* total, float* dx, void* dxb, float* ws, float* dwmc, float* dls,
+                             int B, int L, int C, void* stream);
+int es3_bn_stats_partial(const void* z, long long M, int C, float* ws, double* part, void* stream);
+int es3_bn_stats_combine(const double* part, int W, int C, float eps, float momentum, const float* gamma, const float* beta, float* mean,
+                         float* invstd, float* scale, float* shift, float* running_mean, float* running_var,
+                         long long* num_batches_tracked, double* total, void* stream);
+int es3_bn_act_bwd_partial(const void* da, const void* z, const float* scale, const float* shift, int act, const float* mean,
+                           const float* invstd, long long M, int C, float* ws, double* part, float* dgamma, float* dbeta,
+                           void* stream);
+int es3_bn_bwd_coef(const double* part, int W, int C, const double* total, const float* scale, const float* mean, const float* invstd,
+                    float* coef, void* stream);
 /* out = a + b, bf16 [M][C] with row strides in elements (gradient fan-in at residual joins / LiteMLA multi-scale). */
 int es3_add_bf16(const void* a, long long lda, const void* b, long long ldb, void* out, long long ldo, long long M, int C,
                  void* stream);

@@ -8,7 +8,9 @@
 // (each of the two compute warpgroups holds COUT / 2 columns) -> BN + residual epilogue.  The depthwise output never exists
 // in HBM.
 //
-// Persistent CTAs; warps 0-7 depthwise + wgmma + epilogue, warp 8 lane 0 = TMA; 2-stage ring of (mid chunk, W3 chunk).
+// Persistent CTAs; warps 0-7 depthwise + wgmma + epilogue, warp 8 lane 0 = TMA (its warpgroup hands its registers to the other
+// two); 2-stage ring of (mid chunk, W3 chunk).  A chunk's projection wgmma is retired only after the next chunk's depthwise, so
+// the tensor cores run it while the warps do the depthwise.
 #include <cuda.h>
 
 #include "ptx.cuh"
@@ -37,7 +39,7 @@ __device__ __forceinline__ void mma_1688(float* d, uint32_t a0, uint32_t a1, uin
 }  // namespace
 
 constexpr int DP_TH = 8, DP_TW = 16, DP_HH = DP_TH + 2, DP_HW = DP_TW + 2, DP_PIN = DP_HH * DP_HW;   // 8x16 tile, 10x18 halo
-constexpr int DP_MC = 64, DP_THREADS = 288;
+constexpr int DP_MC = 64, DP_THREADS = 384;   // two compute warpgroups + one TMA warpgroup
 
 template <int MID, int COUT, int WSTAGES>
 struct DPSmem {
@@ -60,9 +62,9 @@ struct DPArgs {
 };
 
 template <int MID, int COUT, int WSTAGES, int ACT>
-// One CTA per SM: with the projection's accumulators live across the asynchronous wgmma window, the two-CTA register cap
-// (96 registers) spills heavily; on H100 the (512, 128) instantiation took 1.58 ms per EV-M step at two CTAs per SM and
-// 0.56 ms at one.
+// One CTA per SM of three warpgroups.  The TMA warpgroup drops to 40 registers so that the two compute warpgroups can hold
+// 232 each: the (1024, 256) projection keeps 128 fp32 accumulators per thread live across the asynchronous wgmma window, and
+// under the 168-register cap of a uniform 288- or 384-thread CTA it spilled 504 bytes per thread.
 __global__ void __launch_bounds__(DP_THREADS, 1)
 dwproj_tc_kernel(const __grid_constant__ CUtensorMap tm_mid, const __grid_constant__ CUtensorMap tm_w3, const DPArgs a) {
   using L = DPSmem<MID, COUT, WSTAGES>;
@@ -100,9 +102,10 @@ dwproj_tc_kernel(const __grid_constant__ CUtensorMap tm_mid, const __grid_consta
   __syncthreads();
   const int tiles_per_img = a.tiles_x * a.tiles_y;
 
-  if (warp == 8) {
-    // ------------------------------------------------------------------------------------ control: TMA
-    if (lane == 0 && my_tiles > 0) {
+  if (warp >= 8) {
+    // ------------------------------------------------------------------------------------ control: TMA (warp 8 lane 0)
+    ptx::setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0 && my_tiles > 0) {
       auto load_a = [&](int g) {       // mid chunk g (tile g / NC, channels (g % NC) * 64 ..) with its 1-pixel halo
         const int t = (int)blockIdx.x + (g / NC) * (int)gridDim.x;
         const int bb = t / tiles_per_img, r = t % tiles_per_img, s = g & 1;
@@ -131,6 +134,7 @@ dwproj_tc_kernel(const __grid_constant__ CUtensorMap tm_mid, const __grid_consta
   } else {
     // ------------------------------------------------------------------------------------ compute warps 0..7 (two warpgroups)
     // warpgroup hsel accumulates the projection's columns hsel * CW .. +CW for all 128 pixels of the tile in registers
+    ptx::setmaxnreg_inc<232>();
     constexpr int CW = COUT / 2;
     const int q = warp & 3, hsel = warp >> 2;
     const int g4 = lane >> 2, t4 = lane & 3;
@@ -192,6 +196,13 @@ dwproj_tc_kernel(const __grid_constant__ CUtensorMap tm_mid, const __grid_consta
         ptx::fence_proxy_async();
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(bar_afree + (g & 1));   // this warp is done reading the mid stage
+        if (c > 0) {
+          // project(g-1) ran on the tensor cores under this chunk's depthwise; retire it before s_dw is overwritten
+          ptx::wg_wait<0>();
+          ptx::wg_fence_regs<CW>(&proj[0][0]);
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(bar_w3free + ((WSTAGES == 2) ? ((g - 1) & 1) : 0));
+        }
         ptx::named_bar(1, 256);                                  // project(g-1) of both warpgroups has finished reading s_dw
         const float* b2 = s_b2 + c * DP_MC;
 #pragma unroll
@@ -225,12 +236,12 @@ dwproj_tc_kernel(const __grid_constant__ CUtensorMap tm_mid, const __grid_consta
             else ptx::wgmma_m64n64<0, 0>(proj[rb], da, db, (c | k) != 0);
           }
         }
-        ptx::wg_commit();
-        ptx::wg_wait<0>();
-        ptx::wg_fence_regs<CW>(&proj[0][0]);
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(bar_w3free + ws);
+        ptx::wg_commit();                                        // retired under the next chunk's depthwise, or below
       }
+      ptx::wg_wait<0>();                                         // the tile's last project: the epilogue reads the accumulators
+      ptx::wg_fence_regs<CW>(&proj[0][0]);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(bar_w3free + ((WSTAGES == 2) ? ((g - 1) & 1) : 0));
 
       // ---- final epilogue: BN3 (+ residual) -> global, from the accumulator fragments
 #pragma unroll
@@ -304,5 +315,5 @@ extern "C" int es3_dwproj_tc_bf16(const void* mid, const float* wdw, const float
   a.total_tiles = B * a.tiles_x * a.tiles_y;
   cudaStream_t st = (cudaStream_t)stream;
   if (Mid == 512) return launch_dwproj<512, 128, 2>(mid, w3, a, B, st);
-  return launch_dwproj<1024, 256, 1>(mid, w3, a, B, st);
+  return launch_dwproj<1024, 256, 2>(mid, w3, a, B, st);
 }

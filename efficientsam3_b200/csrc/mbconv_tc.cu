@@ -13,8 +13,10 @@
 //     project  D_proj[128 x COUT] += s_dw x W3c^T                                  wgmma, SS, accumulating over chunks in registers
 //   final     D_proj fragments -> BN3 + residual (x re-read from global / L2) -> global
 //
-// Warps 0-7 (two warpgroups) issue the MMAs and do the elementwise / depthwise work, warp 8 lane 0 issues TMA; chunk weights
-// sit in a 2-stage ring refilled as soon as the MMA that read a stage retires, so the weight loads overlap the depthwise.
+// Warps 0-7 (two warpgroups) issue the MMAs and do the elementwise / depthwise work, warp 8 lane 0 of the third warpgroup issues
+// TMA (that warpgroup hands its registers to the other two); chunk weights sit in a 2-stage ring refilled as soon as the MMA that
+// read a stage retires, so the weight loads overlap the depthwise.  A chunk's project wgmma is retired only by the next chunk's
+// expand wait, so it runs on the tensor cores while the warps wait for the next weights and issue the next expand.
 // CTAs are persistent: parameters and barriers are set up once, the weight ring runs across tiles and the next tile's input
 // TMA is issued as soon as the current tile's last expand retires.
 #include <cuda.h>
@@ -51,7 +53,7 @@ constexpr int MT_HH = MT_TH + 2, MT_HW = MT_TW + 2;      // haloed input tile: 1
 constexpr int MT_PIN = MT_HH * MT_HW;                    // 180 pixels
 constexpr int MT_MC = 64;                                // expanded-channel chunk
 constexpr int MT_RS_MID = MT_MC * 2 + 16;                // s_mid row stride (bytes)
-constexpr int MT_THREADS = 288;                          // 8 compute warps + 1 control warp
+constexpr int MT_THREADS = 384;                          // two compute warpgroups + one TMA warpgroup
 
 template <int MID, int COUT>
 struct MTSmem {
@@ -80,8 +82,15 @@ struct MTArgs {
   int H, W, tiles_x, tiles_y, total_tiles;
 };
 
-template <int CIN, int MID, int COUT, int ACT>
-__global__ void __launch_bounds__(MT_THREADS, 2)
+// MINB CTAs per SM.  The TMA warpgroup gives its registers to the two compute warpgroups (setmaxnreg): 40 / 232 at one CTA per
+// SM, 24 / 104 at two, against a uniform 168 / 80.
+template <int MINB>
+struct MTRegs {
+  static constexpr int TMA = MINB == 1 ? 40 : 24, MMA = MINB == 1 ? 232 : 104;
+};
+
+template <int CIN, int MID, int COUT, int ACT, int MINB>
+__global__ void __launch_bounds__(MT_THREADS, MINB)
 mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w1,
                  const __grid_constant__ CUtensorMap tm_w3, const MTArgs a) {
   using L = MTSmem<MID, COUT>;
@@ -128,9 +137,10 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
   __syncthreads();
   const int tiles_per_img = a.tiles_x * a.tiles_y;
 
-  if (warp == 8) {
-    // ------------------------------------------------------------------------------------ control: TMA
-    if (lane == 0 && my_tiles > 0) {
+  if (warp >= 8) {
+    // ------------------------------------------------------------------------------------ control: TMA (warp 8 lane 0)
+    ptx::setmaxnreg_dec<MTRegs<MINB>::TMA>();
+    if (warp == 8 && lane == 0 && my_tiles > 0) {
       constexpr uint32_t W1_BYTES = MT_MC * 128, W3_BYTES = COUT * 128;
       auto load_in = [&](int t) {
         const int bb = t / tiles_per_img, r = t % tiles_per_img;
@@ -166,6 +176,7 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
   } else {
     // ------------------------------------------------------------------------------------ compute warps 0..7 (two warpgroups)
     // warpgroup hsel: expand columns hsel*32 .. +32 of the chunk; project columns hsel*32 .. (COUT 64) or rows hsel*64 .. (COUT 32)
+    ptx::setmaxnreg_inc<MTRegs<MINB>::MMA>();
     const int q = warp & 3, hsel = warp >> 2;            // warp inside the warpgroup; warpgroup = column half / m-tile parity (dw)
     const int g = lane >> 2, t4 = lane & 3;
     const int a_row = lane & 15, a_kh = lane >> 4;
@@ -199,12 +210,13 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
           for (int mb = 0; mb < 3; ++mb) ptx::wgmma_m64n32<0, 0>(ex[mb], ptx::make_desc_sw128(u_in + mb * 8192 + k * 32), db, k != 0);
         }
         ptx::wg_commit();
-        ptx::wg_wait<0>();
+        ptx::wg_wait<0>();                                 // also retires project(gc-1), still in flight unless c == 0
         ptx::wg_fence_regs<48>(&ex[0][0]);
         __syncwarp();
         if (lane == 0) {
           ptx::mbar_arrive(bar_w1free + st);
           if (c == NC - 1) ptx::mbar_arrive(bar_infree);
+          if (c > 0) ptx::mbar_arrive(bar_w3free + (st ^ 1));
         }
         compute_bar_sync();                              // every warp is done reading s_mid for the previous chunk
         // ---- expand epilogue: BN1 + act, zero outside the image, bf16 -> s_mid[row][hsel*32 .. +32)
@@ -295,12 +307,12 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
           for (int rb = 0; rb < PRB; ++rb)
             ptx::wgmma_m64n32<0, 0>(proj[rb], ptx::make_desc_sw128(u_dw + (prb0 + rb) * 8192 + k * 32), db, (c | k) != 0);
         }
-        ptx::wg_commit();
-        ptx::wg_wait<0>();
-        ptx::wg_fence_regs<PRB * 16>(&proj[0][0]);
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(bar_w3free + st);
+        ptx::wg_commit();                                // retired by the next chunk's expand wait, or below
       }
+      ptx::wg_wait<0>();                                 // the tile's last project: the final epilogue reads the accumulators
+      ptx::wg_fence_regs<PRB * 16>(&proj[0][0]);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(bar_w3free + ((gc - 1) & 1));
 
       // ---- final epilogue: BN3 + residual (x re-read from global / L2) -> global, from the accumulator fragments
 #pragma unroll
@@ -321,7 +333,7 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
   }
 }
 
-template <int CIN, int MID, int COUT>
+template <int CIN, int MID, int COUT, int MINB>
 static int launch_mbconv_tc(const void* x, void* y, const void* w1, const void* w3, const MTArgs& a, int B, cudaStream_t st) {
   using L = MTSmem<MID, COUT>;
   CUtensorMap tm_in, tm_w1, tm_w3;
@@ -343,7 +355,7 @@ static int launch_mbconv_tc(const void* x, void* y, const void* w1, const void* 
     uint32_t box[2] = {(uint32_t)MT_MC, (uint32_t)COUT};
     if (encode_map(&tm_w3, w3, 2, dims, str, box)) return 1;
   }
-  auto kern = mbconv_tc_kernel<CIN, MID, COUT, ACT_HSWISH>;
+  auto kern = mbconv_tc_kernel<CIN, MID, COUT, ACT_HSWISH, MINB>;
   static bool configured = false;
   if (!configured) {
     ES3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
@@ -355,7 +367,7 @@ static int launch_mbconv_tc(const void* x, void* y, const void* w1, const void* 
     ES3_CHECK_CUDA(cudaGetDevice(&dev));
     ES3_CHECK_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
   }
-  const int ctas = a.total_tiles < 2 * sm_count ? a.total_tiles : 2 * sm_count;   // persistent, two CTAs per SM
+  const int ctas = a.total_tiles < MINB * sm_count ? a.total_tiles : MINB * sm_count;   // persistent
   kern<<<ctas, MT_THREADS, L::TOTAL, st>>>(tm_in, tm_w1, tm_w3, a);
   ES3_LAUNCH_CHECK("mbconv_tc_kernel");
   return 0;
@@ -378,6 +390,8 @@ extern "C" int es3_mbconv_tc_bf16(const void* x, void* y, const void* w1, const 
   a.H = H; a.W = W; a.tiles_x = ceil_div(W, MT_TW); a.tiles_y = ceil_div(H, MT_TH);
   a.total_tiles = B * a.tiles_x * a.tiles_y;
   cudaStream_t st = (cudaStream_t)stream;
-  if (Cin == 32) return launch_mbconv_tc<32, 128, 32>(x, y, w1, w3, a, B, st);
-  return launch_mbconv_tc<64, 256, 64>(x, y, w1, w3, a, B, st);
+  // (32, 128, 32) fits 104 registers and runs faster with a second CTA per SM to overlap its phases; (64, 256, 64) needs more
+  // than 104 (it spills and ptxas serialises its wgmma) and runs at one CTA per SM
+  if (Cin == 32) return launch_mbconv_tc<32, 128, 32, 2>(x, y, w1, w3, a, B, st);
+  return launch_mbconv_tc<64, 256, 64, 1>(x, y, w1, w3, a, B, st);
 }

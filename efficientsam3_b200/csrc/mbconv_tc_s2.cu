@@ -43,7 +43,7 @@ constexpr int S2_RS_MID = S2_MC * 2 + 16;                  // 80-byte rows: conf
 // slot S2_ODD + j).  A stride-2 tap then walks CONSECUTIVE 80-byte rows (8 rows -> 8 distinct 4-bank groups); walking every other
 // row of an interleaved tile (160-byte stride) made every ldmatrix 2-way conflicted.  S2_ODD = 20 also keeps the expand epilogue's 16-byte stores (lanes alternate planes) apart.
 constexpr int S2_ODD = 20, S2_PW = S2_ODD + S2_TW;           // slots per input row: 17 even | 3 unused | 16 odd
-constexpr int S2_THREADS = 288;
+constexpr int S2_THREADS = 384;                           // two compute warpgroups + one TMA warpgroup
 
 template <int MID, int COUT, int WSTAGES>
 struct S2Smem {
@@ -74,8 +74,14 @@ struct S2Args {
   int H, W, Ho, Wo, tiles_x, tiles_y, total_tiles;
 };
 
-template <int CIN, int MID, int COUT, int WSTAGES, int ACT>
-__global__ void __launch_bounds__(S2_THREADS, 2)
+// MINB CTAs per SM; the TMA warpgroup gives its registers to the compute warpgroups (setmaxnreg), as in mbconv_tc.cu.
+template <int MINB>
+struct S2Regs {
+  static constexpr int TMA = MINB == 1 ? 40 : 24, MMA = MINB == 1 ? 232 : 104;
+};
+
+template <int CIN, int MID, int COUT, int WSTAGES, int ACT, int MINB>
+__global__ void __launch_bounds__(S2_THREADS, MINB)
 mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w1,
                     const __grid_constant__ CUtensorMap tm_w3, const S2Args a) {
   using L = S2Smem<MID, COUT, WSTAGES>;
@@ -119,9 +125,10 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
   const int tiles_per_img = a.tiles_x * a.tiles_y;
   constexpr uint32_t W1_BYTES = S2_MC * 128, W3_BYTES = L::W3_STAGE;
 
-  if (warp == 8) {
-    // ------------------------------------------------------------------------------------ control: TMA
-    if (lane == 0 && my_tiles > 0) {
+  if (warp >= 8) {
+    // ------------------------------------------------------------------------------------ control: TMA (warp 8 lane 0)
+    ptx::setmaxnreg_dec<S2Regs<MINB>::TMA>();
+    if (warp == 8 && lane == 0 && my_tiles > 0) {
       auto load_in = [&](int t) {
         const int bb = t / tiles_per_img, r = t % tiles_per_img;
         ptx::mbar_arrive_expect_tx(bar_in, S2_PIN * 128);
@@ -160,6 +167,7 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
     // ------------------------------------------------------------------------------------ compute warps 0..7 (two warpgroups)
     // expand: warpgroup 0 takes the 64-row blocks 0, 2, 4 of the 297 input pixels, warpgroup 1 blocks 1, 3;
     // project: warpgroup hsel takes output columns hsel * PN .. +PN (COUT 32: warpgroup 0 alone)
+    ptx::setmaxnreg_inc<S2Regs<MINB>::MMA>();
     const int q = warp & 3, hsel = warp >> 2;
     const int g4 = lane >> 2, t4 = lane & 3;
     const int a_row = lane & 15, a_kh = lane >> 4;
@@ -197,12 +205,13 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
           }
         }
         ptx::wg_commit();
-        ptx::wg_wait<0>();
+        ptx::wg_wait<0>();                                   // also retires project(g-1), still in flight unless c == 0
         ptx::wg_fence_regs<48>(&ex[0][0]);
         __syncwarp();
         if (lane == 0) {
           ptx::mbar_arrive(bar_w1free + st);
           if (c == NC - 1) ptx::mbar_arrive(bar_infree);
+          if (c > 0) ptx::mbar_arrive(bar_w3free + ((WSTAGES == 2) ? (st ^ 1) : 0));
         }
         compute_bar_sync();                                // every warp is done reading s_mid for the previous chunk
         // ---- expand epilogue: BN1 + act, zero outside the image, bf16 -> s_mid (even / odd column planes)
@@ -291,12 +300,12 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
           if constexpr (PN == 64) ptx::wgmma_m64n64<0, 0>(proj, da, db, (c | k) != 0);
           else ptx::wgmma_m64n32<0, 0>(proj, da, db, (c | k) != 0);
         }
-        ptx::wg_commit();
-        ptx::wg_wait<0>();
-        ptx::wg_fence_regs<PN / 2>(proj);
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(bar_w3free + ws);
+        ptx::wg_commit();                                  // retired by the next chunk's expand wait, or below
       }
+      ptx::wg_wait<0>();                                   // the tile's last project: the final epilogue reads the accumulators
+      ptx::wg_fence_regs<PN / 2>(proj);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(bar_w3free + ((WSTAGES == 2) ? ((g - 1) & 1) : 0));
 
       // ---- final epilogue: BN3 -> global, from the accumulator fragments
       if (pact) {
@@ -315,7 +324,7 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
   }
 }
 
-template <int CIN, int MID, int COUT, int WSTAGES>
+template <int CIN, int MID, int COUT, int WSTAGES, int MINB>
 static int launch_mbconv_tc_s2(const void* x, const void* w1, const void* w3, const S2Args& a, int B, cudaStream_t st) {
   using L = S2Smem<MID, COUT, WSTAGES>;
   CUtensorMap tm_in, tm_w1, tm_w3;
@@ -337,7 +346,7 @@ static int launch_mbconv_tc_s2(const void* x, const void* w1, const void* w3, co
     uint32_t box[2] = {64u, (uint32_t)COUT};
     if (encode_map(&tm_w3, w3, 2, dims, str, box)) return 1;
   }
-  auto kern = mbconv_tc_s2_kernel<CIN, MID, COUT, WSTAGES, ACT_HSWISH>;
+  auto kern = mbconv_tc_s2_kernel<CIN, MID, COUT, WSTAGES, ACT_HSWISH, MINB>;
   static bool configured = false;
   if (!configured) {
     ES3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
@@ -349,7 +358,7 @@ static int launch_mbconv_tc_s2(const void* x, const void* w1, const void* w3, co
     ES3_CHECK_CUDA(cudaGetDevice(&dev));
     ES3_CHECK_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
   }
-  const int ctas = a.total_tiles < 2 * sm_count ? a.total_tiles : 2 * sm_count;
+  const int ctas = a.total_tiles < MINB * sm_count ? a.total_tiles : MINB * sm_count;
   kern<<<ctas, S2_THREADS, L::TOTAL, st>>>(tm_in, tm_w1, tm_w3, a);
   ES3_LAUNCH_CHECK("mbconv_tc_s2_kernel");
   return 0;
@@ -375,7 +384,8 @@ extern "C" int es3_mbconv_tc_s2_bf16(const void* x, void* y, const void* w1, con
   a.tiles_x = ceil_div(a.Wo, S2_TW); a.tiles_y = ceil_div(a.Ho, S2_TH);
   a.total_tiles = B * a.tiles_x * a.tiles_y;
   cudaStream_t st = (cudaStream_t)stream;
-  if (Cin == 16) return launch_mbconv_tc_s2<16, 64, 32, 2>(x, w1, w3, a, B, st);
-  if (Cin == 32) return launch_mbconv_tc_s2<32, 128, 64, 2>(x, w1, w3, a, B, st);
-  return launch_mbconv_tc_s2<64, 256, 128, 1>(x, w1, w3, a, B, st);
+  // two CTAs per SM (104 registers) where that does not spill, one (232 registers) for (64, 256, 128)
+  if (Cin == 16) return launch_mbconv_tc_s2<16, 64, 32, 2, 2>(x, w1, w3, a, B, st);
+  if (Cin == 32) return launch_mbconv_tc_s2<32, 128, 64, 2, 2>(x, w1, w3, a, B, st);
+  return launch_mbconv_tc_s2<64, 256, 128, 1, 1>(x, w1, w3, a, B, st);
 }

@@ -96,6 +96,13 @@ __device__ __forceinline__ void named_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// Per-warpgroup register reallocation (every warp of the warpgroup executes it): a TMA-only warpgroup hands registers back
+// with dec, the MMA warpgroups take them with inc.  N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // Shared-memory matrix descriptor of a bf16 operand stored with the 128-byte swizzle (what TMA SWIZZLE_128B writes):
 // 8-row atoms of 1024 B (SBO = 1024 B).  K-major: rows of 128 B along K, the leading offset unused.  MN-major: rows of
 // 128 B along M / N, one 64-element block per instruction (the leading offset unused as well).

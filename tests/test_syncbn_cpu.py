@@ -187,7 +187,9 @@ def _dp_worker(rank, world, port, q, name, img, embed, counts):
         buf_err = max(((mb[k].double() - rb[k].double()).norm() / rb[k].double().norm().clamp_min(1e-30)).item()
                       for k in rb if "running_" in k)
         nbt_ok = all(torch.equal(mb[k], rb[k]) for k in rb if "num_batches" in k)
-        flat = torch.cat([v.double().reshape(-1) for v in mb.values()])
+        # a list, not a tensor: a CPU tensor on the queue is passed as a file descriptor that the rank, exiting, may
+        # close before the parent has taken it
+        flat = torch.cat([v.double().reshape(-1) for v in mb.values()]).tolist()
         q.put((rank, out_err, gerr, buf_err, nbt_ok, flat))
         dist.destroy_process_group()
     except Exception:
@@ -202,14 +204,14 @@ def test_two_rank_syncbn_step_matches_the_global_batch(name, img, embed):
         assert gerr < 1e-5, gerr                             # fp32 accumulators in the arena are the only rounding left
         assert buf_err < 1e-6, buf_err                       # fp32 running buffers
         assert nbt_ok
-    assert torch.equal(res[0][5], res[1][5])                 # running buffers identical on both ranks
+    assert res[0][5] == res[1][5]                            # running buffers identical on both ranks
 
 
 def test_uneven_batches_give_the_global_statistics():
     res = _run(_dp_worker, 2, "efficientvit_b0", 160, 12, [1, 2])
     for _, out_err, gerr, buf_err, nbt_ok, _ in res:
         assert out_err < 1e-9 and gerr < 1e-5 and buf_err < 1e-6 and nbt_ok, (out_err, gerr, buf_err)
-    assert torch.equal(res[0][5], res[1][5])
+    assert res[0][5] == res[1][5]
 
 
 # ------------------------------------------------------------------------------------------ no synchronisation: unchanged path

@@ -176,7 +176,9 @@ def _step_worker(rank, world, port, q, backend, name, img, embed, b):
             bufs = {kk: v for kk, v in m.state_dict().items() if "running_" in kk or "num_batches" in kk}
             rbufs = {kk: v for kk, v in ref.state_dict().items() if kk in bufs}
             rel_buf = max(_rel(bufs[kk], rbufs[kk]) for kk in bufs if "running_" in kk)
-            flat = torch.cat([v.double().reshape(-1) for v in bufs.values()]).cpu()
+            # a list, not a tensor: a CPU tensor on the queue is passed as a file descriptor that the rank, exiting, may
+            # close before the parent has taken it
+            flat = torch.cat([v.double().reshape(-1) for v in bufs.values()]).cpu().tolist()
             return (_rel(out.detach(), ref_out.detach()[sl]), _rel(opt.flat_grad / k, ropt.flat_grad), rel_buf,
                     sync_bn.exchanges - e0, flat)
 
@@ -199,7 +201,7 @@ def _check_step(res, name):
         assert exch > 0
         # ... and the synchronisation is what brings them there: per-rank statistics are clearly further from the global batch
         assert plain[0] > 2 * rel_out and plain[2] > 2 * rel_buf, (plain, rel_out, rel_buf)
-    assert torch.equal(res[0][5], res[1][5])                      # running buffers bit-identical across ranks
+    assert res[0][5] == res[1][5]                                 # running buffers bit-identical across ranks
 
 
 def test_two_ranks_one_gpu_gloo_evm_step_matches_the_global_batch(cuda):
@@ -253,7 +255,9 @@ def _s0_worker(rank, world, port, q, backend):
             rbufs = {k: v for k, v in ref.state_dict().items() if k in bufs}
             rel_buf = max(_rel(bufs[k], rbufs[k]) for k in bufs if "running_" in k)
             nbt = all(torch.equal(bufs[k], rbufs[k]) for k in bufs if "num_batches" in k)
-            flat = torch.cat([v.double().reshape(-1) for v in bufs.values()]).cpu()
+            # a list, not a tensor: a CPU tensor on the queue is passed as a file descriptor that the rank, exiting, may
+            # close before the parent has taken it
+            flat = torch.cat([v.double().reshape(-1) for v in bufs.values()]).cpu().tolist()
             return _rel(mem, ref_mem[sl]), _rel(mean_g, ref_g), rel_buf, exch, flat, nbt
 
         synced = ranked(True)
@@ -275,4 +279,4 @@ def test_two_ranks_one_gpu_gloo_s0_step_matches_the_global_batch(cuda):
         assert rel_out < 2e-2 and rel_g < 5e-2 and rel_buf < 1e-3, (rel_out, rel_g, rel_buf)   # the S0 train-test tolerances
         assert exch == 8 and nbt                                  # 2 RepMixerBlocks x (2 forward + 2 backward)
         assert plain[0] > 2 * rel_out and plain[2] > 2 * rel_buf, (plain, rel_out, rel_buf)
-    assert torch.equal(res[0][5], res[1][5])
+    assert res[0][5] == res[1][5]

@@ -61,7 +61,7 @@ struct MTSmem {
   static constexpr int W1 = 2 * MT_MC * 128;
   static constexpr int W3 = 2 * COUT * 128;
   static constexpr int DW = 128 * 128;
-  static constexpr int MIDB = MT_PIN * MT_RS_MID;
+  static constexpr int MIDB = (MT_PIN + 1) * MT_RS_MID;   // + row MT_PIN: scratch for the expand's padding rows, never read
   static constexpr int OFF_W1 = IN, OFF_W3 = OFF_W1 + W1, OFF_DW = OFF_W3 + W3, OFF_MID = OFF_DW + DW;
   static constexpr int OFF_WDW = OFF_MID + (MIDB + 15) / 16 * 16;   // bf16 [MID/64][9][64]
   static constexpr int OFF_PAR = OFF_WDW + 9 * MID * 2;              // fp32 s1[MID] b1[MID] b2[MID] s3[COUT] b3[COUT]
@@ -188,16 +188,43 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
     const int prb0 = COUT == 64 ? 0 : hsel, pcol0 = COUT == 64 ? hsel * 32 : 0;
     float proj[PRB][16];
     int gc = 0;
+    // descriptors of the operands' first K-step; every other one is a constant offset from these (ptx::desc_advance)
+    const uint64_t d_in = ptx::make_desc_sw128(u_in), d_dw = ptx::make_desc_sw128(u_dw + prb0 * 8192);
+    const uint64_t d_w1 = ptx::make_desc_sw128(ptx::smem_u32(s_w1) + hsel * 4096);
+    const uint64_t d_w3 = ptx::make_desc_sw128(ptx::smem_u32(s_w3) + pcol0 * 128);
+    // the thread's six expand fragment rows (block mb, half h: pixel mb * 64 + 16 q + g + 8 h) and their s_mid byte offsets,
+    // fixed for the kernel; the padding rows (>= MT_PIN) all write the scratch row, so the epilogue stores without a branch
+    uint32_t mid_off[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      const int row = (k >> 1) * 64 + 16 * q + g + 8 * (k & 1);
+      mid_off[k] = (uint32_t)((row < MT_PIN ? row : MT_PIN) * MT_RS_MID + (hsel * 32 + 2 * t4) * 2);
+    }
 
 #pragma unroll 1
     for (int it = 0; it < my_tiles; ++it) {
       const int t = (int)blockIdx.x + it * (int)gridDim.x;
       const int b = t / tiles_per_img, tr = t % tiles_per_img;
       const int oy0 = (tr / a.tiles_x) * MT_TH, ox0 = (tr % a.tiles_x) * MT_TW;
-      const int iy0 = oy0 - 1, ix0 = ox0 - 1;
+      // bit k: fragment row k lies inside the image (outside it, and on the padding rows, the expand output is the
+      // depthwise's zero padding)
+      uint32_t in_mask = 0;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) {
+        const int row = (k >> 1) * 64 + 16 * q + g + 8 * (k & 1);
+        const int iy = oy0 - 1 + row / MT_HW, ix = ox0 - 1 + row % MT_HW;
+        if (row < MT_PIN && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W) in_mask |= 1u << k;
+      }
 #pragma unroll 1
       for (int c = 0; c < NC; ++c, ++gc) {
         const int st = gc & 1;
+        // the BN1 scale / bias of the thread's four column pairs (hsel * 32 + 8 j + 2 t4) of this chunk
+        float2 sc[4], bi[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          sc[j] = *reinterpret_cast<const float2*>(s_s1 + c * MT_MC + hsel * 32 + 8 * j + 2 * t4);
+          bi[j] = *reinterpret_cast<const float2*>(s_b1 + c * MT_MC + hsel * 32 + 8 * j + 2 * t4);
+        }
         // ---- expand: D_exp[192 x 32] = s_in (three 64-row blocks; rows >= 180 are padding) x W1c[hsel*32 .. +32]^T
         if (c == 0) ptx::mbar_wait(bar_in, (uint32_t)(it & 1));
         ptx::mbar_wait(bar_w1 + st, (uint32_t)((gc >> 1) & 1));
@@ -205,9 +232,9 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         ptx::wg_fence();
 #pragma unroll
         for (int k = 0; k < CIN / 16; ++k) {
-          const uint64_t db = ptx::make_desc_sw128(ptx::smem_u32(s_w1 + st * W1_BYTES) + hsel * 4096 + k * 32);
+          const uint64_t db = ptx::desc_advance(d_w1, st * W1_BYTES + k * 32);
 #pragma unroll
-          for (int mb = 0; mb < 3; ++mb) ptx::wgmma_m64n32<0, 0>(ex[mb], ptx::make_desc_sw128(u_in + mb * 8192 + k * 32), db, k != 0);
+          for (int mb = 0; mb < 3; ++mb) ptx::wgmma_m64n32<0, 0>(ex[mb], ptx::desc_advance(d_in, mb * 8192 + k * 32), db, k != 0);
         }
         ptx::wg_commit();
         ptx::wg_wait<0>();                                 // also retires project(gc-1), still in flight unless c == 0
@@ -220,21 +247,18 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         }
         compute_bar_sync();                              // every warp is done reading s_mid for the previous chunk
         // ---- expand epilogue: BN1 + act, zero outside the image, bf16 -> s_mid[row][hsel*32 .. +32)
+        // (element 4 j + 2 h of ex[mb] is row k = 2 mb + h, column pair j)
 #pragma unroll
-        for (int mb = 0; mb < 3; ++mb)
+        for (int k = 0; k < 6; ++k) {
+          const bool in = (in_mask >> k) & 1u;
 #pragma unroll
-          for (int i = 0; i < 16; i += 2) {
-            const int row = mb * 64 + ptx::wg_frag_row(q, lane, i), col = hsel * 32 + ptx::wg_frag_col(lane, i);
-            if (row < MT_PIN) {
-              const int iy = iy0 + row / MT_HW, ix = ix0 + row % MT_HW;
-              const bool in = iy >= 0 && iy < a.H && ix >= 0 && ix < a.W;   // outside the image: the depthwise's zero padding
-              const float2 sc = *reinterpret_cast<const float2*>(s_s1 + c * MT_MC + col);
-              const float2 bi = *reinterpret_cast<const float2*>(s_b1 + c * MT_MC + col);
-              const float v0 = in ? es3_act_t<ACT>(fmaf(ex[mb][i], sc.x, bi.x)) : 0.f;
-              const float v1 = in ? es3_act_t<ACT>(fmaf(ex[mb][i + 1], sc.y, bi.y)) : 0.f;
-              *reinterpret_cast<uint32_t*>(s_mid + row * MT_RS_MID + col * 2) = pack_bf16x2(v0, v1);
-            }
+          for (int j = 0; j < 4; ++j) {
+            const float* e = &ex[k >> 1][4 * j + 2 * (k & 1)];
+            const float v0 = in ? es3_act_t<ACT>(fmaf(e[0], sc[j].x, bi[j].x)) : 0.f;
+            const float v1 = in ? es3_act_t<ACT>(fmaf(e[1], sc[j].y, bi[j].y)) : 0.f;
+            *reinterpret_cast<uint32_t*>(s_mid + mid_off[k] + 16 * j) = pack_bf16x2(v0, v1);
           }
+        }
         compute_bar_sync();                              // s_mid complete (and project(gc-1) of both warpgroups retired)
 
         // ---- depthwise 3x3 on tensor cores (diagonal-B MMAs): warp -> channel group cg (16 ch), output rows hsel*4 .. hsel*4+3.
@@ -276,7 +300,9 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
               mma_1688(dacc[m][1], af[m + 2][2], af[m + 2][3], b_hi[2]);
             }
           }
-          const float* b2 = s_b2 + c * MT_MC;
+          float2 bb[2];                                   // bias of channels cg * 16 + nt * 8 + 2 t4
+#pragma unroll
+          for (int nt = 0; nt < 2; ++nt) bb[nt] = *reinterpret_cast<const float2*>(s_b2 + c * MT_MC + cg * 16 + nt * 8 + t4 * 2);
 #pragma unroll
           for (int m = 0; m < 4; ++m) {
             const int mt = hsel * 4 + m;
@@ -285,10 +311,8 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
               const int p = mt * MT_TW + g + half * 8;     // output pixel = A-operand row of the project wgmma
 #pragma unroll
               for (int nt = 0; nt < 2; ++nt) {
-                const int ch = cg * 16 + nt * 8 + t4 * 2;
-                const float2 bb = *reinterpret_cast<const float2*>(b2 + ch);
-                const float v0 = es3_act_t<ACT>(dacc[m][nt][half * 2 + 0] + bb.x);
-                const float v1 = es3_act_t<ACT>(dacc[m][nt][half * 2 + 1] + bb.y);
+                const float v0 = es3_act_t<ACT>(dacc[m][nt][half * 2 + 0] + bb[nt].x);
+                const float v1 = es3_act_t<ACT>(dacc[m][nt][half * 2 + 1] + bb[nt].y);
                 const int j = cg * 2 + nt;                  // 16-byte chunk inside the 128-byte row; XOR-swizzled by row % 8
                 *reinterpret_cast<uint32_t*>(s_dw + p * 128 + ((j ^ (p & 7)) << 4) + t4 * 4) = pack_bf16x2(v0, v1);
               }
@@ -302,10 +326,10 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         ptx::wg_fence();
 #pragma unroll
         for (int k = 0; k < MT_MC / 16; ++k) {
-          const uint64_t db = ptx::make_desc_sw128(ptx::smem_u32(s_w3 + st * W3_BYTES) + pcol0 * 128 + k * 32);
+          const uint64_t db = ptx::desc_advance(d_w3, st * W3_BYTES + k * 32);
 #pragma unroll
           for (int rb = 0; rb < PRB; ++rb)
-            ptx::wgmma_m64n32<0, 0>(proj[rb], ptx::make_desc_sw128(u_dw + (prb0 + rb) * 8192 + k * 32), db, (c | k) != 0);
+            ptx::wgmma_m64n32<0, 0>(proj[rb], ptx::desc_advance(d_dw, rb * 8192 + k * 32), db, (c | k) != 0);
         }
         ptx::wg_commit();                                // retired by the next chunk's expand wait, or below
       }
@@ -314,21 +338,37 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(bar_w3free + ((gc - 1) & 1));
 
-      // ---- final epilogue: BN3 + residual (x re-read from global / L2) -> global, from the accumulator fragments
+      // ---- final epilogue: BN3 + residual (x re-read from global / L2) -> global, from the accumulator fragments.  Output
+      // pixel r of the tile (row r / 16, column r % 16) is 32-bit element offset ((r / 16) W + r % 16) COUT from the tile's
+      // first pixel; the thread's rows are (prb0 + rb) * 64 + 16 q + g + 8 h, its columns pcol0 + 8 j + 2 t4.
+      {
+        const long long tile0 = (((long long)b * a.H + oy0) * a.W + ox0) * COUT + pcol0 + 2 * t4;
+        const bf16* xt = a.x + tile0;
+        bf16* yt = a.y + tile0;
+        float2 s3[4], b3[4];
 #pragma unroll
-      for (int rb = 0; rb < PRB; ++rb)
-#pragma unroll
-        for (int i = 0; i < 16; i += 2) {
-          const int r = (prb0 + rb) * 64 + ptx::wg_frag_row(q, lane, i), col = pcol0 + ptx::wg_frag_col(lane, i);
-          const int oy = oy0 + r / MT_TW, ox = ox0 + r % MT_TW;
-          if (oy < a.H && ox < a.W) {
-            const long long pix = (((long long)b * a.H + oy) * a.W + ox) * COUT + col;
-            const float2 xr = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(a.x + pix)));
-            const float f0 = fmaf(proj[rb][i], s_s3[col], s_b3[col]) + xr.x;
-            const float f1 = fmaf(proj[rb][i + 1], s_s3[col + 1], s_b3[col + 1]) + xr.y;
-            *reinterpret_cast<uint32_t*>(a.y + pix) = pack_bf16x2(f0, f1);
-          }
+        for (int j = 0; j < 4; ++j) {
+          s3[j] = *reinterpret_cast<const float2*>(s_s3 + pcol0 + 8 * j + 2 * t4);
+          b3[j] = *reinterpret_cast<const float2*>(s_b3 + pcol0 + 8 * j + 2 * t4);
         }
+#pragma unroll
+        for (int rb = 0; rb < PRB; ++rb)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int ly = (prb0 + rb) * 4 + q, lx = g + 8 * h;
+            if (oy0 + ly < a.H && ox0 + lx < a.W) {
+              const int off = (ly * a.W + lx) * COUT;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const float* p = &proj[rb][4 * j + 2 * h];
+                const float2 xr = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(xt + off + 8 * j)));
+                const float f0 = fmaf(p[0], s3[j].x, b3[j].x) + xr.x;
+                const float f1 = fmaf(p[1], s3[j].y, b3[j].y) + xr.y;
+                *reinterpret_cast<uint32_t*>(yt + off + 8 * j) = pack_bf16x2(f0, f1);
+              }
+            }
+          }
+      }
     }
   }
 }

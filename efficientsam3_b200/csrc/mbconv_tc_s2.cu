@@ -43,6 +43,7 @@ constexpr int S2_RS_MID = S2_MC * 2 + 16;                  // 80-byte rows: conf
 // slot S2_ODD + j).  A stride-2 tap then walks CONSECUTIVE 80-byte rows (8 rows -> 8 distinct 4-bank groups); walking every other
 // row of an interleaved tile (160-byte stride) made every ldmatrix 2-way conflicted.  S2_ODD = 20 also keeps the expand epilogue's 16-byte stores (lanes alternate planes) apart.
 constexpr int S2_ODD = 20, S2_PW = S2_ODD + S2_TW;           // slots per input row: 17 even | 3 unused | 16 odd
+constexpr int S2_SCRATCH = 17;                              // unused slot 17 of input row 0: the expand's padding rows write it
 constexpr int S2_THREADS = 384;                           // two compute warpgroups + one TMA warpgroup
 
 template <int MID, int COUT, int WSTAGES>
@@ -179,16 +180,45 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
     const int pc0 = COUT >= 64 ? hsel * PN : 0;
     float proj[PN / 2];
     int g = 0;
+    // descriptors of the operands' first K-step; every other one is a constant offset from these (ptx::desc_advance)
+    const uint64_t d_in = ptx::make_desc_sw128(u_in + hsel * 8192), d_dw = ptx::make_desc_sw128(u_dw);
+    const uint64_t d_w1 = ptx::make_desc_sw128(ptx::smem_u32(s_w1));
+    const uint64_t d_w3 = ptx::make_desc_sw128(ptx::smem_u32(s_w3) + pc0 * 128);
+    // the thread's expand fragment rows (block j, half h: input pixel (2 j + hsel) * 64 + 16 q + g4 + 8 h; warpgroup 1 has no
+    // block j = 2) and their s_mid byte offsets in the even / odd column planes, fixed for the kernel; the padding rows
+    // (>= S2_PIN) all write the scratch slot, so the epilogue stores without a branch
+    uint32_t mid_off[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      const int row = (2 * (k >> 1) + hsel) * 64 + 16 * q + g4 + 8 * (k & 1), lx = row % S2_IW;
+      const int slot = row < S2_PIN ? (row / S2_IW) * S2_PW + ((lx & 1) ? S2_ODD + (lx >> 1) : (lx >> 1)) : S2_SCRATCH;
+      mid_off[k] = (uint32_t)(slot * S2_RS_MID + 2 * t4 * 2);
+    }
 
 #pragma unroll 1
     for (int it = 0; it < my_tiles; ++it) {
       const int t = (int)blockIdx.x + it * (int)gridDim.x;
       const int b = t / tiles_per_img, tr = t % tiles_per_img;
       const int oy0 = (tr / a.tiles_x) * S2_TH, ox0 = (tr % a.tiles_x) * S2_TW;
-      const int iy0 = 2 * oy0 - 1, ix0 = 2 * ox0 - 1;
+      // bit k: fragment row k lies inside the image (outside it, and on the padding rows, the expand output is the
+      // depthwise's zero padding)
+      uint32_t in_mask = 0;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) {
+        const int row = (2 * (k >> 1) + hsel) * 64 + 16 * q + g4 + 8 * (k & 1);
+        const int iy = 2 * oy0 - 1 + row / S2_IW, ix = 2 * ox0 - 1 + row % S2_IW;
+        if (row < S2_PIN && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W) in_mask |= 1u << k;
+      }
 #pragma unroll 1
       for (int c = 0; c < NC; ++c, ++g) {
         const int st = g & 1, ws = (WSTAGES == 2) ? (g & 1) : 0;
+        // the BN1 scale / bias of the thread's four column pairs (8 j + 2 t4) of this chunk
+        float2 sc[4], bi[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          sc[j] = *reinterpret_cast<const float2*>(s_s1 + c * S2_MC + 8 * j + 2 * t4);
+          bi[j] = *reinterpret_cast<const float2*>(s_b1 + c * S2_MC + 8 * j + 2 * t4);
+        }
         // ---- expand: D_exp[rows of my blocks][32] = s_in x W1c^T
         if (c == 0) ptx::mbar_wait(bar_in, (uint32_t)(it & 1));
         ptx::mbar_wait(bar_w1 + st, (uint32_t)((g >> 1) & 1));
@@ -196,12 +226,12 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
         ptx::wg_fence();
 #pragma unroll
         for (int k = 0; k < CIN / 16; ++k) {
-          const uint64_t db = ptx::make_desc_sw128(ptx::smem_u32(s_w1 + st * W1_BYTES) + k * 32);
+          const uint64_t db = ptx::desc_advance(d_w1, st * W1_BYTES + k * 32);
 #pragma unroll
           for (int j = 0; j < 3; ++j) {
             // warpgroup 1 has two blocks; its third MMA repeats block 3 and is discarded, so no wgmma sits on a divergent path
-            const int mb = (j == 2 && hsel == 1) ? 3 : 2 * j + hsel;
-            ptx::wgmma_m64n32<0, 0>(ex[j], ptx::make_desc_sw128(u_in + mb * 8192 + k * 32), db, k != 0);
+            const int mb_off = (j == 2 && hsel == 1) ? 2 : 2 * j;   // block 2 j + hsel, relative to d_in's block hsel
+            ptx::wgmma_m64n32<0, 0>(ex[j], ptx::desc_advance(d_in, mb_off * 8192 + k * 32), db, k != 0);
           }
         }
         ptx::wg_commit();
@@ -215,24 +245,17 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
         }
         compute_bar_sync();                                // every warp is done reading s_mid for the previous chunk
         // ---- expand epilogue: BN1 + act, zero outside the image, bf16 -> s_mid (even / odd column planes)
+        // (element 4 jc + 2 h of ex[j] is row k = 2 j + h, column pair jc)
 #pragma unroll
-        for (int j = 0; j < 3; ++j) {
-          if (j == 2 && hsel == 1) break;
-          const int mb = 2 * j + hsel;
+        for (int k = 0; k < 6; ++k) {
+          if (k >= 4 && hsel == 1) break;
+          const bool in = (in_mask >> k) & 1u;
 #pragma unroll
-          for (int i = 0; i < 16; i += 2) {
-            const int row = mb * 64 + ptx::wg_frag_row(q, lane, i), col = ptx::wg_frag_col(lane, i);
-            if (row < S2_PIN) {
-              const int iy = iy0 + row / S2_IW, ix = ix0 + row % S2_IW;
-              const bool in = iy >= 0 && iy < a.H && ix >= 0 && ix < a.W;   // outside the image: the depthwise's zero padding
-              const int lx = row % S2_IW;
-              const float2 sc = *reinterpret_cast<const float2*>(s_s1 + c * S2_MC + col);
-              const float2 bi = *reinterpret_cast<const float2*>(s_b1 + c * S2_MC + col);
-              const float v0 = in ? es3_act_t<ACT>(fmaf(ex[j][i], sc.x, bi.x)) : 0.f;
-              const float v1 = in ? es3_act_t<ACT>(fmaf(ex[j][i + 1], sc.y, bi.y)) : 0.f;
-              *reinterpret_cast<uint32_t*>(s_mid + ((row / S2_IW) * S2_PW + ((lx & 1) ? S2_ODD + (lx >> 1) : (lx >> 1))) * S2_RS_MID +
-                                           col * 2) = pack_bf16x2(v0, v1);
-            }
+          for (int jc = 0; jc < 4; ++jc) {
+            const float* e = &ex[k >> 1][4 * jc + 2 * (k & 1)];
+            const float v0 = in ? es3_act_t<ACT>(fmaf(e[0], sc[jc].x, bi[jc].x)) : 0.f;
+            const float v1 = in ? es3_act_t<ACT>(fmaf(e[1], sc[jc].y, bi[jc].y)) : 0.f;
+            *reinterpret_cast<uint32_t*>(s_mid + mid_off[k] + 16 * jc) = pack_bf16x2(v0, v1);
           }
         }
         compute_bar_sync();                                // s_mid complete (and project(g-1) of both warpgroups retired)
@@ -272,16 +295,16 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
             mma_1688(dacc[0], fa[0], fa[1], la);
             mma_1688(dacc[1], fa[2], fa[3], ha);
           }
-          const float* b2 = s_b2 + c * S2_MC;
+          float2 bb[2];                                     // bias of channels cg * 16 + nt * 8 + 2 t4
+#pragma unroll
+          for (int nt = 0; nt < 2; ++nt) bb[nt] = *reinterpret_cast<const float2*>(s_b2 + c * S2_MC + cg * 16 + nt * 8 + t4 * 2);
 #pragma unroll
           for (int half = 0; half < 2; ++half) {
             const int p = mt * S2_TW + g4 + half * 8;      // output pixel = A-operand row (0..63) of the project wgmma
 #pragma unroll
             for (int nt = 0; nt < 2; ++nt) {
-              const int ch = cg * 16 + nt * 8 + t4 * 2;
-              const float2 bb = *reinterpret_cast<const float2*>(b2 + ch);
-              const float v0 = es3_act_t<ACT>(dacc[nt][half * 2 + 0] + bb.x);
-              const float v1 = es3_act_t<ACT>(dacc[nt][half * 2 + 1] + bb.y);
+              const float v0 = es3_act_t<ACT>(dacc[nt][half * 2 + 0] + bb[nt].x);
+              const float v1 = es3_act_t<ACT>(dacc[nt][half * 2 + 1] + bb[nt].y);
               const int j = cg * 2 + nt;                    // 16-byte chunk 0..3 of the 128-byte row, XOR-swizzled by row % 8
               *reinterpret_cast<uint32_t*>(s_dw + p * 128 + ((j ^ (p & 7)) << 4) + t4 * 4) = pack_bf16x2(v0, v1);
             }
@@ -295,8 +318,8 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
         ptx::wg_fence();
 #pragma unroll
         for (int k = 0; k < S2_MC / 16; ++k) {
-          const uint64_t da = ptx::make_desc_sw128(u_dw + k * 32);
-          const uint64_t db = ptx::make_desc_sw128(ptx::smem_u32(s_w3 + ws * W3_BYTES) + pc0 * 128 + k * 32);
+          const uint64_t da = ptx::desc_advance(d_dw, k * 32);
+          const uint64_t db = ptx::desc_advance(d_w3, ws * W3_BYTES + k * 32);
           if constexpr (PN == 64) ptx::wgmma_m64n64<0, 0>(proj, da, db, (c | k) != 0);
           else ptx::wgmma_m64n32<0, 0>(proj, da, db, (c | k) != 0);
         }
@@ -308,15 +331,21 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
       if (lane == 0) ptx::mbar_arrive(bar_w3free + ((WSTAGES == 2) ? ((g - 1) & 1) : 0));
 
       // ---- final epilogue: BN3 -> global, from the accumulator fragments
+      // (output pixel r = 16 q + g4 + 8 h of the tile is row q, column g4 + 8 h; element 4 j + 2 h is column pc0 + 8 j + 2 t4)
       if (pact) {
+        bf16* yt = a.y + (((long long)b * a.Ho + oy0) * a.Wo + ox0) * COUT + pc0 + 2 * t4;
 #pragma unroll
-        for (int i = 0; i < PN / 2; i += 2) {
-          const int r = ptx::wg_frag_row(q, lane, i), col = pc0 + ptx::wg_frag_col(lane, i);
-          const int oy = oy0 + r / S2_TW, ox = ox0 + r % S2_TW;
-          if (oy < a.Ho && ox < a.Wo) {
-            const long long pix = (((long long)b * a.Ho + oy) * a.Wo + ox) * COUT + col;
-            *reinterpret_cast<uint32_t*>(a.y + pix) =
-                pack_bf16x2(fmaf(proj[i], s_s3[col], s_b3[col]), fmaf(proj[i + 1], s_s3[col + 1], s_b3[col + 1]));
+        for (int h = 0; h < 2; ++h) {
+          const int lx = g4 + 8 * h;
+          if (oy0 + q < a.Ho && ox0 + lx < a.Wo) {
+            const int off = (q * a.Wo + lx) * COUT;
+#pragma unroll
+            for (int j = 0; j < PN / 8; ++j) {
+              const int col = pc0 + 8 * j + 2 * t4;
+              const float2 s3 = *reinterpret_cast<const float2*>(s_s3 + col), b3 = *reinterpret_cast<const float2*>(s_b3 + col);
+              *reinterpret_cast<uint32_t*>(yt + off + 8 * j) =
+                  pack_bf16x2(fmaf(proj[4 * j + 2 * h], s3.x, b3.x), fmaf(proj[4 * j + 2 * h + 1], s3.y, b3.y));
+            }
           }
         }
       }

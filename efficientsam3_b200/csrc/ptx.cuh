@@ -116,6 +116,12 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;
   return d;
 }
+// make_desc_sw128(addr + off) from d = make_desc_sw128(addr), for off a multiple of 16 with addr + off inside the CTA's shared
+// memory: the start field holds (addr >> 4) in 14 bits and every shared address is below 2^18 (228 KB on sm_90), so the field
+// never carries into the LBO bits and one 32-bit add on the low word does it.
+__device__ __forceinline__ uint64_t desc_advance(uint64_t d, uint32_t off) {
+  return ((d >> 32) << 32) | (uint32_t)((uint32_t)d + (off >> 4));
+}
 
 // D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T, fp32 accumulator fragment d[16] (see wg_frag_row / wg_frag_col).
 template <int TA, int TB>

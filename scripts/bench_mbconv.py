@@ -1,7 +1,7 @@
 """Time the fused MBConv kernels (mbconv_tc, mbconv_tc_s2, dwproj_tc) one instantiation at a time, at the shapes the EV-M
 student runs them at in bench.py (batch 32, 1024^2 input), and check each output against the op-by-op statement.
 
-    python scripts/bench_mbconv.py [--lib PATH] [--batch 32] [--img 1024] [--seconds 1.0] [--json OUT]
+    python scripts/bench_mbconv.py [--lib PATH] [--batch 32] [--img 1024] [--seconds 1.0] [--json OUT] [--save-outputs DIR]
 
 --lib loads another build of libes3.so (same C ABI), so that two builds can be timed alternately, one process each.  Prints one
 JSON line: per instantiation the kernel time (CUDA events over enough launches to run for --seconds after warm-up), the
@@ -66,7 +66,7 @@ def _time(run, seconds):
     return e0.elapsed_time(e1) / n, n
 
 
-def bench_case(ops, name, kind, cin, mid, cout, stride, side, B, seconds, dev):
+def bench_case(ops, name, kind, cin, mid, cout, stride, side, B, seconds, dev, save_dir=None):
     g = torch.Generator().manual_seed(mid + side + stride)
     bf = lambda t: t.to(torch.bfloat16).to(dev)
     H = W = side
@@ -99,6 +99,10 @@ def bench_case(ops, name, kind, cin, mid, cout, stride, side, B, seconds, dev):
         resid = xn if res else None
     y = run()
     assert y is not None, f"{name}: not instantiated"
+    if save_dir:
+        # the kernel's bf16 output bits, so that two builds can be compared bit for bit (inputs are seeded per instantiation)
+        tag = "".join(ch if ch.isalnum() else "_" for ch in name).strip("_")
+        torch.save(y.view(torch.int16).cpu(), os.path.join(save_dir, f"{tag}.pt"))
     d = F.hardswish(d).to(torch.bfloat16).float()
     ref = F.conv2d(d, w3.float()[:, :, None, None]) * s3.view(1, -1, 1, 1) + b3.view(1, -1, 1, 1)
     del d
@@ -121,7 +125,11 @@ def main():
     ap.add_argument("--seconds", type=float, default=1.0, help="timed window per instantiation (after warm-up)")
     ap.add_argument("--only", default=None, help="substring of the instantiation names to run")
     ap.add_argument("--json", default=None, help="also write the result line to this file")
+    ap.add_argument("--save-outputs", default=None, metavar="DIR",
+                    help="write each instantiation's output (bf16 bits as int16, <name>.pt) under DIR")
     args = ap.parse_args()
+    if args.save_outputs:
+        os.makedirs(args.save_outputs, exist_ok=True)
     if not torch.cuda.is_available():
         sys.exit("bench_mbconv: no CUDA device")
     from efficientsam3_b200 import _lib
@@ -130,7 +138,8 @@ def main():
     from efficientsam3_b200 import ops
     _lib.init(0)
     dev = torch.device("cuda", 0)
-    rows = [bench_case(ops, *c, args.batch, args.seconds, dev) for c in cases(args.img) if not args.only or args.only in c[0]]
+    rows = [bench_case(ops, *c, args.batch, args.seconds, dev, args.save_outputs) for c in cases(args.img)
+            if not args.only or args.only in c[0]]
     out = {"gpu": _gpu_info(), "lib": str(_lib.LIB_PATH), "batch": args.batch, "img": args.img, "kernels": rows,
            "total_ms": round(sum(r["ms"] for r in rows), 4), "total_bytes": sum(r["bytes"] for r in rows),
            "all_ok": all(r["ok"] for r in rows)}

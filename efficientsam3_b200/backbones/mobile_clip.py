@@ -679,19 +679,23 @@ class RepMixerUnit:
             return p
         return cached_pack(blk, "train_fold", blk.layer_scale, build)
 
-    def forward(self, x, B, L):
+    def prologue(self, x, B, L):
+        """(x1 fp32, u bf16, the parameter pack, what the conv + BatchNorm backward needs besides)."""
         p = self._pack()
-        x1, u = ops.repmixer(x, B, L, p["wm"], p["bm"], p["wf"], p["bf"])
+        return (*ops.repmixer(x, B, L, p["wm"], p["bm"], p["wf"], p["bf"]), p, None)
+
+    def forward(self, x, B, L):
+        x1, u, p, bn = self.prologue(x, B, L)
         h = self.fc1.forward(u)
         x2 = ops.gemm(h, self.fc2._w(), scale=p["lsb"], bias=p["b2s"], residual=x1, out_dtype=torch.float32)
-        self.saved = (x, x1, h, p, B, L)
+        self.saved = (x, x1, h, p, bn, B, L)
         return x2
 
     def backward(self, g, gb, grads, want_bf16=True):
         """g: fp32 gradient of the block output (gb, its bf16 copy, is not needed) -> (fp32 input gradient, bf16 copy | None)."""
-        x, x1, h, p, B, L = self.saved
+        x, x1, h, p, bn, B, L = self.saved
         self.saved = None
-        tm, ffn = self.tm, self.ffn
+        ffn = self.ffn
         y = ops.gemm(h, self.fc2._w(), bias=p["b2"], out_dtype=torch.float32)
         dy = ops.repmixer_ls_bwd(g, y, p["lsb"], B, L, dls=_grad_of(grads, self.blk.layer_scale),
                                  dbias=_grad_of(grads, ffn.fc2.bias))
@@ -699,13 +703,17 @@ class RepMixerUnit:
         if gw2 is not None:
             ops.wgrad_pw(dy, h, gw2)
         du = self.fc1.backward(ops.gemm(dy, self.fc2._wt()), grads, out_dtype=torch.float32)
-        bnf = ffn.conv.bn
-        e = ops.repmixer_ffn_bwd(x1, du, g, p["f_taps"], p["bnf"], B, L, dtaps=_grad_of(grads, ffn.conv.conv.weight),
-                                 dgamma=_grad_of(grads, bnf.weight), dbeta=_grad_of(grads, bnf.bias))
-        bns = (tm.mixer.rbr_skip, tm.mixer.rbr_conv[0].bn, tm.norm.rbr_skip)
-        return ops.repmixer_tm_bwd(x, e, p["tm_taps"], p["bnp"], B, L, dtaps=_grad_of(grads, tm.mixer.rbr_conv[0].conv.weight),
-                                   dls=_grad_of(grads, tm.layer_scale),
-                                   dbn=[_grad_of(grads, t) for bn in bns for t in (bn.weight, bn.bias)], want_bf16=want_bf16)
+        dbn = [_grad_of(grads, t) for b in repmixer_bns(self.blk) for t in (b.weight, b.bias)]
+        dst = (_grad_of(grads, ffn.conv.conv.weight), _grad_of(grads, self.tm.mixer.rbr_conv[0].conv.weight),
+               _grad_of(grads, self.tm.layer_scale), dbn)
+        return self.conv_bn_backward(x, x1, du, g, p, bn, B, L, dst, want_bf16)
+
+    def conv_bn_backward(self, x, x1, du, g, p, bn, B, L, dst, want_bf16):
+        """The two depthwise convs and their BatchNorms: du (fc1's input gradient) and g -> the block's input gradient.  dst: the
+        gradients of the ConvFFN taps, the token-mixer taps, its layer scale and (gamma, beta) x (BN_ms, BN_mc, BN_ns, BN_f)."""
+        d_ftaps, d_mtaps, d_ls, dbn = dst
+        e = ops.repmixer_ffn_bwd(x1, du, g, p["f_taps"], p["bnf"], B, L, dtaps=d_ftaps, dgamma=dbn[6], dbeta=dbn[7])
+        return ops.repmixer_tm_bwd(x, e, p["tm_taps"], p["bnp"], B, L, dtaps=d_mtaps, dls=d_ls, dbn=dbn[:6], want_bf16=want_bf16)
 
 
 class RepMixerBatchStatUnit(RepMixerUnit):
@@ -719,43 +727,23 @@ class RepMixerBatchStatUnit(RepMixerUnit):
         super().__init__(blk)
         self.enc = enc
 
-    def forward(self, x, B, L):
+    def prologue(self, x, B, L):
         x1, u, stats, p, sync = repmixer_bn_forward(self.blk, x, B, L)
         invalidate_running_folds(self.enc)
-        h = self.fc1.forward(u)
-        x2 = ops.gemm(h, self.fc2._w(), scale=p["lsb"], bias=p["b2s"], residual=x1, out_dtype=torch.float32)
-        self.saved = (x, x1, h, p, stats, sync, B, L)
-        return x2
+        return x1, u, p, (stats, sync)
 
-    def backward(self, g, gb, grads, want_bf16=True):
-        x, x1, h, p, stats, sync, B, L = self.saved
-        self.saved = None
-        tm, ffn = self.tm, self.ffn
-        y = ops.gemm(h, self.fc2._w(), bias=p["b2"], out_dtype=torch.float32)
-        dy = ops.repmixer_ls_bwd(g, y, p["lsb"], B, L, dls=_grad_of(grads, self.blk.layer_scale),
-                                 dbias=_grad_of(grads, ffn.fc2.bias))
-        gw2 = _grad_of(grads, ffn.fc2.weight)
-        if gw2 is not None:
-            ops.wgrad_pw(dy, h, gw2)
-        du = self.fc1.backward(ops.gemm(dy, self.fc2._wt()), grads, out_dtype=torch.float32)
-        bnf = ffn.conv.bn
-        bns = repmixer_bns(self.blk)[:3]
-        dbn = [_grad_of(grads, t) for bn in bns for t in (bn.weight, bn.bias)]
-        d_ftaps, d_mtaps = _grad_of(grads, ffn.conv.conv.weight), _grad_of(grads, tm.mixer.rbr_conv[0].conv.weight)
+    def conv_bn_backward(self, x, x1, du, g, p, bn, B, L, dst, want_bf16):
+        (stats, sync), (d_ftaps, d_mtaps, d_ls, dbn), taps, aff = bn, dst, p["taps"], p["aff"]
         if sync is None:
-            e = ops.repmixer_bn_ffn_bwd(x1, du, g, p["taps"], p["aff"], stats, B, L, dtaps=d_ftaps, dgamma=_grad_of(grads, bnf.weight),
-                                        dbeta=_grad_of(grads, bnf.bias))
-            return ops.repmixer_bn_tm_bwd(x, e, p["taps"], p["aff"], stats, B, L, dtaps=d_mtaps, dls=_grad_of(grads, tm.layer_scale),
-                                          dbn=dbn, want_bf16=want_bf16)
+            e = ops.repmixer_bn_ffn_bwd(x1, du, g, taps, aff, stats, B, L, dtaps=d_ftaps, dgamma=dbn[6], dbeta=dbn[7])
+            return ops.repmixer_bn_tm_bwd(x, e, taps, aff, stats, B, L, dtaps=d_mtaps, dls=d_ls, dbn=dbn[:6], want_bf16=want_bf16)
         # synchronised: each BN sum is all-gathered and added in rank order; the BNs' gamma / beta gradients stay this rank's own
         group, total = sync
-        sums = ops.repmixer_bn_ffn_sums(x1, du, p["taps"], stats, B, L, p["aff"], dgamma=_grad_of(grads, bnf.weight),
-                                        dbeta=_grad_of(grads, bnf.bias))
-        e = ops.repmixer_bn_ffn_apply(x1, du, g, p["taps"], p["aff"], stats, sync_bn.all_gather_partials(sums, group), total, B, L,
-                                      dtaps=d_ftaps)
-        sums = ops.repmixer_bn_tm_sums(x, e, p["taps"], p["aff"], stats, B, L, dbn=dbn)
-        return ops.repmixer_bn_tm_apply(x, e, p["taps"], p["aff"], stats, sync_bn.all_gather_partials(sums, group), total, B, L,
-                                        dtaps=d_mtaps, dls=_grad_of(grads, tm.layer_scale), want_bf16=want_bf16)
+        sums = ops.repmixer_bn_ffn_sums(x1, du, taps, stats, B, L, aff, dgamma=dbn[6], dbeta=dbn[7])
+        e = ops.repmixer_bn_ffn_apply(x1, du, g, taps, aff, stats, sync_bn.all_gather_partials(sums, group), total, B, L, dtaps=d_ftaps)
+        sums = ops.repmixer_bn_tm_sums(x, e, taps, aff, stats, B, L, dbn=dbn[:6])
+        return ops.repmixer_bn_tm_apply(x, e, taps, aff, stats, sync_bn.all_gather_partials(sums, group), total, B, L, dtaps=d_mtaps,
+                                        dls=d_ls, want_bf16=want_bf16)
 
 
 class TextEmbedUnit:

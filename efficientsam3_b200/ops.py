@@ -617,73 +617,16 @@ def repmixer_tm_bwd(x, e, taps, bnp, B, L, dtaps=None, dls=None, dbn=(None,) * 6
 KERNELS_PER_CALL.update({"es3_repmixer_bn_fwd": 5, "es3_repmixer_bn_ffn_bwd": 4, "es3_repmixer_bn_tm_bwd": 4})
 
 
-def _repmixer_bn_args(name, rows, B, L, taps, aff, stats=None):
-    """_repmixer_bwd_args plus B*L >= 2 (a batch statistic needs more than one value per channel, as nn.BatchNorm2d requires);
-    taps [2, 11, C], aff [9, C], stats [8, C] fp32 contiguous."""
-    if B * L < 2:
+def _repmixer_bn_args(name, rows, B, L, taps, aff=None, stats=None, fold=None, own_stats=False):
+    """_repmixer_bwd_args for the batch-statistics calls: taps [2, 11, C] and those given of aff [9, C], stats [8, C], fold [24, C],
+    fp32 contiguous.  own_stats: the statistics are this batch's alone, so B*L >= 2 (a batch statistic needs more than one value
+    per channel, as nn.BatchNorm2d requires).  Returns (C, the es3_repmixer_bn_ws_floats workspace)."""
+    if own_stats and B * L < 2:
         raise ValueError(f"{name}: batch-statistics BatchNorm needs more than 1 value per channel (B*L = {B * L})")
     C = rows[0].shape[-1]
-    params = [(taps, (2, 11, C)), (aff, (9, C))] + ([(stats, (8, C))] if stats is not None else [])
-    return _repmixer_bwd_args(name, rows, B, L, params)
-
-
-def repmixer_bn_fwd(x, B, L, taps, aff, bns):
-    """RepMixerBlock prologue with batch-statistics BatchNorm on x [B*L, C] fp32.  taps [2, 11, C] = raw w_mc, w_f; aff [9, C] =
-    ls_tm, (gamma, beta) of BN_ms, BN_mc, BN_ns, BN_f; bns = those four nn.BatchNorm2d, whose running_mean / running_var /
-    num_batches_tracked are updated in place on the device.  Returns (x1 fp32, u bf16, fold [24, C] = wm, bm, wf, bf,
-    stats [8, C] = (batch mean, invstd) of the four BNs)."""
-    C = _repmixer_bn_args("repmixer_bn_fwd", (x,), B, L, taps, aff)
-    run = []
-    for bn in bns:
-        for t in (bn.running_mean, bn.running_var):
-            _chk(t, torch.float32, "running statistics")
-            if not (t.is_contiguous() and t.numel() == C):
-                raise ValueError(f"repmixer_bn_fwd: expected contiguous fp32 running statistics of {C} channels")
-        _chk(bn.num_batches_tracked, torch.int64, "num_batches_tracked")
-        run += [bn.running_mean.data_ptr(), bn.running_var.data_ptr(), bn.num_batches_tracked.data_ptr()]
-    x1 = torch.empty_like(x)
-    u = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16)
-    fold = torch.empty((24, C), device=x.device, dtype=torch.float32)
-    stats = torch.empty((8, C), device=x.device, dtype=torch.float32)
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
-    _call("es3_repmixer_bn_fwd", "repmixer_bn_fwd", _nb(x, x, x1, u, x), 3 * 4 * 11 * B * L * C, x.data_ptr(), x1.data_ptr(),
-          u.data_ptr(), taps.data_ptr(), aff.data_ptr(), *run, *[float(bn.eps) for bn in bns],
-          *[float(bn.momentum) for bn in bns], fold.data_ptr(), stats.data_ptr(), ws.data_ptr(), B, L, C, _stream())
-    return x1, u, fold, stats
-
-
-def repmixer_bn_ffn_bwd(x1, du, g, taps, aff, stats, B, L, dtaps=None, dgamma=None, dbeta=None):
-    """ConvFFN.conv + BN_f backward with batch statistics (stats from repmixer_bn_fwd): returns e = g + dw^T(df; w_f) fp32;
-    dtaps [C,1,1,11], dgamma, dbeta [C] accumulated."""
-    C = _repmixer_bn_args("repmixer_bn_ffn_bwd", (x1, du, g), B, L, taps, aff, stats)
-    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dgamma, C, "dgamma"), _grad_dst(dbeta, C, "dbeta")]
-    e = torch.empty_like(x1)
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x1.device)
-    _call("es3_repmixer_bn_ffn_bwd", "repmixer_bn_ffn_bwd", _nb(x1, du, x1, du, g, e), 8 * 11 * x1.numel(), x1.data_ptr(),
-          du.data_ptr(), g.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), e.data_ptr(), ws.data_ptr(), *ptrs,
-          B, L, C, _stream())
-    return e
-
-
-def repmixer_bn_tm_bwd(x, e, taps, aff, stats, B, L, dtaps=None, dls=None, dbn=(None,) * 6, want_bf16=False):
-    """RepMixer token-mixer backward with batch statistics: returns (dx fp32, bf16 copy | None); dtaps [C,1,1,11], dls [C,1,1]
-    and dbn = (dgamma, dbeta) x (ms, mc, ns) accumulated."""
-    C = _repmixer_bn_args("repmixer_bn_tm_bwd", (x, e), B, L, taps, aff, stats)
-    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dls, C, "dls")] + [_grad_dst(t, C, "dbn") for t in dbn]
-    dx = torch.empty_like(x)
-    dxb = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
-    _call("es3_repmixer_bn_tm_bwd", "repmixer_bn_tm_bwd", _nb(x, e, x, e, dx, dxb), 10 * 11 * x.numel(), x.data_ptr(),
-          e.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), dx.data_ptr(), _ptr(dxb), ws.data_ptr(), *ptrs,
-          B, L, C, _stream())
-    return dx, dxb
-
-
-# RepMixerBlock with synchronised BatchNorm: the forward split at its finalize points, the backward at its sums (the ranks
-# all-gather what the *_partial / *_sums calls return, sync_bn.repmixer_*).  A rank may hold B*L == 1: only the group's count
-# matters, and with two or more ranks it is >= 2.
-KERNELS_PER_CALL.update({"es3_repmixer_bn_stats_partial": 2, "es3_repmixer_bn_ffn_sums": 2, "es3_repmixer_bn_tm_sums": 2,
-                         "es3_repmixer_bn_ffn_apply": 3, "es3_repmixer_bn_tm_apply": 3})
+    params = [(t, (*shape, C)) for t, shape in ((taps, (2, 11)), (aff, (9,)), (stats, (8,)), (fold, (24,))) if t is not None]
+    _repmixer_bwd_args(name, rows, B, L, params)
+    return C, _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), rows[0].device)
 
 
 def _running_ptrs(bns, C, name):
@@ -698,13 +641,60 @@ def _running_ptrs(bns, C, name):
     return run
 
 
+def repmixer_bn_fwd(x, B, L, taps, aff, bns):
+    """RepMixerBlock prologue with batch-statistics BatchNorm on x [B*L, C] fp32.  taps [2, 11, C] = raw w_mc, w_f; aff [9, C] =
+    ls_tm, (gamma, beta) of BN_ms, BN_mc, BN_ns, BN_f; bns = those four nn.BatchNorm2d, whose running_mean / running_var /
+    num_batches_tracked are updated in place on the device.  Returns (x1 fp32, u bf16, fold [24, C] = wm, bm, wf, bf,
+    stats [8, C] = (batch mean, invstd) of the four BNs)."""
+    C, ws = _repmixer_bn_args("repmixer_bn_fwd", (x,), B, L, taps, aff, own_stats=True)
+    run = _running_ptrs(bns, C, "repmixer_bn_fwd")
+    x1 = torch.empty_like(x)
+    u = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16)
+    fold = torch.empty((24, C), device=x.device, dtype=torch.float32)
+    stats = torch.empty((8, C), device=x.device, dtype=torch.float32)
+    _call("es3_repmixer_bn_fwd", "repmixer_bn_fwd", _nb(x, x, x1, u, x), 3 * 4 * 11 * B * L * C, x.data_ptr(), x1.data_ptr(),
+          u.data_ptr(), taps.data_ptr(), aff.data_ptr(), *run, *[float(bn.eps) for bn in bns],
+          *[float(bn.momentum) for bn in bns], fold.data_ptr(), stats.data_ptr(), ws.data_ptr(), B, L, C, _stream())
+    return x1, u, fold, stats
+
+
+def repmixer_bn_ffn_bwd(x1, du, g, taps, aff, stats, B, L, dtaps=None, dgamma=None, dbeta=None):
+    """ConvFFN.conv + BN_f backward with batch statistics (stats from repmixer_bn_fwd): returns e = g + dw^T(df; w_f) fp32;
+    dtaps [C,1,1,11], dgamma, dbeta [C] accumulated."""
+    C, ws = _repmixer_bn_args("repmixer_bn_ffn_bwd", (x1, du, g), B, L, taps, aff, stats, own_stats=True)
+    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dgamma, C, "dgamma"), _grad_dst(dbeta, C, "dbeta")]
+    e = torch.empty_like(x1)
+    _call("es3_repmixer_bn_ffn_bwd", "repmixer_bn_ffn_bwd", _nb(x1, du, x1, du, g, e), 8 * 11 * x1.numel(), x1.data_ptr(),
+          du.data_ptr(), g.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), e.data_ptr(), ws.data_ptr(), *ptrs,
+          B, L, C, _stream())
+    return e
+
+
+def repmixer_bn_tm_bwd(x, e, taps, aff, stats, B, L, dtaps=None, dls=None, dbn=(None,) * 6, want_bf16=False):
+    """RepMixer token-mixer backward with batch statistics: returns (dx fp32, bf16 copy | None); dtaps [C,1,1,11], dls [C,1,1]
+    and dbn = (dgamma, dbeta) x (ms, mc, ns) accumulated."""
+    C, ws = _repmixer_bn_args("repmixer_bn_tm_bwd", (x, e), B, L, taps, aff, stats, own_stats=True)
+    ptrs = [_grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dls, C, "dls")] + [_grad_dst(t, C, "dbn") for t in dbn]
+    dx = torch.empty_like(x)
+    dxb = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
+    _call("es3_repmixer_bn_tm_bwd", "repmixer_bn_tm_bwd", _nb(x, e, x, e, dx, dxb), 10 * 11 * x.numel(), x.data_ptr(),
+          e.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), dx.data_ptr(), _ptr(dxb), ws.data_ptr(), *ptrs,
+          B, L, C, _stream())
+    return dx, dxb
+
+
+# RepMixerBlock with synchronised BatchNorm: the forward split at its finalize points, the backward at its sums (the ranks
+# all-gather what the *_partial / *_sums calls return, sync_bn.repmixer_*).  A rank may hold B*L == 1: only the group's count
+# matters, and with two or more ranks it is >= 2.
+KERNELS_PER_CALL.update({"es3_repmixer_bn_stats_partial": 2, "es3_repmixer_bn_ffn_sums": 2, "es3_repmixer_bn_tm_sums": 2,
+                         "es3_repmixer_bn_ffn_apply": 3, "es3_repmixer_bn_tm_apply": 3})
+
+
 def repmixer_bn_stats_partial(x, B, L, taps, fold, mode):
     """This rank's (count, mean, M2) fp64: mode 0 [2, 3, C] of x and c = dw(x; w_mc), mode 1 [1, 3, C] of f = dw(x1; w_f) with x1
     from fold's wm, bm (repmixer_bn_finalize_sync mode 0).  fold [24, C] fp32 (mode 0 does not read it)."""
-    C = x.shape[-1]
-    _repmixer_bwd_args("repmixer_bn_stats_partial", (x,), B, L, [(taps, (2, 11, C)), (fold, (24, C))])
+    C, ws = _repmixer_bn_args("repmixer_bn_stats_partial", (x,), B, L, taps, fold=fold)
     part = torch.empty((2 if mode == 0 else 1, 3, C), device=x.device, dtype=torch.float64)
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
     _call("es3_repmixer_bn_stats_partial", "repmixer_bn_stats_partial", _nb(x), 2 * 11 * x.numel(), x.data_ptr(), taps.data_ptr(),
           fold.data_ptr(), int(mode), ws.data_ptr(), part.data_ptr(), B, L, C, _stream())
     return part
@@ -745,11 +735,9 @@ def _sync_total(total, name):
 
 def repmixer_bn_ffn_sums(x1, du, taps, stats, B, L, aff, dgamma=None, dbeta=None):
     """First half of repmixer_bn_ffn_bwd: this rank's sums fp32 [2, C]; BN_f's dgamma / dbeta accumulated (this rank's)."""
-    C = x1.shape[-1]
-    _repmixer_bwd_args("repmixer_bn_ffn_sums", (x1, du), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    C, ws = _repmixer_bn_args("repmixer_bn_ffn_sums", (x1, du), B, L, taps, aff, stats)
     ptrs = [_grad_dst(dgamma, C, "dgamma"), _grad_dst(dbeta, C, "dbeta")]
     sums = torch.empty((2, C), device=x1.device, dtype=torch.float32)
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x1.device)
     _call("es3_repmixer_bn_ffn_sums", "repmixer_bn_ffn_sums", _nb(x1, du), 3 * 11 * x1.numel(), x1.data_ptr(), du.data_ptr(),
           taps.data_ptr(), stats.data_ptr(), ws.data_ptr(), sums.data_ptr(), *ptrs, B, L, C, _stream())
     return sums
@@ -757,12 +745,10 @@ def repmixer_bn_ffn_sums(x1, du, taps, stats, B, L, aff, dgamma=None, dbeta=None
 
 def repmixer_bn_ffn_apply(x1, du, g, taps, aff, stats, parts, total, B, L, dtaps=None):
     """Second half of repmixer_bn_ffn_bwd with every rank's sums parts [W, 2, C] (rank order) and the group's count: returns e."""
-    C = x1.shape[-1]
-    _repmixer_bwd_args("repmixer_bn_ffn_apply", (x1, du, g), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    C, ws = _repmixer_bn_args("repmixer_bn_ffn_apply", (x1, du, g), B, L, taps, aff, stats)
     _sync_parts(parts, 2, C, "repmixer_bn_ffn_apply")
     _sync_total(total, "repmixer_bn_ffn_apply")
     e = torch.empty_like(x1)
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x1.device)
     _call("es3_repmixer_bn_ffn_apply", "repmixer_bn_ffn_apply", _nb(x1, du, g, e), 5 * 11 * x1.numel(), x1.data_ptr(), du.data_ptr(),
           g.data_ptr(), taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), parts.data_ptr(), parts.shape[0], total.data_ptr(),
           e.data_ptr(), ws.data_ptr(), _grad_dst(dtaps, 11 * C, "dtaps"), B, L, C, _stream())
@@ -771,11 +757,9 @@ def repmixer_bn_ffn_apply(x1, du, g, taps, aff, stats, parts, total, B, L, dtaps
 
 def repmixer_bn_tm_sums(x, e, taps, aff, stats, B, L, dbn=(None,) * 6):
     """First half of repmixer_bn_tm_bwd: this rank's sums fp32 [3, C]; dbn = (dgamma, dbeta) x (ms, mc, ns) accumulated."""
-    C = x.shape[-1]
-    _repmixer_bwd_args("repmixer_bn_tm_sums", (x, e), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    C, ws = _repmixer_bn_args("repmixer_bn_tm_sums", (x, e), B, L, taps, aff, stats)
     ptrs = [_grad_dst(t, C, "dbn") for t in dbn]
     sums = torch.empty((3, C), device=x.device, dtype=torch.float32)
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
     _call("es3_repmixer_bn_tm_sums", "repmixer_bn_tm_sums", _nb(x, e), 4 * 11 * x.numel(), x.data_ptr(), e.data_ptr(),
           taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), ws.data_ptr(), sums.data_ptr(), *ptrs, B, L, C, _stream())
     return sums
@@ -783,13 +767,11 @@ def repmixer_bn_tm_sums(x, e, taps, aff, stats, B, L, dbn=(None,) * 6):
 
 def repmixer_bn_tm_apply(x, e, taps, aff, stats, parts, total, B, L, dtaps=None, dls=None, want_bf16=False):
     """Second half of repmixer_bn_tm_bwd with every rank's sums parts [W, 3, C] and the group's count: (dx fp32, bf16 copy | None)."""
-    C = x.shape[-1]
-    _repmixer_bwd_args("repmixer_bn_tm_apply", (x, e), B, L, [(taps, (2, 11, C)), (aff, (9, C)), (stats, (8, C))])
+    C, ws = _repmixer_bn_args("repmixer_bn_tm_apply", (x, e), B, L, taps, aff, stats)
     _sync_parts(parts, 3, C, "repmixer_bn_tm_apply")
     _sync_total(total, "repmixer_bn_tm_apply")
     dx = torch.empty_like(x)
     dxb = torch.empty((B * L, C), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
-    ws = _f32ws(_lib.size("es3_repmixer_bn_ws_floats", B, C), x.device)
     _call("es3_repmixer_bn_tm_apply", "repmixer_bn_tm_apply", _nb(x, e, dx, dxb), 6 * 11 * x.numel(), x.data_ptr(), e.data_ptr(),
           taps.data_ptr(), aff.data_ptr(), stats.data_ptr(), parts.data_ptr(), parts.shape[0], total.data_ptr(), dx.data_ptr(),
           _ptr(dxb), ws.data_ptr(), _grad_dst(dtaps, 11 * C, "dtaps"), _grad_dst(dls, C, "dls"), B, L, C, _stream())

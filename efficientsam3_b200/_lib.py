@@ -74,7 +74,6 @@ SIGNATURES: dict[str, list] = {
     "es3_stem_conv3x3_s2": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp],
     "es3_dwconv_bf16": [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _i, _vp],
     "es3_dwconv_tiled_bf16": [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _i, _vp],
-    "es3_litemla_aggreg_tiled": [_vp, _ll, _vp, _vp, _i, _i, _i, _i, _vp],
     "es3_mbconv_fused_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "es3_mbconv_tc_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "es3_mbconv_tc_s2_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
@@ -85,11 +84,8 @@ SIGNATURES: dict[str, list] = {
     "es3_maxpool2x2_bf16": [_vp, _vp, _i, _i, _i, _i, _vp],
     "es3_nhwc_to_nchw_f32": [_vp, _vp, _i, _i, _i, _vp],
     "es3_nchw_f32_to_nhwc": [_vp, _vp, _i, _i, _i, _vp],
-    "es3_litemla_aggreg": [_vp, _ll, _vp, _vp, _i, _i, _i, _i, _vp],
-    "es3_litemla_aggreg_tc": [_vp, _ll, _vp, _i, _i, _i, _i, _vp],
     "es3_litemla_aggreg_dwpw": [_vp, _ll, _vp, _vp, _i, _i, _i, _i, _vp],
     "es3_litemla_attn_tc": [_vp, _ll, _vp, _vp, _ll, _i, _i, _i, _f, _vp],
-    "es3_litemla_attn": [_vp, _ll, _vp, _vp, _ll, _i, _i, _i, _f, _vp],
     "es3_litemla_attn_generic": [_vp, _ll, _vp, _vp, _ll, _i, _i, _i, _i, _f, _vp],
     # student backward (train_bwd.cu)
     "es3_bn_stats": [_vp, _ll, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
@@ -116,7 +112,6 @@ SIGNATURES: dict[str, list] = {
     "es3_round_taps_sum_bf16": [_vp, _vp, _i, _i, _vp],
     "es3_dwconv_tc_bf16": [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _vp],
     "es3_dwconv_wgrad_win": [_vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp],
-    "es3_dwconv_wgrad_tiled": [_vp, _vp, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp],
     "es3_se_bwd_dgate": [_vp, _vp, _i, _i, _i, _vp, _vp, _vp],
     "es3_se_bwd_apply": [_vp, _vp, _vp, _vp, _i, _i, _i, _vp],
     "es3_layernorm_bwd": [_vp, _vp, _vp, _vp, _f, _vp, _ll, _i, _vp, _vp, _vp, _vp],
@@ -149,7 +144,6 @@ SIZE_HELPERS: dict[str, list] = {
     "es3_wgrad_pw_ws_floats": [_ll, _i, _i],
     "es3_dwconv_wgrad_ws_floats": [_i, _i, _i, _i, _i, _i],
     "es3_dwconv_wgrad_win_ws_floats": [_i, _i, _i, _i, _i, _i],
-    "es3_dwconv_wgrad_tiled_ws_floats": [_i, _i, _i, _i, _i],
     "es3_se_bwd_ws_floats": [_i, _i, _i],
     "es3_layernorm_bwd_ws_floats": [_ll, _i],
     "es3_layernorm_bwd_f32_ws_floats": [_ll, _i],

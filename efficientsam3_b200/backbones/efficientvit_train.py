@@ -358,8 +358,6 @@ class HeadTrainUnit:
     """ImageStudentEncoder.head + resize (stage1/model.py:194-211): Conv1x1(no bias) -> BN -> GELU -> Conv3x3(bias) ->
     bilinear to embed_size -> NCHW fp32."""
 
-    WGRAD_TC = True   # head.3 weight gradient on wgmma (False: nine es3_wgrad_pw launches)
-
     def __init__(self, head: nn.Sequential, embed_size: int):
         self.c0 = ConvUnit(head[0], head[1], "gelu", "pw")
         self.conv3 = head[3]
@@ -389,14 +387,8 @@ class HeadTrainUnit:
         if gb is not None:      # d bias = column sums of dy: the reduce half of the BN/act backward with act = none
             ops.bn_act_bwd(dy, dy, None, None, None, "none", dbeta=gb, apply=False)
         gw = _grad_of(grads, conv3.weight)
-        if gw is not None and self.WGRAD_TC:      # nine wgmma GEMMs over the zero-framed, transposed pixel index
+        if gw is not None:      # nine wgmma GEMMs over the zero-framed, transposed pixel index
             ops.conv3x3_wgrad(dy, a1, gw)
-        elif gw is not None:    # one shifted mma.sync weight gradient per tap, written with the [N][C][3][3] strides
-            flat = gw.view(-1)
-            dy2, a2 = dy.view(-1, n), a1.view(-1, c)
-            for ky in range(3):
-                for kx in range(3):
-                    ops.wgrad_pw(dy2, a2, flat[ky * 3 + kx:], ldn=9 * c, ldk=9, shift=(h, wd, ky - 1, kx - 1))
         # input gradient: 3x3 conv of dy with the rotated, in/out-transposed kernel
         wt9 = cached_pack(conv3, "wt9", conv3.weight,
                           lambda: conv3.weight.detach().flip(2, 3).permute(1, 2, 3, 0).reshape(c, 9 * n).to(torch.bfloat16).contiguous())

@@ -93,15 +93,9 @@ class SEUnit:
         se = self.se
         x, m, h, g, w1, w2 = self.saved
         self.saved = None
-        B, H, W, C = x.shape
-        HW = H * W
+        HW = x.shape[1] * x.shape[2]
         dy = dy.contiguous()
-        if ops.SE_BWD_BATCHED:
-            dgate = ops.se_bwd_dgate(dy, x)
-        else:
-            dgate = torch.zeros((B, C), device=x.device, dtype=torch.float32)
-            for b in range(B):                               # d gate[b, c] = sum_hw dy x
-                _colsum_grads(dy[b], x[b], dgate[b], None)
+        dgate = ops.se_bwd_dgate(dy, x)                                                         # d gate[b, c] = sum_hw dy x
         # the two 1x1 convs on the pooled [B, C] vectors (O(B C) element-wise prep in torch, contractions on es3_gemm_simt)
         dpre2 = (dgate * g * (1.0 - g)).contiguous()                                            # [B, C]
         f32 = dict(out_dtype=torch.float32)
@@ -118,12 +112,7 @@ class SEUnit:
         if g_b1 is not None:
             g_b1 += dpre1.sum(0)
         dm = (ops.gemm_simt(dpre1, w1.t().contiguous(), **f32) / HW).contiguous()                # [B, C]: d mean / HW
-        if ops.SE_BWD_BATCHED:
-            return ops.se_bwd_apply(dy, g, dm)
-        dx = torch.empty_like(x)
-        for b in range(B):                                   # dx = dy * gate + d mean / HW
-            ops.affine_act(dy[b], g[b], dm[b], None, out=dx[b])
-        return dx
+        return ops.se_bwd_apply(dy, g, dm)                                                     # dx = dy * gate + d mean / HW
 
 
 class RepVGGDWUnit:

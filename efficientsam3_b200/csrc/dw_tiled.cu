@@ -1,16 +1,13 @@
-// Shared-memory tiled depthwise convolution (NHWC bf16, fp32 math), optionally fused with the
-// LiteMLA grouped 1x1 that follows the 5x5 depthwise ("aggreg", efficientvit/nn/ops.py:560-575).
+// Shared-memory tiled depthwise convolution (NHWC bf16, fp32 math) for the stride-2 3x3 convs with C % 32 == 0 (the stride-1
+// shapes run on the tensor-core kernel in dw_tc.cu).
 //
-// Why: the one-thread-per-output kernel in conv.cu re-reads every input pixel KS*KS times through
-// L1/L2 and (for aggreg) gathered its 16x16 group weights with 32 distinct cache lines per load.  Here a block stages the
-// haloed input tile of CG channels once (cp.async, zero-filled outside the image), every thread
-// produces a strip of 4 output pixels x 8 channels from a sliding register window, and weights sit in
-// shared memory.  HBM traffic = input tile (+halo) once + output once.
+// Why: the one-thread-per-output kernel in conv.cu re-reads every input pixel KS*KS times through L1/L2.  Here a block stages
+// the haloed input tile of CG channels once (cp.async, zero-filled outside the image), every thread produces a strip of 4 output
+// pixels x 8 channels from a sliding register window, and weights sit in shared memory.  HBM traffic = input tile (+halo) once +
+// output once.
 //
 // Block: 256 threads.  Tile: TH x TW outputs x CG channels.  smem pixel stride = CG*2 + 16 bytes
 // (the pad keeps 16-byte accesses of 8 consecutive pixels on distinct bank groups).
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace es3 {
@@ -33,27 +30,23 @@ struct DwTile {
   static constexpr int PIX_BYTES = CG * 2 + 16;
   static constexpr int TILE_BYTES = IH * IW * PIX_BYTES;
   static constexpr int W_FLOATS = KS * KS * CG;
-  static constexpr int GPW_FLOATS = (CG / 8) * (8 * 16 + 4);  // grouped-1x1 weights, padded per 8-ch group
   static constexpr int WB_FLOATS = W_FLOATS + CG;                      // one (tap weights, bias) set
-  static constexpr int SMEM = 2 * TILE_BYTES + (2 * WB_FLOATS + GPW_FLOATS) * 4;   // double-buffered tile + weights (persistent CTAs)
+  static constexpr int SMEM = 2 * TILE_BYTES + 2 * WB_FLOATS * 4;   // double-buffered tile + weights (persistent CTAs)
 };
 
 // x: [B,H,W,*] bf16 with pixel stride ldx, channel window [c_in0, c_in0 + C) ; out likewise (ldo, c_out0).
 // w: [KS*KS][C] fp32 tap-major (scale folded); bias [C] or null.
-// GROUP_PW: after the depthwise, apply a grouped 1x1 with 16-channel groups, wpw [C][16] fp32, no bias.
 // Persistent CTAs over work items (tile, channel group, image): while the strips of item i are computed from one shared-memory
 // buffer, the haloed tile (cp.async) and the weights of item i + gridDim.x stream into the other -- the one-item-per-CTA version was
 // a load -> wait -> compute -> store sequence with nothing overlapped inside a CTA.
-template <int KS, int STRIDE, int CG, int TH, int TW, int ACT, bool GROUP_PW>
+template <int KS, int STRIDE, int CG, int TH, int TW, int ACT>
 __global__ void __launch_bounds__(256, (2 * (DwTile<KS, STRIDE, CG, TH, TW>::SMEM + 1024) <= 227 * 1024) ? 2 : 1) dw_tiled_kernel(const bf16* x, long long ldx, const float* __restrict__ w,
-                                                       const float* __restrict__ bias,
-                                                       const float* __restrict__ wpw, bf16* out, long long ldo,
+                                                       const float* __restrict__ bias, bf16* out, long long ldo,
                                                        int H, int W, int C, int Ho, int Wo, int tiles_x, int tiles_per_img,
                                                        int n_cg, int total_items) {
   using T = DwTile<KS, STRIDE, CG, TH, TW>;
   extern __shared__ __align__(16) uint8_t smem[];
   float* s_wb = reinterpret_cast<float*>(smem + 2 * T::TILE_BYTES);     // [2][W_FLOATS + CG]
-  float* s_g = s_wb + 2 * T::WB_FLOATS;
   constexpr int PAD = KS / 2;
   constexpr int NV = CG / 8;  // 16-byte vectors per pixel
 
@@ -91,7 +84,6 @@ __global__ void __launch_bounds__(256, (2 * (DwTile<KS, STRIDE, CG, TH, TW>::SME
 
   int item = blockIdx.x;
   if (item >= total_items) return;
-  int gpw_c0 = -1;
   stage(item, 0);
   int buf = 0;
   for (; item < total_items; item += gridDim.x, buf ^= 1) {
@@ -104,13 +96,6 @@ __global__ void __launch_bounds__(256, (2 * (DwTile<KS, STRIDE, CG, TH, TW>::SME
     }
     int tile, c0, b;
     decode(item, tile, c0, b);
-    if (GROUP_PW && c0 != gpw_c0) {
-      for (int i = threadIdx.x; i < CG * 16; i += 256) {
-        const int c = i / 16, k = i % 16;  // output channel c (within block), input k within its 16-group
-        s_g[(c / 8) * (8 * 16 + 4) + (c % 8) * 16 + k] = wpw[(long long)(c0 + c) * 16 + k];
-      }
-      gpw_c0 = c0;
-    }
     __syncthreads();
     const uint8_t* s_tile = smem + buf * T::TILE_BYTES;
     const float* s_w = s_wb + buf * T::WB_FLOATS;
@@ -122,7 +107,6 @@ __global__ void __launch_bounds__(256, (2 * (DwTile<KS, STRIDE, CG, TH, TW>::SME
   constexpr int STRIPS_X = TW / 4;
   constexpr int ITEMS = TH * STRIPS_X * NV;
   constexpr int WIN = 3 * STRIDE + KS;  // input columns covering 4 outputs
-  static_assert(!GROUP_PW || (ITEMS % 256 == 0 && NV % 2 == 0), "GROUP_PW needs full warps (shuffle pairing)");
   // (unroll 1: with ITEMS = 2 x 256 the compiler fused both iterations into one 150 .. 255-register body -- one resident CTA per SM,
   //  spills in the 5x5 variants)
 #pragma unroll 1
@@ -169,29 +153,6 @@ __global__ void __launch_bounds__(256, (2 * (DwTile<KS, STRIDE, CG, TH, TW>::SME
       float o[8];
 #pragma unroll
       for (int e = 0; e < 4; ++e) { o[2 * e] = es3_act_t<ACT>(acc[j][e].x); o[2 * e + 1] = es3_act_t<ACT>(acc[j][e].y); }
-      if (GROUP_PW) {
-        // materialise the depthwise output in bf16 (as the unfused reference path does), then the
-        // 16x16 group product: this thread owns 8 of the group's 16 channels, lane^1 owns the rest.
-        float mine[8], other[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) mine[e] = __bfloat162float(__float2bfloat16(o[e]));
-#pragma unroll
-        for (int e = 0; e < 8; ++e) other[e] = __shfl_xor_sync(0xffffffffu, mine[e], 1);
-        const bool hi = (v & 1);  // this thread holds input channels 8..15 of the group
-        const float* g = s_g + v * (8 * 16 + 4);
-#pragma unroll
-        for (int n = 0; n < 8; ++n) {
-          float a = 0.f;
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const float lo_in = hi ? other[k] : mine[k];
-            const float hi_in = hi ? mine[k] : other[k];
-            a = fmaf(lo_in, g[n * 16 + k], a);
-            a = fmaf(hi_in, g[n * 16 + 8 + k], a);
-          }
-          o[n] = a;
-        }
-      }
       const int ox = ox0 + sx * 4 + j;
       if (oy < Ho && ox < Wo)
         *reinterpret_cast<uint4*>(out + (((long long)b * Ho + oy) * Wo + ox) * ldo + c0 + v * 8) = pack8(o);
@@ -201,11 +162,10 @@ __global__ void __launch_bounds__(256, (2 * (DwTile<KS, STRIDE, CG, TH, TW>::SME
   }
 }
 
-template <int KS, int STRIDE, int CG, int TH, int TW, int ACT, bool GROUP_PW>
-static int launch_dw_tiled(const bf16* x, long long ldx, const float* w, const float* bias, const float* wpw,
-                           bf16* out, long long ldo, int B, int H, int W, int C, int Ho, int Wo, cudaStream_t st) {
+template <int KS, int STRIDE, int CG, int TH, int TW, int ACT>
+static int launch_dw_tiled(const bf16* x, long long ldx, const float* w, const float* bias, bf16* out, long long ldo, int B, int H, int W, int C, int Ho, int Wo, cudaStream_t st) {
   using T = DwTile<KS, STRIDE, CG, TH, TW>;
-  auto kern = dw_tiled_kernel<KS, STRIDE, CG, TH, TW, ACT, GROUP_PW>;
+  auto kern = dw_tiled_kernel<KS, STRIDE, CG, TH, TW, ACT>;
   static bool configured = false;
   if (!configured) {
     ES3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM));
@@ -223,7 +183,7 @@ static int launch_dw_tiled(const bf16* x, long long ldx, const float* w, const f
   }
   const int per_sm = 2 * (T::SMEM + 1024) <= 227 * 1024 ? 2 : 1;       // resident CTAs (shared memory: two buffers each)
   const long long ctas = (long long)sm_count * per_sm;
-  kern<<<(unsigned)(total < ctas ? total : ctas), 256, T::SMEM, st>>>(x, ldx, w, bias, wpw, out, ldo, H, W, C, Ho, Wo, tiles_x,
+  kern<<<(unsigned)(total < ctas ? total : ctas), 256, T::SMEM, st>>>(x, ldx, w, bias, out, ldo, H, W, C, Ho, Wo, tiles_x,
                                                                       tiles_x * tiles_y, n_cg, (int)total);
   ES3_LAUNCH_CHECK("dw_tiled_kernel");
   return 0;
@@ -233,43 +193,21 @@ static int launch_dw_tiled(const bf16* x, long long ldx, const float* w, const f
 
 using namespace es3;
 
-// Depthwise ks x ks (3|5), stride 1|2, pad ks/2, C % 32 == 0.  Same contract as es3_dwconv_bf16.
+// Depthwise 3x3, stride 2, pad 1, C % 32 == 0.  Same contract as es3_dwconv_bf16.
 extern "C" int es3_dwconv_tiled_bf16(const void* x, long long ldx, const float* w, const float* bias, void* out,
                                      long long ldo, int B, int H, int W, int C, int ks, int stride, int act,
                                      void* stream) {
   ES3_REQUIRE(C % 32 == 0 && ldx % 8 == 0 && ldo % 8 == 0, "es3_dwconv_tiled_bf16: C=%d must be a multiple of 32", C);
-  ES3_REQUIRE(act == ACT_NONE || act == ACT_HSWISH || act == ACT_GELU || act == ACT_RELU,
-              "es3_dwconv_tiled_bf16: activation %d not instantiated", act);
-  const int pad = ks / 2;
-  const int Ho = (H + 2 * pad - ks) / stride + 1, Wo = (W + 2 * pad - ks) / stride + 1;
+  ES3_REQUIRE(ks == 3 && stride == 2, "es3_dwconv_tiled_bf16: unsupported ks=%d stride=%d", ks, stride);
+  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   cudaStream_t st = (cudaStream_t)stream;
   const bf16* xi = (const bf16*)x;
   bf16* o = (bf16*)out;
-#define ES3_DW_CASE(KS_, S_, CG_, TH_, TW_)                                                                         \
-  switch (act) {                                                                                                    \
-    case ACT_NONE: return launch_dw_tiled<KS_, S_, CG_, TH_, TW_, ACT_NONE, false>(xi, ldx, w, bias, nullptr, o, ldo, B, H, W, C, Ho, Wo, st);     \
-    case ACT_RELU: return launch_dw_tiled<KS_, S_, CG_, TH_, TW_, ACT_RELU, false>(xi, ldx, w, bias, nullptr, o, ldo, B, H, W, C, Ho, Wo, st);     \
-    case ACT_HSWISH: return launch_dw_tiled<KS_, S_, CG_, TH_, TW_, ACT_HSWISH, false>(xi, ldx, w, bias, nullptr, o, ldo, B, H, W, C, Ho, Wo, st); \
-    default: return launch_dw_tiled<KS_, S_, CG_, TH_, TW_, ACT_GELU, false>(xi, ldx, w, bias, nullptr, o, ldo, B, H, W, C, Ho, Wo, st);           \
+  switch (act) {
+    case ACT_NONE: return launch_dw_tiled<3, 2, 32, 4, 32, ACT_NONE>(xi, ldx, w, bias, o, ldo, B, H, W, C, Ho, Wo, st);
+    case ACT_RELU: return launch_dw_tiled<3, 2, 32, 4, 32, ACT_RELU>(xi, ldx, w, bias, o, ldo, B, H, W, C, Ho, Wo, st);
+    case ACT_HSWISH: return launch_dw_tiled<3, 2, 32, 4, 32, ACT_HSWISH>(xi, ldx, w, bias, o, ldo, B, H, W, C, Ho, Wo, st);
+    case ACT_GELU: return launch_dw_tiled<3, 2, 32, 4, 32, ACT_GELU>(xi, ldx, w, bias, o, ldo, B, H, W, C, Ho, Wo, st);
   }
-  if (ks == 3 && stride == 1) {
-    if (C % 64 == 0) { ES3_DW_CASE(3, 1, 64, 8, 32) } else { ES3_DW_CASE(3, 1, 32, 8, 32) }
-  } else if (ks == 3 && stride == 2) {
-    ES3_DW_CASE(3, 2, 32, 4, 32)
-  } else if (ks == 5 && stride == 1) {
-    // 32-channel groups: two double-buffered 35 KB tiles -> two CTAs per SM (the 64-channel tile needs 124 KB: one CTA, 8 warps per SM);
-    // ES3_DW5_CG64=1 selects the wide variant for A/B timing
-    static const bool wide = [] { const char* e = getenv("ES3_DW5_CG64"); return e && e[0] == '1'; }();
-    if (wide && C % 64 == 0) { ES3_DW_CASE(5, 1, 64, 8, 32) } else { ES3_DW_CASE(5, 1, 32, 8, 32) }
-  }
-#undef ES3_DW_CASE
-  ES3_REQUIRE(false, "es3_dwconv_tiled_bf16: unsupported ks=%d stride=%d", ks, stride);
-}
-
-// LiteMLA aggreg, tiled: ms [B,H,W,ld]: reads qkv channels [0,C3), writes grouped1x1(dw5x5(qkv)) to [C3,2*C3).
-extern "C" int es3_litemla_aggreg_tiled(void* ms, long long ld, const float* wdw, const float* wpw, int B, int H, int W,
-                                        int C3, void* stream) {
-  ES3_REQUIRE(C3 % 64 == 0 && ld % 8 == 0 && ld >= 2 * C3, "es3_litemla_aggreg_tiled: bad C3=%d ld=%lld", C3, ld);
-  return launch_dw_tiled<5, 1, 64, 8, 32, ACT_NONE, true>((const bf16*)ms, ld, wdw, nullptr, wpw, (bf16*)ms + C3, ld, B, H,
-                                                          W, C3, H, W, (cudaStream_t)stream);
+  ES3_REQUIRE(false, "es3_dwconv_tiled_bf16: activation %d not instantiated", act);
 }

@@ -1,210 +1,13 @@
-// EfficientViT LiteMLA (ReLU linear attention) -- reference efficientvit/nn/ops.py:521-671.
+// EfficientViT LiteMLA ReLU linear attention for any head dim DIM <= 32 -- reference efficientvit/nn/ops.py:592-621.
+// efficientvit_b2 / b3 use dim = 32; the tensor-core kernels in litemla_tc.cu are specialised for dim = 16 (b0 / b1, the
+// benchmarked student).  CUDA-core formulation, all arithmetic fp32 (the reference forces fp32 here, ops.py:586-589).
 //
-// Data layout: one NHWC bf16 buffer `ms` of 6*TD channels per pixel (TD = heads*dim):
-//   channels [0, 3TD)   = qkv           (written by the qkv 1x1 GEMM with ldo = 6TD)
-//   channels [3TD, 6TD) = aggreg(qkv)   (dw5x5 -> grouped 1x1, written by litemla_aggreg_kernel)
-// which is exactly torch.cat([qkv, aggreg(qkv)], dim=1) (ops.py:656-660); viewed as
-// (B, 2*heads, 3*dim, HW), head h owns channels [48h, 48h+48): q | k | v (ops.py:590-606, dim = 16).
-//
-//   kv kernel   : KV[b,h] (17x16) = sum_p [v_p ; 1] relu(k_p)^T        (ops.py:609-616, the padded ones row)
-//                 two-stage, fixed summation order -> bit-reproducible
-//   apply kernel: out_p = KV[:16] relu(q_p) / (KV[16] . relu(q_p) + eps) (ops.py:617-620)
-// All arithmetic fp32 (the reference forces fp32 here, ops.py:586-589).
+// Head h owns channels [h*3*dim, (h+1)*3*dim) of the NHWC bf16 input as q | k | v (ops.py:590-606).
+//   kv kernel   : KV[b,h] ((dim+1) x dim) = sum_p [v_p ; 1] relu(k_p)^T       (ops.py:609-616, the padded ones row)
+//                 two-stage, fixed summation order -> bit-reproducible (no atomics)
+//   apply kernel: out_p = KV[:dim] relu(q_p) / (KV[dim] . relu(q_p) + eps)   (ops.py:617-620)
 #include "common.cuh"
 
-namespace es3 {
-
-constexpr int LDIM = 16;  // LiteMLA head dim of the b0/b1 backbones (backbone.py:158-176: dim=16)
-
-// dw5x5 (no bias) -> grouped 1x1 (groups of 16 channels, no bias).  Thread = (pixel, 16-channel group).
-// wdw: [25][C3] fp32 tap-major; wpw: [C3][16] fp32 (nn.Conv2d weight (C3,16,1,1) squeezed).
-__global__ void litemla_aggreg_kernel(const bf16* ms_in, bf16* ms_out, long long ld, const float* __restrict__ wdw,
-                                      const float* __restrict__ wpw, int B, int H, int W, int C3) {
-  const int ng = C3 / 16;
-  const long long total = (long long)B * H * W * ng;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int g = (int)(idx % ng);
-  const long long p = idx / ng;
-  const int ox = (int)(p % W);
-  const int oy = (int)((p / W) % H);
-  const int b = (int)(p / ((long long)W * H));
-  const int c0 = g * 16;
-  float acc[16];
-#pragma unroll
-  for (int e = 0; e < 16; ++e) acc[e] = 0.f;
-#pragma unroll 1
-  for (int ky = 0; ky < 5; ++ky) {
-    const int iy = oy - 2 + ky;
-    if (iy < 0 || iy >= H) continue;
-#pragma unroll
-    for (int kx = 0; kx < 5; ++kx) {
-      const int ix = ox - 2 + kx;
-      if (ix < 0 || ix >= W) continue;
-      const uint4* xp = reinterpret_cast<const uint4*>(ms_in + (((long long)b * H + iy) * W + ix) * ld + c0);
-      float f[16];
-      unpack8(xp[0], f);
-      unpack8(xp[1], f + 8);
-      const float4* wp = reinterpret_cast<const float4*>(wdw + (ky * 5 + kx) * C3 + c0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float4 w4 = __ldg(wp + j);
-        acc[4 * j + 0] = fmaf(f[4 * j + 0], w4.x, acc[4 * j + 0]);
-        acc[4 * j + 1] = fmaf(f[4 * j + 1], w4.y, acc[4 * j + 1]);
-        acc[4 * j + 2] = fmaf(f[4 * j + 2], w4.z, acc[4 * j + 2]);
-        acc[4 * j + 3] = fmaf(f[4 * j + 3], w4.w, acc[4 * j + 3]);
-      }
-    }
-  }
-  // the reference materialises the depthwise output (nn.Sequential of two convs): round to the
-  // activation dtype before the grouped 1x1 so fused and unfused paths agree.
-#pragma unroll
-  for (int e = 0; e < 16; ++e) acc[e] = __bfloat162float(__float2bfloat16(acc[e]));
-  float o[16];
-#pragma unroll
-  for (int n = 0; n < 16; ++n) {
-    const float4* wr = reinterpret_cast<const float4*>(wpw + (long long)(c0 + n) * 16);
-    float a = 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float4 w4 = __ldg(wr + j);
-      a = fmaf(acc[4 * j + 0], w4.x, a);
-      a = fmaf(acc[4 * j + 1], w4.y, a);
-      a = fmaf(acc[4 * j + 2], w4.z, a);
-      a = fmaf(acc[4 * j + 3], w4.w, a);
-    }
-    o[n] = a;
-  }
-  uint4* op = reinterpret_cast<uint4*>(ms_out + p * ld + c0);
-  op[0] = pack8(o);
-  op[1] = pack8(o + 8);
-}
-
-// Deterministic two-stage reduction (no atomics: results must not depend on scheduling, the
-// reference's masks are compared bit-for-bit downstream).
-// Stage 1: grid (chunks of KV_CHUNK pixels, heads2, B), block 256.
-//          part: [B][heads2][nchunk][17][16] fp32 partial sums.
-constexpr int KV_CHUNK = 512;
-__global__ void litemla_kv_kernel(const bf16* __restrict__ ms, long long ld, float* __restrict__ part, int HW) {
-  __shared__ float sk[128][LDIM];
-  __shared__ float sv[128][LDIM + 1];
-  const int h = blockIdx.y, b = blockIdx.z, heads2 = gridDim.y, nchunk = gridDim.x;
-  const int i = threadIdx.x >> 4, j = threadIdx.x & 15;
-  float acc = 0.f, ones = 0.f;
-  for (int sub = 0; sub < KV_CHUNK / 128; ++sub) {
-    const int p0 = blockIdx.x * KV_CHUNK + sub * 128;
-    if (p0 >= HW) break;
-    // 128 pixels x 4 uint4 (k: 2, v: 2)
-    for (int t = threadIdx.x; t < 128 * 4; t += blockDim.x) {
-      const int pl = t >> 2, v = t & 3;
-      const int p = p0 + pl;
-      float f[8];
-      if (p < HW) {
-        unpack8(__ldg(reinterpret_cast<const uint4*>(ms + ((long long)b * HW + p) * ld + h * 48 + 16 + v * 8)), f);
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) f[e] = 0.f;
-      }
-      if (v < 2) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) sk[pl][v * 8 + e] = fmaxf(f[e], 0.f);
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) sv[pl][(v - 2) * 8 + e] = f[e];
-      }
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int p = 0; p < 128; ++p) {
-      const float kk = sk[p][j];
-      acc = fmaf(sv[p][i], kk, acc);
-      ones += kk;  // rows beyond HW hold k = 0
-    }
-    __syncthreads();
-  }
-  float* dst = part + (((long long)b * heads2 + h) * nchunk + blockIdx.x) * 17 * LDIM;
-  dst[i * LDIM + j] = acc;
-  if (i == 0) dst[16 * LDIM + j] = ones;
-}
-
-// Stage 2 + apply: grid (chunks of 128 pixels, heads2, B), block 128.  Sums the partials in fixed order.
-// att: [B][HW][ldo] bf16, head h -> channels [16h, 16h+16).
-__global__ void litemla_apply_kernel(const bf16* __restrict__ ms, long long ld, const float* __restrict__ part,
-                                     int nchunk, bf16* __restrict__ att, long long ldo, int HW, float eps) {
-  __shared__ float skv[17 * LDIM];
-  const int h = blockIdx.y, b = blockIdx.z, heads2 = gridDim.y;
-  const float* src = part + ((long long)b * heads2 + h) * nchunk * 17 * LDIM;
-  for (int i = threadIdx.x; i < 17 * LDIM; i += blockDim.x) {
-    float a = 0.f;
-    for (int c = 0; c < nchunk; ++c) a += src[c * 17 * LDIM + i];
-    skv[i] = a;
-  }
-  __syncthreads();
-  const int p = blockIdx.x * 128 + threadIdx.x;
-  if (p >= HW) return;
-  const uint4* qp = reinterpret_cast<const uint4*>(ms + ((long long)b * HW + p) * ld + h * 48);
-  float q[16];
-  unpack8(__ldg(qp), q);
-  unpack8(__ldg(qp + 1), q + 8);
-#pragma unroll
-  for (int e = 0; e < 16; ++e) q[e] = fmaxf(q[e], 0.f);
-  float den = 0.f;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) den = fmaf(skv[16 * LDIM + j], q[j], den);
-  const float inv = 1.f / (den + eps);
-  float o[16];
-#pragma unroll
-  for (int d = 0; d < 16; ++d) {
-    float a = 0.f;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) a = fmaf(skv[d * LDIM + j], q[j], a);
-    o[d] = a * inv;
-  }
-  uint4* op = reinterpret_cast<uint4*>(att + ((long long)b * HW + p) * ldo + h * 16);
-  op[0] = pack8(o);
-  op[1] = pack8(o + 8);
-}
-
-}  // namespace es3
-
-using namespace es3;
-
-// ms: [B,H,W,ld] bf16 with qkv in channels [0,C3) -> writes aggreg(qkv) to channels [C3, 2*C3).
-extern "C" int es3_litemla_aggreg(void* ms, long long ld, const float* wdw, const float* wpw, int B, int H, int W,
-                                  int C3, void* stream) {
-  ES3_REQUIRE(C3 % 16 == 0 && ld % 8 == 0 && ld >= 2 * C3, "es3_litemla_aggreg: bad C3=%d ld=%lld", C3, ld);
-  const long long total = (long long)B * H * W * (C3 / 16);
-  const int threads = 128;
-  litemla_aggreg_kernel<<<(unsigned)ceil_div(total, threads), threads, 0, (cudaStream_t)stream>>>(
-      (const bf16*)ms, (bf16*)ms + C3, ld, wdw, wpw, B, H, W, C3);
-  ES3_LAUNCH_CHECK("litemla_aggreg_kernel");
-  return 0;
-}
-
-// ms: [B,HW,ld] bf16 (ld = 48*heads2), kv_ws: fp32 workspace of B*heads2*ceil(HW/512)*17*16 floats
-// (es3_litemla_ws_floats), att: [B,HW,ldo] bf16 output (ldo >= 16*heads2).
-extern "C" long long es3_litemla_ws_floats(int B, int HW, int heads2) {
-  return (long long)B * heads2 * ceil_div(HW, KV_CHUNK) * 17 * LDIM;
-}
-
-extern "C" int es3_litemla_attn(const void* ms, long long ld, float* kv_ws, void* att, long long ldo, int B, int HW,
-                                int heads2, float eps, void* stream) {
-  ES3_REQUIRE(ld >= 48 * heads2 && ld % 8 == 0 && ldo % 8 == 0, "es3_litemla_attn: bad ld=%lld ldo=%lld heads2=%d", ld, ldo, heads2);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nchunk = ceil_div(HW, KV_CHUNK);
-  dim3 grid1(nchunk, heads2, B);
-  litemla_kv_kernel<<<grid1, 256, 0, st>>>((const bf16*)ms, ld, kv_ws, HW);
-  ES3_LAUNCH_CHECK("litemla_kv_kernel");
-  dim3 grid(ceil_div(HW, 128), heads2, B);
-  litemla_apply_kernel<<<grid, 128, 0, st>>>((const bf16*)ms, ld, kv_ws, nchunk, (bf16*)att, ldo, HW, eps);
-  ES3_LAUNCH_CHECK("litemla_apply_kernel");
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------ generic head dim
-// ReLU linear attention for any head dim DIM <= 32 (efficientvit_b2 / b3 use dim = 32; ops.py:592-621).  CUDA-core
-// formulation, fp32 state, same deterministic two-stage KV reduction as above: the tensor-core kernels in litemla_tc.cu
-// are specialised for dim = 16 (b0 / b1, the benchmarked student).
 namespace es3 {
 constexpr int GA_PX = 128;
 
@@ -273,6 +76,8 @@ __global__ void __launch_bounds__(128) litemla_apply_generic_kernel(const bf16* 
   }
 }
 }  // namespace es3
+
+using namespace es3;
 
 extern "C" long long es3_litemla_generic_ws_floats(int B, int HW, int heads2, int dim) {
   return (long long)B * heads2 * ceil_div(HW, GA_PX) * (dim + 1) * dim;

@@ -1,14 +1,14 @@
-// LiteMLA on tensor cores (mma.sync bf16, fp32 accumulate) -- reference efficientvit/nn/ops.py:521-671.
+// LiteMLA on tensor cores (mma.sync bf16, fp32 accumulate) -- reference efficientvit/nn/ops.py:521-671, head dim 16.
 //
-// Why: the FMA formulations in dw_tiled.cu / litemla.cu spent ~60 thread
-// instructions per output element.
-// Every stage here is a small dense contraction:
+// Data layout: one NHWC bf16 buffer `ms` of 6*TD channels per pixel (TD = heads*dim):
+//   channels [0, 3TD)   = qkv           (written by the qkv 1x1 GEMM with ldo = 6TD)
+//   channels [3TD, 6TD) = aggreg(qkv)   (dw5x5 -> grouped 1x1, written by litemla_aggreg_dwpw_kernel)
+// which is exactly torch.cat([qkv, aggreg(qkv)], dim=1) (ops.py:656-660); viewed as
+// (B, 2*heads, 3*dim, HW), head h owns channels [48h, 48h+48): q | k | v (ops.py:590-606, dim = 16).
 //
-//  aggreg : grouped1x1(dw5x5(x)) for one 16-channel group is ONE grouped 5x5 conv,
-//           y[p][n] = sum_tap sum_i W'[tap][n][i] x[p+tap][i],  W'[tap][n][i] = wpw[n][i] * wdw[tap][i]
-//           = a K = 25*16 = 400 contraction per (pixel, group): 25 x (ldmatrix A from the haloed smem tile,
-//           2 mma) per 16 pixels.  (W' is rounded to bf16 once on the host; the FMA path rounded the
-//           depthwise output instead -- both are within the bf16 activation tolerance.)
+// Every stage is a small dense contraction:
+//  aggreg : depthwise 5x5 as diagonal MMAs, its result rounded to bf16 and fed back as the A fragment of the 16x16 grouped
+//           pointwise MMA.
 //  kv     : KV[i][j] = sum_p v[p][i] relu(k[p][j])   (M=16, N=16, K=pixels; A and B via ldmatrix.trans),
 //           ones row (ops.py:613 F.pad value=1) via a constant A fragment.  Deterministic two-stage reduce.
 //  apply  : out[p][d] = sum_j KV[d][j] relu(q[p][j]) / (KV[16] . relu(q[p]) + eps)
@@ -46,81 +46,11 @@ __device__ __forceinline__ uint32_t relu_bf16x2(uint32_t v) {
 // ------------------------------------------------------------------------------------------ aggreg
 constexpr int AG_TH = 16, AG_TW = 32, AG_IH = AG_TH + 4, AG_IW = AG_TW + 4, AG_PS = 48;  // 16 ch = 32 B + 16 B pad
 constexpr int AG_TILE_BYTES = AG_IH * AG_IW * AG_PS;      // 34560
-constexpr int AG_W_BYTES = 25 * 16 * AG_PS;               // 19200
-constexpr int AG_SMEM = AG_TILE_BYTES + AG_W_BYTES;
 
+// Aggregation: depthwise 5x5 as 25 x 2 DIAGONAL m16n8k8 MMAs (no structural zeros), its fp32 result rounded to bf16 and re-used
+// in registers as the A fragment of ONE 16x16x16 grouped-pointwise MMA pair; the depthwise output is rounded to bf16 exactly
+// where the unfused reference path materialises it.
 // ms: [B,H,W,ld] bf16.  Reads channels [grp*16, +16) (qkv), writes channels [C3 + grp*16, +16).
-// wcomb: [C3/16][25][16 n][16 i] bf16 (combined depthwise x grouped-pointwise weights).
-__global__ void __launch_bounds__(256) litemla_aggreg_tc_kernel(const bf16* ms_in, bf16* ms_out, long long ld,
-                                                                const bf16* __restrict__ wcomb, int H, int W,
-                                                                int tiles_x) {
-  extern __shared__ __align__(16) uint8_t smem[];
-  const uint32_t u_tile = static_cast<uint32_t>(__cvta_generic_to_shared(smem));
-  const uint32_t u_w = u_tile + AG_TILE_BYTES;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int tile = blockIdx.x, grp = blockIdx.y, b = blockIdx.z;
-  const int oy0 = (tile / tiles_x) * AG_TH, ox0 = (tile % tiles_x) * AG_TW;
-
-  const bf16* xb = ms_in + (long long)b * H * W * ld + grp * 16;
-  for (int i = tid; i < AG_IH * AG_IW * 2; i += 256) {
-    const int v = i & 1, p = i >> 1;
-    const int iy = oy0 - 2 + p / AG_IW, ix = ox0 - 2 + p % AG_IW;
-    const bool ok = iy >= 0 && iy < H && ix >= 0 && ix < W;
-    cpa16(u_tile + p * AG_PS + v * 16, ok ? xb + ((long long)iy * W + ix) * ld + v * 8 : xb, ok);
-  }
-  const bf16* wg = wcomb + (long long)grp * 25 * 256;
-  for (int i = tid; i < 25 * 16 * 2; i += 256) {
-    const int v = i & 1, r = i >> 1;  // r = tap*16 + n
-    cpa16(u_w + r * AG_PS + v * 16, wg + r * 16 + v * 8, true);
-  }
-  cpa_wait_all();
-  __syncthreads();
-
-  const int a_row = lane & 15, a_kh = lane >> 4;
-  const int b_n = (lane & 7) + ((lane >> 4) << 3), b_kh = (lane >> 3) & 1;
-  const int g = lane >> 2, t4 = lane & 3;
-  float acc[4][2][4];
-#pragma unroll
-  for (int m = 0; m < 4; ++m)
-#pragma unroll
-    for (int n = 0; n < 2; ++n) { acc[m][n][0] = acc[m][n][1] = acc[m][n][2] = acc[m][n][3] = 0.f; }
-
-#pragma unroll 1
-  for (int ky = 0; ky < 5; ++ky) {
-#pragma unroll
-    for (int kx = 0; kx < 5; ++kx) {
-      uint32_t b0, b1, b2, b3;
-      ldsm4(u_w + ((ky * 5 + kx) * 16 + b_n) * AG_PS + b_kh * 16, b0, b1, b2, b3);
-#pragma unroll
-      for (int m = 0; m < 4; ++m) {
-        const int y = warp * 2 + (m >> 1), x0 = (m & 1) * 16;
-        uint32_t af[4];
-        ldsm4(u_tile + ((y + ky) * AG_IW + x0 + a_row + kx) * AG_PS + a_kh * 16, af[0], af[1], af[2], af[3]);
-        mma16816(acc[m][0], af, b0, b1);
-        mma16816(acc[m][1], af, b2, b3);
-      }
-    }
-  }
-  bf16* ob = ms_out + (long long)b * H * W * ld + grp * 16;
-#pragma unroll
-  for (int m = 0; m < 4; ++m) {
-    const int oy = oy0 + warp * 2 + (m >> 1);
-    if (oy >= H) continue;
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      const int ox = ox0 + (m & 1) * 16 + g + half * 8;
-      if (ox >= W) continue;
-      bf16* dst = ob + ((long long)oy * W + ox) * ld + t4 * 2;
-      *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(acc[m][0][half * 2], acc[m][0][half * 2 + 1]);
-      *reinterpret_cast<uint32_t*>(dst + 8) = pack_bf16x2(acc[m][1][half * 2], acc[m][1][half * 2 + 1]);
-    }
-  }
-}
-
-// Second formulation of the aggregation: depthwise 5x5 as 25 x 2 DIAGONAL m16n8k8 MMAs (no structural zeros), its fp32 result
-// rounded to bf16 and re-used in registers as the A fragment of ONE 16x16x16 grouped-pointwise MMA pair.  27 half-cost MMAs
-// per 16 pixels instead of 50 full ones for the combined K = 400 contraction above; the depthwise output is rounded to bf16
-// exactly where the unfused reference path materialises it.
 // wdw: [C3/16][25][16] bf16 (group, tap, channel);  wpw: [C3][16] bf16 (output channel, input channel within its group).
 constexpr int AG2_SMEM = AG_TILE_BYTES + 25 * 16 * 2 + 16 * AG_PS;
 __device__ __forceinline__ void mma1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
@@ -370,25 +300,8 @@ __global__ void __launch_bounds__(128) litemla_apply_tc_kernel(const bf16* __res
 
 using namespace es3;
 
-// Same data contract as es3_litemla_aggreg, but the weights are the combined grouped-5x5 tensor
-// wcomb [C3/16][25][16][16] bf16, wcomb[g][tap][n][i] = wpw[g*16+n][i] * wdw[tap][g*16+i].
-extern "C" int es3_litemla_aggreg_tc(void* ms, long long ld, const void* wcomb, int B, int H, int W, int C3,
-                                     void* stream) {
-  ES3_REQUIRE(C3 % 16 == 0 && ld % 8 == 0 && ld >= 2 * C3, "es3_litemla_aggreg_tc: bad C3=%d ld=%lld", C3, ld);
-  static bool configured = false;
-  if (!configured) {
-    ES3_CHECK_CUDA(cudaFuncSetAttribute(litemla_aggreg_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_SMEM));
-    configured = true;
-  }
-  const int tiles_x = ceil_div(W, AG_TW), tiles_y = ceil_div(H, AG_TH);
-  dim3 grid(tiles_x * tiles_y, C3 / 16, B);
-  litemla_aggreg_tc_kernel<<<grid, 256, AG_SMEM, (cudaStream_t)stream>>>((const bf16*)ms, (bf16*)ms + C3, ld,
-                                                                          (const bf16*)wcomb, H, W, tiles_x);
-  ES3_LAUNCH_CHECK("litemla_aggreg_tc_kernel");
-  return 0;
-}
-
-// Same data contract; depthwise and grouped-pointwise weights separately: wdw [C3/16][25][16] bf16, wpw [C3][16] bf16.
+// ms: [B,H,W,ld] bf16 with qkv in channels [0,C3) -> writes aggreg(qkv) to channels [C3, 2*C3).
+// wdw [C3/16][25][16] bf16 (depthwise taps), wpw [C3][16] bf16 (grouped pointwise).
 extern "C" int es3_litemla_aggreg_dwpw(void* ms, long long ld, const void* wdw, const void* wpw, int B, int H, int W, int C3,
                                        void* stream) {
   ES3_REQUIRE(C3 % 16 == 0 && ld % 8 == 0 && ld >= 2 * C3, "es3_litemla_aggreg_dwpw: bad C3=%d ld=%lld", C3, ld);
@@ -405,7 +318,12 @@ extern "C" int es3_litemla_aggreg_dwpw(void* ms, long long ld, const void* wdw, 
   return 0;
 }
 
-// Same contract as es3_litemla_attn (workspace es3_litemla_ws_floats), tensor-core kernels.
+// ms: [B,HW,ld] bf16 (ld >= 48*heads2), kv_ws: fp32 workspace of B*heads2*ceil(HW/512)*17*16 floats (es3_litemla_ws_floats): the
+// partial KV sums, which es3_litemla_attn_bwd reads.  att: [B,HW,ldo] bf16 output (ldo >= 16*heads2).
+extern "C" long long es3_litemla_ws_floats(int B, int HW, int heads2) {
+  return (long long)B * heads2 * ceil_div(HW, KV_PX) * 17 * 16;
+}
+
 extern "C" int es3_litemla_attn_tc(const void* ms, long long ld, float* kv_ws, void* att, long long ldo, int B, int HW,
                                    int heads2, float eps, void* stream) {
   ES3_REQUIRE(ld >= 48 * heads2 && ld % 8 == 0 && ldo % 8 == 0, "es3_litemla_attn_tc: bad ld=%lld ldo=%lld heads2=%d", ld, ldo, heads2);

@@ -71,90 +71,10 @@ __device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b
 // part: [nblk][2][C] fp32.
 constexpr int CR_THREADS = 256;
 
-template <int ACT, bool STATS>
-__global__ void __launch_bounds__(CR_THREADS, 3) col_reduce_kernel(const bf16* __restrict__ z, const bf16* __restrict__ da,
-                                                                const float* __restrict__ scale, const float* __restrict__ shift,
-                                                                long long M, int C, int CVB, long long rows_per_block,
-                                                                float* __restrict__ part) {
-  __shared__ float red[CR_THREADS][17];
-  const int tid = threadIdx.x;
-  const int lanes = CR_THREADS / CVB;
-  const int cvl = tid % CVB, pl = tid / CVB;
-  const int cv = blockIdx.y * CVB + cvl;
-  const bool active = pl < lanes && cv * 8 < C;
-  float s0[8], s1[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) s0[i] = s1[i] = 0.f;
-  if (active) {
-    float sc[8], sh[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      sc[i] = (!STATS && scale) ? scale[cv * 8 + i] : 1.f;
-      sh[i] = (!STATS && shift) ? shift[cv * 8 + i] : 0.f;
-    }
-    float piv[8];
-    if constexpr (STATS) unpack8(__ldg(reinterpret_cast<const uint4*>(z + cv * 8)), piv);
-    const long long r0 = (long long)blockIdx.x * rows_per_block;
-    const long long r1 = min(M, r0 + rows_per_block);
-    // CR_ROWS rows per iteration: all loads (twice as many in the backward form) are issued before any arithmetic -- the kernel is
-    // a pure stream, its speed is the number of 16-byte loads in flight per SM
-    constexpr int CR_ROWS = STATS ? 4 : 2;     // (four rows in the backward form cost registers / resident CTAs)
-    for (long long r = r0 + pl; r < r1; r += (long long)CR_ROWS * lanes) {
-      uint4 uz[CR_ROWS], ud[CR_ROWS];
-      bool ok[CR_ROWS];
-#pragma unroll
-      for (int h = 0; h < CR_ROWS; ++h) {
-        const long long rr = r + (long long)h * lanes;
-        ok[h] = rr < r1;
-        uz[h] = ok[h] ? __ldg(reinterpret_cast<const uint4*>(z + rr * C + cv * 8)) : make_uint4(0, 0, 0, 0);
-        if constexpr (!STATS) ud[h] = ok[h] ? __ldg(reinterpret_cast<const uint4*>(da + rr * C + cv * 8)) : make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll
-      for (int h = 0; h < CR_ROWS; ++h) {
-        if (!ok[h]) break;
-        float fz[8];
-        unpack8(uz[h], fz);
-        if constexpr (STATS) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const float d = fz[i] - piv[i]; s0[i] += d; s1[i] = fmaf(d, d, s1[i]); }
-        } else {
-          float fd[8];
-          unpack8(ud[h], fd);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float g = fd[i] * act_grad_t<ACT>(fmaf(sc[i], fz[i], sh[i]));
-            s0[i] += g;
-            s1[i] = fmaf(g, fz[i], s1[i]);
-          }
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) { red[tid][i] = s0[i]; red[tid][8 + i] = s1[i]; }
-  __syncthreads();
-  int top = 1;
-  while (top < lanes) top <<= 1;
-  for (int stride = top >> 1; stride > 0; stride >>= 1) {
-    if (pl < stride && pl + stride < lanes) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) red[tid][i] += red[tid + stride * CVB][i];
-    }
-    __syncthreads();
-  }
-  if (pl == 0 && cv * 8 < C) {
-    float* p0 = part + ((long long)blockIdx.x * 2) * C + cv * 8;
-    float* p1 = p0 + C;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { p0[i] = red[tid][i]; p1[i] = red[tid][8 + i]; }
-  }
-}
-
-// The same reduction with the loads DECOUPLED from the registers: every thread streams its rows through a private ring of CRR_STAGES
-// 16-byte shared-memory slots per tensor with cp.async (it reads back only what it copied itself, so no barrier is involved) and keeps
-// CRR_STAGES - 1 rows in flight whatever the register pressure of the arithmetic.  The register-fed version above had two (backward
-// form) or four (statistics) rows in flight per thread; with three
-// resident CTAs this one keeps 3 x 256 x 5 x 32 B = 120 KB per SM in flight.  part / geometry identical to col_reduce_kernel.
+// The loads are DECOUPLED from the registers: every thread streams its rows through a private ring of CRR_STAGES 16-byte
+// shared-memory slots per tensor with cp.async (it reads back only what it copied itself, so no barrier is involved) and keeps
+// CRR_STAGES - 1 rows in flight whatever the register pressure of the arithmetic.  With three resident CTAs that is
+// 3 x 256 x 5 x 32 B = 120 KB per SM in flight.
 constexpr int CRR_STAGES = 6;
 template <int ACT, bool STATS>
 __global__ void __launch_bounds__(CR_THREADS, 3) col_reduce_ring_kernel(const bf16* __restrict__ z, const bf16* __restrict__ da,
@@ -717,98 +637,9 @@ __global__ void __launch_bounds__(256) dw_wgrad_strip_kernel(const bf16* __restr
   }
 }
 
-// Shared-memory tiled version for stride 1, C % 32 == 0 (the default route for these shapes since round 2, ops.DW_WGRAD_TILED;
-// GPU parity: test_dwconv_wgrad_tiled).  A CTA owns a 32-channel slab and walks
-// 8 x 32 output-pixel tiles: the dz tile and the haloed x tile are staged once with cp.async (zero fill outside the map), a
-// half-warp = the 16 channel pairs of one pixel, so every shared-memory read is 64 contiguous bytes and the KS*KS taps of a pixel
-// re-use the staged tile instead of L1.  acc[KS*KS][2] per thread (<= 50 registers) -> full occupancy.
-constexpr int DWT_TH = 8, DWT_TW = 32, DWT_CS = 32;          // tile height / width (output pixels), channel slab
-template <int KS>
-struct DwtCfg {
-  static constexpr int IH = DWT_TH + KS - 1, IW = DWT_TW + KS - 1;
-  static constexpr int X_BYTES = IH * IW * DWT_CS * 2;      // haloed input tile, 64 B per pixel
-  static constexpr int DZ_BYTES = DWT_TH * DWT_TW * DWT_CS * 2;
-  static constexpr int RED_BYTES = 8 * KS * KS * DWT_CS * 4;
-  static constexpr int SMEM = (X_BYTES + DZ_BYTES > RED_BYTES) ? X_BYTES + DZ_BYTES : RED_BYTES;
-};
-
-template <int KS>
-__global__ void __launch_bounds__(256) dw_wgrad_tiled_kernel(const bf16* __restrict__ dz, const bf16* __restrict__ x, long long ldx, int B,
-                                                             int H, int W, int C, int tiles_x, int tiles_y, float* __restrict__ part) {
-  using Cfg = DwtCfg<KS>;
-  constexpr int KK = KS * KS, PAD = KS / 2;
-  extern __shared__ __align__(16) uint8_t dwt_smem[];
-  const uint32_t u_x = static_cast<uint32_t>(__cvta_generic_to_shared(dwt_smem));
-  const uint32_t u_dz = u_x + Cfg::X_BYTES;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int cp = lane & 15, half = lane >> 4;               // channel pair inside the slab, which of the warp's two pixels
-  const int c0 = blockIdx.y * DWT_CS;
-  float acc[KK][2];
-#pragma unroll
-  for (int t = 0; t < KK; ++t) acc[t][0] = acc[t][1] = 0.f;
-  const long long ntiles = (long long)B * tiles_y * tiles_x;
-  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int tx = (int)(tile % tiles_x), ty = (int)((tile / tiles_x) % tiles_y), b = (int)(tile / ((long long)tiles_x * tiles_y));
-    const int oy0 = ty * DWT_TH, ox0 = tx * DWT_TW;
-    __syncthreads();                                         // previous tile fully consumed
-    for (int i = tid; i < Cfg::IH * Cfg::IW * 4; i += 256) {
-      const int v = i & 3, pix = i >> 2;
-      const int iy = oy0 - PAD + pix / Cfg::IW, ix = ox0 - PAD + pix % Cfg::IW;
-      const bool ok = iy >= 0 && iy < H && ix >= 0 && ix < W;
-      cpa16(u_x + pix * 64 + v * 16, ok ? x + (((long long)b * H + iy) * W + ix) * ldx + c0 + v * 8 : x, ok);
-    }
-    for (int i = tid; i < DWT_TH * DWT_TW * 4; i += 256) {
-      const int v = i & 3, pix = i >> 2;
-      const int oy = oy0 + pix / DWT_TW, ox = ox0 + pix % DWT_TW;
-      const bool ok = oy < H && ox < W;
-      cpa16(u_dz + pix * 64 + v * 16, ok ? dz + (((long long)b * H + oy) * W + ox) * C + c0 + v * 8 : dz, ok);
-    }
-    cpa_wait_all();
-    __syncthreads();
-    // warp w, half h: pixels 16 w + 2 j + h of each 128-pixel half of the tile (adjacent pixels in the two half-warps)
-#pragma unroll 2
-    for (int j = 0; j < (DWT_TH * DWT_TW) / 16; ++j) {
-      const int pix = j * 16 + warp * 2 + half;
-      const int py = pix / DWT_TW, px = pix % DWT_TW;
-      const float2 g = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dwt_smem + Cfg::X_BYTES + pix * 64 + cp * 4));
-#pragma unroll
-      for (int ky = 0; ky < KS; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < KS; ++kx) {
-          const float2 xv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dwt_smem + ((py + ky) * Cfg::IW + px + kx) * 64 + cp * 4));
-          acc[ky * KS + kx][0] = fmaf(g.x, xv.x, acc[ky * KS + kx][0]);
-          acc[ky * KS + kx][1] = fmaf(g.y, xv.y, acc[ky * KS + kx][1]);
-        }
-    }
-  }
-  // the two half-warps, then the 8 warps through shared memory: red[warp][tap][32 channels]
-#pragma unroll
-  for (int t = 0; t < KK; ++t) {
-    acc[t][0] += __shfl_xor_sync(0xffffffffu, acc[t][0], 16);
-    acc[t][1] += __shfl_xor_sync(0xffffffffu, acc[t][1], 16);
-  }
-  __syncthreads();
-  float* red = reinterpret_cast<float*>(dwt_smem);
-  if (half == 0) {
-#pragma unroll
-    for (int t = 0; t < KK; ++t) {
-      red[(warp * KK + t) * DWT_CS + cp * 2] = acc[t][0];
-      red[(warp * KK + t) * DWT_CS + cp * 2 + 1] = acc[t][1];
-    }
-  }
-  __syncthreads();
-  for (int i = tid; i < KK * DWT_CS; i += 256) {
-    float sum = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) sum += red[w * KK * DWT_CS + i];
-    const int t = i / DWT_CS, c = i % DWT_CS;
-    part[((long long)blockIdx.x * KK + t) * C + c0 + c] = sum;
-  }
-}
-
-// Sliding-window version (stride 1 | 2, C % 32 == 0; the default route since round 2, ops.DW_WGRAD_WIN).  Same staging as the tiled
-// kernel above, different walk: a thread owns one channel pair and a 16-pixel run of ONE output row, keeps the KS x KS input window
-// of the current pixel in registers (as channel-pair float2s) and slides it along x -- STRIDE new columns (KS x STRIDE shared-memory
+// Sliding-window version (stride 1 | 2, C % 32 == 0; the route for these shapes).  A CTA owns a 32-channel slab and walks 8 x 32
+// output-pixel tiles: the dz tile and the haloed x tile are staged once with cp.async (zero fill outside the map).  A thread owns one
+// channel pair and a 16-pixel run of ONE output row, keeps the KS x KS input window of the current pixel in registers (as channel-pair float2s) and slides it along x -- STRIDE new columns (KS x STRIDE shared-memory
 // reads) per pixel instead of KS x KS, every multiply-add a packed FFMA2.  Per pixel and channel pair: 3x3 s1  4 LDS + 9 FFMA2 (was
 // 10 LDS + 18 FFMA), 5x5 s1  6 + 25 (was 26 + 50), 3x3 s2  7 + 9.
 // The two half-warps of a warp walk output rows py and py + 1: the row strides are padded so that their reads fall into opposite
@@ -914,7 +745,7 @@ dw_wgrad_win_kernel(const bf16* __restrict__ dz, const bf16* __restrict__ x, lon
 // ------------------------------------------------------------------------------------------ SqueezeExcite backward (batched)
 // Per-image column reductions / per-image affine of the SqueezeExcite backward in ONE launch each (the training graph's first
 // version loops over the batch with es3_bn_act_bwd_reduce / es3_affine_act: ~100 launches per SE block at batch 32).
-// Default path since round 2 (ops.SE_BWD_BATCHED; GPU parity in tests/test_zz_train_gpu.py::test_se_bwd_batched).
+// GPU parity: tests/test_zz_train_gpu.py::test_se_bwd_batched.
 //   se_dgate:  part[chunk][b][c] = sum over the chunk's pixels of dy[b][p][c] * x[b][p][c]          grid (nchunk, B), block 256
 //   se_apply:  dx[b][p][c] = dy[b][p][c] * gate[b][c] + add[b][c]                                    one thread per 8-channel vector
 __global__ void __launch_bounds__(256) se_dgate_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, int HW, int C, int CVB,
@@ -1180,14 +1011,6 @@ __device__ __forceinline__ void load16(const bf16* p, float* f) {
   unpack8(__ldg(reinterpret_cast<const uint4*>(p) + 1), f + 8);
 }
 
-__device__ __forceinline__ void sum_kv_partials(const float* __restrict__ src, int nchunk, float* s_dst, int tid, int nthr) {
-  for (int i = tid; i < 17 * 16; i += nthr) {
-    float a = 0.f;
-    for (int c = 0; c < nchunk; ++c) a += src[(long long)c * 17 * 16 + i];
-    s_dst[i] = a;
-  }
-}
-
 // The partial KV / dKV sums are reduced ONCE per (image, head) by this kernel (fixed chunk order); round 1 had every CTA of the two
 // kernels below re-sum all chunks from global memory (43 KB of L2 reads per CTA, 0.7 GB per launch at stage 3).
 __global__ void __launch_bounds__(288) litemla_sum_partials_kernel(const float* __restrict__ src, int nchunk, float* __restrict__ dst) {
@@ -1357,12 +1180,6 @@ extern "C" long long es3_col_reduce_ws_floats(long long M, int C) {
   return (long long)nblk * 2 * C;
 }
 
-// ES3_COL_REDUCE_RING=0 selects the register-fed kernels (A/B timing); default: the cp.async ring
-static bool col_reduce_use_ring() {
-  static const bool on = [] { const char* e = getenv("ES3_COL_REDUCE_RING"); return !(e && e[0] == '0'); }();
-  return on;
-}
-
 static int col_reduce_geometry(long long M, int C, int* CVB, int* nblk, long long* rpb, int* gy) {
   const int CV = C / 8;
   *CVB = CV < CR_THREADS ? CV : CR_THREADS;
@@ -1392,31 +1209,22 @@ int es3::col_reduce_partials(bool stats, int act, const void* z, const void* da,
   long long rpb;
   col_reduce_geometry(M, C, &CVB, &nblk, &rpb, &gy);
   *nblk_out = nblk;
-  const bool ring = col_reduce_use_ring();
   if (stats) {
-    if (ring) {
-      constexpr int RING = CRR_STAGES * 1 * CR_THREADS * 16;
-      col_reduce_ring_kernel<ACT_NONE, true><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, nullptr, nullptr, nullptr, M, C, CVB, rpb, ws);
-    } else {
-      col_reduce_kernel<ACT_NONE, true><<<dim3(nblk, gy), CR_THREADS, 0, st>>>((const bf16*)z, nullptr, nullptr, nullptr, M, C, CVB, rpb, ws);
-    }
-    ES3_LAUNCH_CHECK("col_reduce_kernel<stats>");
+    constexpr int RING = CRR_STAGES * 1 * CR_THREADS * 16;
+    col_reduce_ring_kernel<ACT_NONE, true><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, nullptr, nullptr, nullptr, M, C, CVB, rpb, ws);
+    ES3_LAUNCH_CHECK("col_reduce_ring_kernel<stats>");
     return 0;
   }
   ES3_DISPATCH_ACT_BWD(act, A, {
-    if (ring) {
-      constexpr int RING = CRR_STAGES * 2 * CR_THREADS * 16;                     // 48 KB: needs the opt-in above the default 48 KB with `red`
-      static bool configured = false;
-      if (!configured) {
-        ES3_CHECK_CUDA(cudaFuncSetAttribute(col_reduce_ring_kernel<A, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RING));
-        configured = true;
-      }
-      col_reduce_ring_kernel<A, false><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, (const bf16*)da, scale, shift, M, C, CVB, rpb, ws);
-    } else {
-      col_reduce_kernel<A, false><<<dim3(nblk, gy), CR_THREADS, 0, st>>>((const bf16*)z, (const bf16*)da, scale, shift, M, C, CVB, rpb, ws);
+    constexpr int RING = CRR_STAGES * 2 * CR_THREADS * 16;                       // 48 KB: needs the opt-in above the default 48 KB with `red`
+    static bool configured = false;
+    if (!configured) {
+      ES3_CHECK_CUDA(cudaFuncSetAttribute(col_reduce_ring_kernel<A, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RING));
+      configured = true;
     }
+    col_reduce_ring_kernel<A, false><<<dim3(nblk, gy), CR_THREADS, RING, st>>>((const bf16*)z, (const bf16*)da, scale, shift, M, C, CVB, rpb, ws);
   })
-  ES3_LAUNCH_CHECK("col_reduce_kernel<bwd>");
+  ES3_LAUNCH_CHECK("col_reduce_ring_kernel<bwd>");
   return 0;
 }
 
@@ -1666,45 +1474,6 @@ extern "C" int es3_dwconv_wgrad(const void* dz, const void* x, long long ldx, in
   return 0;
 }
 
-static int dwt_blocks(int B, int H, int W, int C) {
-  const long long ntiles = (long long)B * ceil_div(H, DWT_TH) * ceil_div(W, DWT_TW);
-  long long want = (4LL * 132 + C / DWT_CS - 1) / (C / DWT_CS);      // ~4 CTAs per SM over all channel slabs
-  if (want > ntiles) want = ntiles;
-  if (want < 1) want = 1;
-  return (int)want;
-}
-
-extern "C" long long es3_dwconv_wgrad_tiled_ws_floats(int B, int H, int W, int C, int ks) {
-  return (long long)dwt_blocks(B, H, W, C) * ks * ks * C;
-}
-
-/* Same contract as es3_dwconv_wgrad for stride 1 and C % 32 == 0, shared-memory tiled (not yet the default: unmeasured). */
-extern "C" int es3_dwconv_wgrad_tiled(const void* dz, const void* x, long long ldx, int B, int H, int W, int C, int ks, float* ws,
-                                      float* dW, void* stream) {
-  ES3_REQUIRE(C % DWT_CS == 0 && ldx % 8 == 0 && (ks == 3 || ks == 5), "es3_dwconv_wgrad_tiled: need C %% 32 == 0, ks 3|5 (C=%d ks=%d)", C, ks);
-  ES3_REQUIRE(((uintptr_t)dz & 15) == 0 && ((uintptr_t)x & 15) == 0, "es3_dwconv_wgrad_tiled: operands must be 16-byte aligned");
-  const int nblk = dwt_blocks(B, H, W, C);
-  const int tiles_x = ceil_div(W, DWT_TW), tiles_y = ceil_div(H, DWT_TH);
-  cudaStream_t st = (cudaStream_t)stream;
-  static bool configured = false;
-  if (!configured) {
-    ES3_CHECK_CUDA(cudaFuncSetAttribute(dw_wgrad_tiled_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, DwtCfg<3>::SMEM));
-    ES3_CHECK_CUDA(cudaFuncSetAttribute(dw_wgrad_tiled_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, DwtCfg<5>::SMEM));
-    configured = true;
-  }
-  if (ks == 3)
-    dw_wgrad_tiled_kernel<3><<<dim3(nblk, C / DWT_CS), 256, DwtCfg<3>::SMEM, st>>>((const bf16*)dz, (const bf16*)x, ldx, B, H, W, C, tiles_x,
-                                                                                    tiles_y, ws);
-  else
-    dw_wgrad_tiled_kernel<5><<<dim3(nblk, C / DWT_CS), 256, DwtCfg<5>::SMEM, st>>>((const bf16*)dz, (const bf16*)x, ldx, B, H, W, C, tiles_x,
-                                                                                    tiles_y, ws);
-  ES3_LAUNCH_CHECK("dw_wgrad_tiled_kernel");
-  const long long n = (long long)ks * ks * C;
-  sum_partials_kernel<<<(unsigned)ceil_div(n, 32), 256, 0, st>>>(ws, nblk, n, C, 1, (long long)ks * ks, dW);
-  ES3_LAUNCH_CHECK("sum_partials_kernel");
-  return 0;
-}
-
 static int dww_blocks(int B, int Ho, int Wo, int C) {
   const long long ntiles = (long long)B * ceil_div(Ho, DWW_TH) * ceil_div(Wo, DWW_TW);
   long long want = (2LL * 132 + C / DWW_CS - 1) / (C / DWW_CS);      // two resident CTAs per SM over all channel slabs
@@ -1866,13 +1635,13 @@ extern "C" long long es3_litemla_bwd_ws_floats(int B, int HW, int heads2) {
   return (long long)B * heads2 * (ceil_div(HW, LB_PX) + 2) * 17 * 16;
 }
 
-/* kv_part: the [B][heads2][nchunk_f][17][16] partial KV sums es3_litemla_attn[_tc] left in its workspace
+/* kv_part: the [B][heads2][nchunk_f][17][16] partial KV sums es3_litemla_attn_tc left in its workspace
  * (nchunk_f = ceil(HW / 512)). */
 extern "C" int es3_litemla_attn_bwd(const void* ms, long long ld, const void* dy, long long lddy, const float* kv_part, int nchunk_f,
                                     float* dkv_ws, void* dms, long long lddms, int B, int HW, int heads2, float eps, void* stream) {
   ES3_REQUIRE(ld >= 48 * heads2 && ld % 8 == 0 && lddy % 8 == 0 && lddms % 8 == 0 && lddy >= 16 * heads2 && lddms >= 48 * heads2,
               "es3_litemla_attn_bwd: bad strides ld=%lld lddy=%lld lddms=%lld heads2=%d", ld, lddy, lddms, heads2);
-  ES3_REQUIRE(nchunk_f == ceil_div(HW, 512), "es3_litemla_attn_bwd: kv_part must come from es3_litemla_attn (nchunk %d != %d)", nchunk_f,
+  ES3_REQUIRE(nchunk_f == ceil_div(HW, 512), "es3_litemla_attn_bwd: kv_part must come from es3_litemla_attn_tc (nchunk %d != %d)", nchunk_f,
               ceil_div(HW, 512));
   cudaStream_t st = (cudaStream_t)stream;
   const int nchunk_b = ceil_div(HW, LB_PX);

@@ -47,7 +47,7 @@ class strict_precision:
 
 # ------------------------------------------------------------------------------------ accounting
 # kernels launched per C-ABI call (memsets excluded) -- bench.py reports the sum as `gpu_launches`.
-KERNELS_PER_CALL = {"es3_colsum_f32": 2, "es3_layernorm_bwd": 2, "es3_litemla_attn": 2, "es3_litemla_attn_generic": 2, "es3_fill_small_components": 4, "es3_grad_norm": 2, "es3_adamw_flat": 2, "es3_litemla_attn_tc": 2, "es3_kd_loss_fwd": 2, "es3_channel_mean": 2}
+KERNELS_PER_CALL = {"es3_colsum_f32": 2, "es3_layernorm_bwd": 2, "es3_litemla_attn_generic": 2, "es3_fill_small_components": 4, "es3_grad_norm": 2, "es3_adamw_flat": 2, "es3_litemla_attn_tc": 2, "es3_kd_loss_fwd": 2, "es3_channel_mean": 2}
 launch_count = 0
 
 
@@ -96,6 +96,24 @@ def _call(name, tag, nbytes, flops, *args):
     _profiler.records.append((tag, e0, e1, nbytes, flops))
 
 
+def _call_rc(name, tag, nbytes, flops, *args):
+    """Try one C-ABI op that returns -1 for shapes it does not instantiate (_lib.call_rc); launches and the profiler entry are
+    counted only when it ran (rc == 0)."""
+    global launch_count
+    if _profiler is None:
+        rc = _lib.call_rc(name, *args)
+    else:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        rc = _lib.call_rc(name, *args)
+        if rc == 0:
+            e1.record()
+            _profiler.records.append((tag, e0, e1, nbytes, flops))
+    if rc == 0:
+        launch_count += KERNELS_PER_CALL.get(name, 1)
+    return rc
+
+
 def _chk(t: torch.Tensor, dtype, name: str):
     if not t.is_cuda:
         raise _lib.Es3Error(f"{name}: expected a CUDA tensor (the native path has no CPU fallback)")
@@ -137,18 +155,9 @@ def gemm(a, w, *, scale=None, bias=None, act=None, residual=None, out=None, out_
     if (PW_SMALL and K <= 64 and N <= 64 and scale is None and bias is None and act in (None, "none") and rope is None
             and out.dtype == torch.bfloat16 and (residual is None or residual.dtype == torch.bfloat16)):
         # 16..64-channel pointwise convs of stages 0-1 (and their input gradients): one thread per pixel row (pw_small.cu)
-        global launch_count
-        prof = _profiler
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        rc = _lib.call_rc("es3_pw_small_bf16", a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), out.data_ptr(), out.stride(0),
-                          _ptr(residual), residual.stride(0) if residual is not None else 0, M, N, K, _stream())
-        if rc == 0:
-            launch_count += 1
-            if prof is not None:
-                e1.record()
-                prof.records.append((f"pw_small[K={K},N={N}]", e0, e1, M * K * 2 + M * N * 2 + _nb(w, residual), 2 * M * N * K))
+        if _call_rc("es3_pw_small_bf16", f"pw_small[K={K},N={N}]", M * K * 2 + M * N * 2 + _nb(w, residual), 2 * M * N * K,
+                    a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), out.data_ptr(), out.stride(0),
+                    _ptr(residual), residual.stride(0) if residual is not None else 0, M, N, K, _stream()) == 0:
             return out
     if rope is not None:
         tab, rcols, rH, rW, rwin = rope
@@ -227,12 +236,9 @@ def _tc_taps(w):
     return c[1]
 
 
-DW_TC = True   # stride-1 3x3 / 5x5 depthwise convs with C % 32 == 0 on the tensor-core kernel (csrc/dw_tc.cu; GPU parity: test_dwconv_tc)
-
-
-def dwconv(x, w, bias, ks, stride, act, out=None, force_simple=False, impl=None):
-    """x: [B,H,W,C] bf16 (channel-sliced views allowed); w: [ks*ks, C] fp32.  impl: None (default routing), "tc" (tensor-core kernel,
-    stride 1), "tiled" (CUDA-core shared-memory kernel)."""
+def dwconv(x, w, bias, ks, stride, act, out=None, force_simple=False):
+    """x: [B,H,W,C] bf16 (channel-sliced views allowed); w: [ks*ks, C] fp32.  C % 32 == 0 runs on the tensor-core kernel at stride 1
+    (csrc/dw_tc.cu) and the shared-memory tiled kernel at stride 2; other C, and force_simple, on the one-thread-per-output kernel."""
     _chk(x, torch.bfloat16, "x")
     _ensure_init(x)
     B, H, W, Cc = x.shape
@@ -241,7 +247,7 @@ def dwconv(x, w, bias, ks, stride, act, out=None, force_simple=False, impl=None)
     Ho, Wo = (H + 2 * pad - ks) // stride + 1, (W + 2 * pad - ks) // stride + 1
     if out is None:
         out = torch.empty((B, Ho, Wo, Cc), device=x.device, dtype=torch.bfloat16)
-    if DW_TC and stride == 1 and ks in (3, 5) and Cc % 32 == 0 and not force_simple and impl in (None, "tc"):
+    if stride == 1 and ks in (3, 5) and Cc % 32 == 0 and not force_simple:
         _call("es3_dwconv_tc_bf16", f"dwconv_tc{ks}x{ks}", B * H * W * Cc * 2 + B * Ho * Wo * Cc * 2, 2 * B * Ho * Wo * Cc * ks * ks,
               x.data_ptr(), x.stride(2), _tc_taps(w).data_ptr(), _ptr(bias), out.data_ptr(), out.stride(2), B, H, W, Cc, ks, ACT[act], _stream())
         return out
@@ -307,37 +313,6 @@ def nchw_f32_to_nhwc(x):
     return out
 
 
-def litemla_aggreg(ms, wdw, wpw, C3, force_simple=False):
-    """ms: [B,H,W,2*C3] bf16; fills channels [C3, 2*C3) in place."""
-    _chk(ms, torch.bfloat16, "ms")
-    _ensure_init(ms)
-    assert ms.is_contiguous()
-    B, H, W, ld = ms.shape
-    fn = "es3_litemla_aggreg_tiled" if (C3 % 64 == 0 and not force_simple) else "es3_litemla_aggreg"
-    _call(fn, "litemla_aggreg", 2 * B * H * W * C3 * 2, 2 * B * H * W * C3 * (25 + 16), ms.data_ptr(), ld, wdw.data_ptr(), wpw.data_ptr(), B, H, W, C3, _stream())
-    return ms
-
-
-def litemla_wcomb(wdw, wpw):
-    """Combined aggreg weights: wdw [25, C3] fp32 (tap-major), wpw [C3, 16] fp32 -> [C3/16, 25, 16, 16] bf16."""
-    C3 = wpw.shape[0]
-    G = C3 // 16
-    d = wdw.t().reshape(G, 16, 25)                     # [g][i][tap]
-    w = wpw.reshape(G, 16, 16)                         # [g][n][i]
-    comb = w.unsqueeze(1) * d.permute(0, 2, 1).unsqueeze(2)   # [g][tap][n][i]
-    return comb.to(torch.bfloat16).contiguous()
-
-
-def litemla_aggreg_tc(ms, wcomb, C3):
-    _chk(ms, torch.bfloat16, "ms"); _chk(wcomb, torch.bfloat16, "wcomb")
-    _ensure_init(ms)
-    assert ms.is_contiguous() and wcomb.is_contiguous() and wcomb.shape == (C3 // 16, 25, 16, 16)
-    B, H, W, ld = ms.shape
-    _call("es3_litemla_aggreg_tc", "litemla_aggreg_tc", 2 * B * H * W * C3 * 2, 2 * B * H * W * C3 * 400,
-          ms.data_ptr(), ld, wcomb.data_ptr(), B, H, W, C3, _stream())
-    return ms
-
-
 def litemla_dwpw_weights(wdw, wpw):
     """wdw [25, C3] fp32 (tap-major), wpw [C3, 16] fp32 -> ([C3/16, 25, 16] bf16, [C3, 16] bf16) for es3_litemla_aggreg_dwpw."""
     C3 = wpw.shape[0]
@@ -356,16 +331,16 @@ def litemla_aggreg_dwpw(ms, wd, wp, C3):
     return ms
 
 
-def litemla_attn(ms, heads2, eps=1e-15, tc=True, return_kv=False):
-    """ms: [B,H,W,48*heads2] bf16 -> att [B,H,W,16*heads2] bf16.  return_kv: also return the workspace holding the
-    [B][heads2][ceil(HW/512)][17][16] partial KV sums (es3_litemla_attn_bwd consumes it)."""
+def litemla_attn(ms, heads2, eps=1e-15, return_kv=False):
+    """ms: [B,H,W,48*heads2] bf16 -> att [B,H,W,16*heads2] bf16 (tensor-core kernels).  return_kv: also return the workspace holding
+    the [B][heads2][ceil(HW/512)][17][16] partial KV sums (es3_litemla_attn_bwd consumes it)."""
     _chk(ms, torch.bfloat16, "ms")
     _ensure_init(ms)
     assert ms.is_contiguous()
     B, H, W, ld = ms.shape
     att = torch.empty((B, H, W, 16 * heads2), device=ms.device, dtype=torch.bfloat16)
     kv = torch.empty((B * heads2 * ((H * W + 511) // 512) * 17 * 16,), device=ms.device, dtype=torch.float32)
-    _call("es3_litemla_attn_tc" if tc else "es3_litemla_attn", "litemla_attn_tc" if tc else "litemla_attn", _nb(ms) * 2 // 3 + _nb(ms) // 3 + _nb(att), 2 * B * H * W * heads2 * 17 * 16 * 2,
+    _call("es3_litemla_attn_tc", "litemla_attn_tc", _nb(ms) * 2 // 3 + _nb(ms) // 3 + _nb(att), 2 * B * H * W * heads2 * 17 * 16 * 2,
           ms.data_ptr(), ld, kv.data_ptr(), att.data_ptr(), att.shape[3], B, H * W, heads2,
               float(eps), _stream())
     return (att, kv) if return_kv else att
@@ -385,13 +360,9 @@ def litemla_attn_generic(ms, heads2, dim, eps=1e-15, return_kv=False):
     return (att, kv) if return_kv else att
 
 
-MBCONV_TC = True   # stride-1 residual blocks on the wgmma kernel (es3_mbconv_tc_bf16); False -> mma.sync kernel only
-
-
 def mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, residual, act, impl=None):
     """Fused MBConv (expand -> dw3x3 -> project [+x]); returns None when the shape is not instantiated.
     impl: None = wgmma kernel where it applies, else the mma.sync kernel; "tc" / "mma" force one (None if not instantiated)."""
-    global launch_count
     _chk(x, torch.bfloat16, "x")
     _ensure_init(x)
     assert x.is_contiguous()
@@ -403,31 +374,20 @@ def mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, residual, act, impl
     args = (x.data_ptr(), y.data_ptr(), w1.data_ptr(), s1.data_ptr(), b1.data_ptr(), wdw.data_ptr(), b2.data_ptr(),
             w3.data_ptr(), s3.data_ptr(), b3.data_ptr(), B, H, W, Cin, Mid, Cout, stride, int(residual), ACT[act],
             _stream())
-    prof = _profiler
-    if prof is not None:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-    rc, tag = -1, "mbconv_tc"
-    if impl == "tc" or (impl is None and MBCONV_TC):
-        rc = _lib.call_rc("es3_mbconv_tc_bf16", *args)
+    shape, nbytes, flops = f"[{Cin}-{Mid}-{Cout},s{stride}]", _nb(x, y), 2 * B * (H * W * Cin * Mid + Ho * Wo * Mid * (9 + Cout))
+    rc = -1
+    if impl in (None, "tc"):
+        rc = _call_rc("es3_mbconv_tc_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
         if rc < 0:
-            rc = _lib.call_rc("es3_mbconv_tc_s2_bf16", *args)
+            rc = _call_rc("es3_mbconv_tc_s2_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
     if rc < 0 and impl != "tc":
-        rc, tag = _lib.call_rc("es3_mbconv_fused_bf16", *args), "mbconv_fused"
-    if rc < 0:
-        return None
-    launch_count += 1
-    if prof is not None:
-        e1.record()
-        flops = 2 * B * (H * W * Cin * Mid + Ho * Wo * Mid * (9 + Cout))
-        prof.records.append((f"{tag}[{Cin}-{Mid}-{Cout},s{stride}]", e0, e1, _nb(x, y), flops))
-    return y
+        rc = _call_rc("es3_mbconv_fused_bf16", "mbconv_fused" + shape, nbytes, flops, *args)
+    return y if rc == 0 else None
 
 
 def dwproj(mid, wdw, b2, w3, s3, b3, residual=None, act="hswish"):
     """act(dw3x3(mid) + b2) -> 1x1 projection -> s3 * . + b3 (+ residual) in one wgmma kernel; None if the shape is not
     instantiated (the caller then runs dwconv + gemm).  mid [B,H,W,Mid] bf16, w3 [Cout, Mid] bf16, residual [B,H,W,Cout]."""
-    global launch_count
     _chk(mid, torch.bfloat16, "mid"); _chk(w3, torch.bfloat16, "w3")
     _ensure_init(mid)
     assert mid.is_contiguous() and w3.is_contiguous()
@@ -437,19 +397,10 @@ def dwproj(mid, wdw, b2, w3, s3, b3, residual=None, act="hswish"):
         _chk(residual, torch.bfloat16, "residual")
         assert residual.is_contiguous() and residual.shape == (B, H, W, Cout)
     y = torch.empty((B, H, W, Cout), device=mid.device, dtype=torch.bfloat16)
-    prof = _profiler
-    if prof is not None:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-    rc = _lib.call_rc("es3_dwproj_tc_bf16", mid.data_ptr(), _tc_taps(wdw).data_ptr(), b2.data_ptr(), w3.data_ptr(), s3.data_ptr(),
-                      b3.data_ptr(), _ptr(residual), y.data_ptr(), B, H, W, Mid, Cout, ACT[act], _stream())
-    if rc < 0:
-        return None
-    launch_count += 1
-    if prof is not None:
-        e1.record()
-        prof.records.append((f"dwproj_tc[{Mid}-{Cout}]", e0, e1, _nb(mid, y, residual), 2 * B * H * W * Mid * (9 + Cout)))
-    return y
+    rc = _call_rc("es3_dwproj_tc_bf16", f"dwproj_tc[{Mid}-{Cout}]", _nb(mid, y, residual), 2 * B * H * W * Mid * (9 + Cout),
+                  mid.data_ptr(), _tc_taps(wdw).data_ptr(), b2.data_ptr(), w3.data_ptr(), s3.data_ptr(), b3.data_ptr(), _ptr(residual),
+                  y.data_ptr(), B, H, W, Mid, Cout, ACT[act], _stream())
+    return y if rc == 0 else None
 
 
 def layernorm(x, gamma, beta, eps=1e-5, *, pos=None, pos_size=0, H=0, W=0, out_bf16=True, out_f32=False):
@@ -1262,8 +1213,8 @@ def win_attn_bias(qkv, qkv_pad, bias, B, H, W, C, heads, ws, scale):
 # ------------------------------------------------------------------------------------ student backward (train_bwd.cu)
 BN_MODE = {"none": 0, "eval": 1, "batch": 2}
 KERNELS_PER_CALL.update({"es3_bn_stats": 2, "es3_bn_act_bwd_reduce": 2, "es3_wgrad_pw": 2, "es3_dwconv_wgrad": 2,
-                         "es3_stem_wgrad": 2, "es3_litemla_attn_bwd": 4, "es3_dwconv_wgrad_tiled": 2, "es3_se_bwd_dgate": 2,
-                         "es3_litemla_attn_bwd_generic": 2})
+                         "es3_stem_wgrad": 2, "es3_litemla_attn_bwd": 4, "es3_se_bwd_dgate": 2,
+                         "es3_litemla_attn_bwd_generic": 2, "es3_wgrad_tc": 2})
 
 
 def _f32ws(n, dev):
@@ -1442,9 +1393,6 @@ def add_bf16(a, b):
     return out
 
 
-WGRAD_TC = True    # 1x1-conv weight gradients with N % 64 == 0 and K % 64 == 0 on the wgmma split-K kernel (es3_wgrad_tc)
-
-
 def wgrad_pw(dz, x, dW, ldn=None, ldk=1, shift=None):
     """dW[n*ldn + k*ldk] += sum_m dz[m,n] x[m,k].  dz [M,N], x [M,K] bf16 (row strides allowed); dW fp32 (flat indexing
     from its data pointer).  shift = (H, W, dy, dx): x row of pixel (b,y,x) is (b,y+dy,x+dx), zero outside the map."""
@@ -1453,21 +1401,11 @@ def wgrad_pw(dz, x, dW, ldn=None, ldk=1, shift=None):
     assert dz.dim() == 2 and x.dim() == 2 and dz.stride(1) == 1 and x.stride(1) == 1 and dz.shape[0] == x.shape[0]
     M, N = dz.shape
     K = x.shape[1]
-    if WGRAD_TC and shift is None and ldk == 1 and N % 64 == 0 and K % 64 == 0 and M >= 64:
+    if shift is None and ldk == 1 and N % 64 == 0 and K % 64 == 0 and M >= 64:
         # dense contraction over the pixel index: split-K wgmma with both operands MN-major (wgrad_tc.cu)
-        global launch_count
         ws = _f32ws(_lib.size("es3_wgrad_tc_ws_floats", M, N, K), dz.device)
-        prof = _profiler
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        rc = _lib.call_rc("es3_wgrad_tc", dz.data_ptr(), dz.stride(0), x.data_ptr(), x.stride(0), M, N, K, ws.data_ptr(), dW.data_ptr(),
-                          K if ldn is None else ldn, _stream())
-        if rc == 0:
-            launch_count += 2
-            if prof is not None:
-                e1.record()
-                prof.records.append((f"wgrad_tc[N={N},K={K}]", e0, e1, M * (N + K) * 2, 2 * M * N * K))
+        if _call_rc("es3_wgrad_tc", f"wgrad_tc[N={N},K={K}]", M * (N + K) * 2, 2 * M * N * K, dz.data_ptr(), dz.stride(0), x.data_ptr(),
+                    x.stride(0), M, N, K, ws.data_ptr(), dW.data_ptr(), K if ldn is None else ldn, _stream()) == 0:
             return dW
     H, W, dy, dx = shift if shift is not None else (0, 0, 0, 0)
     ws = _f32ws(_lib.size("es3_wgrad_pw_ws_floats", M, N, K), dz.device)
@@ -1531,30 +1469,20 @@ def dwconv_bwd_data(dz, w, H, W, ks, stride):
     return dx
 
 
-DW_WGRAD_WIN = True      # route C % 32 == 0 weight gradients (stride 1 | 2) to es3_dwconv_wgrad_win (GPU parity: test_dwconv_wgrad_win)
-DW_WGRAD_TILED = True    # route stride-1, C % 32 == 0 weight gradients to es3_dwconv_wgrad_tiled (GPU parity: test_dwconv_wgrad_tiled, r2)
-
-
 def dwconv_wgrad(dz, x, dW, ks, stride, impl=None):
     """dW [C,1,ks,ks] fp32 += depthwise weight gradient; dz [B,Ho,Wo,C] bf16 contiguous, x [B,H,W,C] bf16 (channel slice ok).
-    impl="win": register sliding window over shared-memory tiles (C % 32 == 0; the default for such shapes); impl="tiled": the first
-    shared-memory tiled kernel (stride 1, C % 32 == 0); impl="direct": the global-memory kernels."""
+    C % 32 == 0 runs the register sliding window over shared-memory tiles (es3_dwconv_wgrad_win), any other C the global-memory
+    kernels (es3_dwconv_wgrad).  impl="win" / "direct" forces one of the two."""
     _chk(dz, torch.bfloat16, "dz"); _chk(x, torch.bfloat16, "x"); _chk(dW, torch.float32, "dW")
     _ensure_init(dz)
     B, H, W, C = x.shape
     assert dz.is_contiguous() and dW.is_contiguous() and dW.numel() == C * ks * ks and dz.shape[3] == C
     assert x.stride(3) == 1 and x.stride(1) == W * x.stride(2) and x.stride(0) == H * x.stride(1)
-    if impl == "win" or (impl is None and DW_WGRAD_WIN and C % 32 == 0):
+    if impl == "win" or (impl is None and C % 32 == 0):
         assert C % 32 == 0
         ws = _f32ws(_lib.size("es3_dwconv_wgrad_win_ws_floats", B, H, W, C, ks, stride), dz.device)
         _call("es3_dwconv_wgrad_win", f"dwconv_wgrad_win{ks}x{ks}s{stride}", _nb(dz) + B * H * W * C * 2, 2 * dz.numel() * ks * ks,
               dz.data_ptr(), x.data_ptr(), x.stride(2), B, H, W, C, ks, stride, ws.data_ptr(), dW.data_ptr(), _stream())
-        return dW
-    if impl == "tiled" or (impl is None and DW_WGRAD_TILED and stride == 1 and C % 32 == 0):   # (impl="direct" falls through)
-        assert stride == 1 and C % 32 == 0
-        ws = _f32ws(_lib.size("es3_dwconv_wgrad_tiled_ws_floats", B, H, W, C, ks), dz.device)
-        _call("es3_dwconv_wgrad_tiled", f"dwconv_wgrad_tiled{ks}x{ks}", _nb(dz) + B * H * W * C * 2, 2 * dz.numel() * ks * ks,
-              dz.data_ptr(), x.data_ptr(), x.stride(2), B, H, W, C, ks, ws.data_ptr(), dW.data_ptr(), _stream())
         return dW
     ws = _f32ws(_lib.size("es3_dwconv_wgrad_ws_floats", B, H, W, C, ks, stride), dz.device)
     _call("es3_dwconv_wgrad", f"dwconv_wgrad{ks}x{ks}s{stride}", _nb(dz) + B * H * W * C * 2, 2 * dz.numel() * ks * ks,
@@ -1621,9 +1549,6 @@ def colsum_f32(src, out):
     ws = _f32ws(_lib.size("es3_colsum_f32_ws_floats", M, L), src.device)
     _call("es3_colsum_f32", "colsum_f32", _nb(src), M * L, src.data_ptr(), src.stride(0), M, L, ws.data_ptr(), out.data_ptr(), _stream())
     return out
-
-
-SE_BWD_BATCHED = True    # SqueezeExcite backward through es3_se_bwd_* instead of per-image loops (GPU parity: test_se_bwd_batched, r2)
 
 
 def se_bwd_dgate(dy, x):

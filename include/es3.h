@@ -76,7 +76,7 @@ int es3_stem_conv3x3_s2(const float* x, const float* w, const float* bias, void*
 int es3_dwconv_bf16(const void* x, long long ldx, const float* w, const float* bias, void* out, long long ldo, int B,
                     int H, int W, int C, int ks, int stride, int act, void* stream);
 
-/* Same contract as es3_dwconv_bf16 (C % 32 == 0): shared-memory tiled, 4-pixel register strips. */
+/* Same contract as es3_dwconv_bf16 for ks 3, stride 2, C % 32 == 0: shared-memory tiled, 4-pixel register strips. */
 int es3_dwconv_tiled_bf16(const void* x, long long ldx, const float* w, const float* bias, void* out, long long ldo,
                           int B, int H, int W, int C, int ks, int stride, int act, void* stream);
 
@@ -97,7 +97,7 @@ int es3_stem_fused_c16(const float* img, const void* w0, const float* s0, const 
  * tensor kept in shared memory (mma.sync expand/project around an fp32 depthwise).  w1 [Mid][Cin], w3 [Cout][Mid]
  * bf16; s1,b1,b2 [Mid], s3,b3 [Cout] fp32 (BN folded; ones/zeros where the reference has bias-only convs);
  * wdw [9][Mid] fp32.  Returns -1 (no error set) when the shape is not instantiated -- the caller then runs
- * es3_gemm_bf16 + es3_dwconv_tiled_bf16.  Replaces MBConv inside ResidualBlock (efficientvit/nn/ops.py:315-367,
+ * es3_gemm_bf16 + es3_dwconv_tc_bf16 / es3_dwconv_tiled_bf16.  Replaces MBConv inside ResidualBlock (efficientvit/nn/ops.py:315-367,
  * 740-770) for efficientvit_b1 stages 1-3 heads. */
 int es3_mbconv_fused_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
                           const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W,
@@ -118,7 +118,7 @@ int es3_mbconv_tc_s2_bf16(const void* x, void* y, const void* w1, const float* s
  * 64-channel chunks with its halo, the depthwise runs as diagonal m16n8k8 MMAs, its output goes straight into the swizzled A
  * operand of wgmmas accumulating [128 px x Cout] in registers.  wdw [9][Mid] fp32 (BN scale folded), b2 [Mid], w3 [Cout][Mid] bf16,
  * s3/b3 [Cout]; residual [B,H,W,Cout] bf16 or NULL.  Instantiated (Mid, Cout) = (512,128), (1024,256); -1 otherwise.
- * Replaces es3_dwconv_tiled_bf16 + es3_gemm_bf16 for ops.py:315-367 (depth_conv + point_conv). */
+ * Replaces es3_dwconv_tc_bf16 + es3_gemm_bf16 for ops.py:315-367 (depth_conv + point_conv). */
 int es3_dwproj_tc_bf16(const void* mid, const float* wdw, const float* b2, const void* w3, const float* s3, const float* b3,
                        const void* residual, void* y, int B, int H, int W, int Mid, int Cout, int act, void* stream);
 
@@ -131,26 +131,18 @@ int es3_nhwc_to_nchw_f32(const void* in, float* out, int B, int HW, int C, void*
 int es3_nchw_f32_to_nhwc(const float* in, void* out, int B, int HW, int C, void* stream);
 
 /* ------------------------------------------------------------------------------------------ LiteMLA */
-/* ms [B,H,W,ld] bf16: reads qkv in channels [0,C3), writes aggreg(qkv) = grouped1x1(dw5x5(qkv)) into
- * channels [C3,2*C3).  wdw [25][C3] fp32, wpw [C3][16] fp32.  Replaces LiteMLA.aggreg (ops.py:560-575,655-660). */
-int es3_litemla_aggreg(void* ms, long long ld, const float* wdw, const float* wpw, int B, int H, int W, int C3,
-                       void* stream);
-/* Same contract as es3_litemla_aggreg (C3 % 64 == 0): tiled dw5x5 with the grouped 1x1 fused in registers. */
-int es3_litemla_aggreg_tiled(void* ms, long long ld, const float* wdw, const float* wpw, int B, int H, int W, int C3,
-                             void* stream);
-/* Tensor-core aggreg: the depthwise 5x5 and the grouped 1x1 are folded into one grouped 5x5 conv,
- * wcomb [C3/16][25][16][16] bf16 with wcomb[g][tap][n][i] = wpw[g*16+n][i] * wdw[tap][g*16+i] (K = 400 per group). */
-int es3_litemla_aggreg_tc(void* ms, long long ld, const void* wcomb, int B, int H, int W, int C3, void* stream);
-/* Same contract with the two weight tensors kept apart: depthwise 5x5 as diagonal m16n8k8 MMAs, its bf16-rounded result fed
- * from registers into the grouped 16x16 pointwise MMA.  wdw [C3/16][25][16] bf16 (group, tap, channel), wpw [C3][16] bf16. */
+/* ms [B,H,W,ld] bf16: reads qkv in channels [0,C3), writes aggreg(qkv) = grouped1x1(dw5x5(qkv)) into channels [C3,2*C3).
+ * Replaces LiteMLA.aggreg (ops.py:560-575,655-660).  Depthwise 5x5 as diagonal m16n8k8 MMAs, its bf16-rounded result fed from
+ * registers into the grouped 16x16 pointwise MMA.  wdw [C3/16][25][16] bf16 (group, tap, channel), wpw [C3][16] bf16. */
 int es3_litemla_aggreg_dwpw(void* ms, long long ld, const void* wdw, const void* wpw, int B, int H, int W, int C3,
                             void* stream);
-/* ReLU linear attention over the multi-scale qkv buffer (head h = channels [48h,48h+48) = q|k|v, dim 16).
- * kv_ws: es3_litemla_ws_floats(B,HW,heads2) floats of scratch (two-stage deterministic reduction, no atomics).  att [B,HW,ldo] bf16.  Replaces relu_linear_att (ops.py:584-621). */
+/* ReLU linear attention over the multi-scale qkv buffer (head h = channels [48h,48h+48) = q|k|v, dim 16) on mma.sync: KV state
+ * and the apply step (KV split hi+lo bf16).  kv_ws: es3_litemla_ws_floats(B,HW,heads2) floats of scratch (two-stage deterministic
+ * reduction, no atomics).  att [B,HW,ldo] bf16.  Replaces relu_linear_att (ops.py:584-621). */
 long long es3_litemla_ws_floats(int B, int HW, int heads2);
-int es3_litemla_attn(const void* ms, long long ld, float* kv_ws, void* att, long long ldo, int B, int HW, int heads2,
-                     float eps, void* stream);
-/* Same contract for any head dim in {16, 32} (efficientvit_b2 / b3: dim 32): head h occupies channels [h*3*dim, +3*dim)
+int es3_litemla_attn_tc(const void* ms, long long ld, float* kv_ws, void* att, long long ldo, int B, int HW, int heads2,
+                        float eps, void* stream);
+/* The same attention for any head dim in {16, 32} (efficientvit_b2 / b3: dim 32): head h occupies channels [h*3*dim, +3*dim)
  * of ms as q|k|v and [h*dim, +dim) of att.  CUDA-core fp32 formulation; kv_ws = es3_litemla_generic_ws_floats floats. */
 long long es3_litemla_generic_ws_floats(int B, int HW, int heads2, int dim);
 int es3_litemla_attn_generic(const void* ms, long long ld, float* kv_ws, void* att, long long ldo, int B, int HW, int heads2,
@@ -181,10 +173,6 @@ int es3_tokens_f32_to_nchw(const float* in, float* out, int B, int HW, int C, vo
 /* fp32 -> fp16 (RN) over n contiguous elements: the stored format of the teacher-embedding dump
  * (save_embedding_image_stage1.py:92); done on the device so the D2H copy moves 2 bytes per element. */
 int es3_cast_f32_to_f16(const float* in, void* out, long long n, void* stream);
-
-/* Same contract as es3_litemla_attn; KV state and the apply step run on mma.sync (KV split hi+lo bf16). */
-int es3_litemla_attn_tc(const void* ms, long long ld, float* kv_ws, void* att, long long ldo, int B, int HW, int heads2,
-                        float eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------ text encoders */
 /* Causal softmax attention, head_dim 64, over B sequences of L tokens on the fused qkv activation [B*L, 3C] bf16 ->
@@ -469,10 +457,8 @@ int es3_win_attn_bias_bwd(const void* qkv, const void* dout, const float* bias, 
                           int C, int num_heads, int ws, float scale, void* stream);
 long long es3_colsum_f32_ws_floats(long long M, int L);
 int es3_colsum_f32(const float* src, long long ld, long long M, int L, float* ws, float* out, void* stream);
-/* Shared-memory tiled variant of es3_dwconv_wgrad for stride 1 and C % 32 == 0 (same result contract).  The default
- * route for these shapes (GPU parity: test_dwconv_wgrad_tiled). */
 /* Stride-1 depthwise conv (ks 3 | 5, pad ks/2, C % 32 == 0) on mma.sync with diagonal tap operands: same contract as
- * es3_dwconv_tiled_bf16 at stride 1, taps rounded to bf16 (nn.Conv2d(groups=C): efficientvit/nn/ops.py:39-80, repvit.py:84-122,
+ * es3_dwconv_bf16 at stride 1, taps rounded to bf16 (nn.Conv2d(groups=C): efficientvit/nn/ops.py:39-80, repvit.py:84-122,
  * tiny_vit.py:97-133; also the backward-data pass of those layers, on flipped taps). */
 int es3_dwconv_tc_bf16(const void* x, long long ldx, const float* w, const float* bias, void* out, long long ldo, int B, int H, int W, int C,
                        int ks, int act, void* stream);
@@ -485,12 +471,8 @@ int es3_round_taps_sum_bf16(const float* w, float* out, int KK, int C, void* str
 long long es3_dwconv_wgrad_win_ws_floats(int B, int H, int W, int C, int ks, int stride);
 int es3_dwconv_wgrad_win(const void* dz, const void* x, long long ldx, int B, int H, int W, int C, int ks, int stride, float* ws, float* dW,
                          void* stream);
-long long es3_dwconv_wgrad_tiled_ws_floats(int B, int H, int W, int C, int ks);
-int es3_dwconv_wgrad_tiled(const void* dz, const void* x, long long ldx, int B, int H, int W, int C, int ks, float* ws, float* dW,
-                           void* stream);
 /* SqueezeExcite backward (timm SqueezeExcite, repvit.py:23,136) in one launch each instead of per-image loops:
- * dgate[b][c] += sum_p dy x; dx = dy * gate[b][c] + add[b][c].  dy, x, dx: [B][HW][C] bf16.  Not on the default path yet
- * (no GPU parity run; ops.SE_BWD_BATCHED). */
+ * dgate[b][c] += sum_p dy x; dx = dy * gate[b][c] + add[b][c].  dy, x, dx: [B][HW][C] bf16. */
 long long es3_se_bwd_ws_floats(int B, int HW, int C);
 int es3_se_bwd_dgate(const void* dy, const void* x, int B, int HW, int C, float* ws, float* dgate, void* stream);
 int es3_se_bwd_apply(const void* dy, const float* gate, const float* add, void* dx, int B, int HW, int C, void* stream);
@@ -500,7 +482,7 @@ long long es3_stem_wgrad_ws_floats(int B, int H, int W, int Cout);
 int es3_stem_wgrad(const float* img, const void* dz, int B, int H, int W, int Cout, float* ws, float* dW, void* stream);
 /* Adjoint of es3_bilinear_nhwc_to_nchw: dout [B,C,Ho,Wo] fp32 NCHW -> din [B,Hi,Wi,C] bf16 NHWC. */
 int es3_bilinear_bwd(const float* dout, void* din, int B, int Hi, int Wi, int C, int Ho, int Wo, void* stream);
-/* Backward of es3_litemla_attn[_tc] (ReLU linear attention, head dim 16, ops.py:592-621): dy [B,HW,lddy] (head h at
+/* Backward of es3_litemla_attn_tc (ReLU linear attention, head dim 16, ops.py:592-621): dy [B,HW,lddy] (head h at
  * [16h, 16h+16)) -> dms [B,HW,lddms] in the q|k|v layout of ms.  kv_part: the partial KV sums the forward call left in its
  * workspace (nchunk_f = ceil(HW / 512)); dkv_ws: es3_litemla_bwd_ws_floats floats. */
 long long es3_litemla_bwd_ws_floats(int B, int HW, int heads2);

@@ -78,7 +78,7 @@ def _dw(x4, w, ks, stride):
     return F.conv2d(x4, w.t().reshape(C, 1, ks, ks), None, stride=stride, padding=ks // 2, groups=C)
 
 
-def dwconv(x, w, bias, ks, stride, act, out=None, force_simple=False, impl=None):
+def dwconv(x, w, bias, ks, stride, act, out=None, force_simple=False):
     v = _dw(_nchw(x), w.to(CD), ks, stride)
     if bias is not None:
         v = v + bias.view(1, -1, 1, 1)
@@ -116,7 +116,7 @@ def _lite_attn(ms, heads2, eps, dim=16):
     return y.reshape(B, HW, heads2 * dim), kv
 
 
-def litemla_attn(ms, heads2, eps=1e-15, tc=True, return_kv=False):
+def litemla_attn(ms, heads2, eps=1e-15, return_kv=False):
     B, H, W, ld = ms.shape
     y, kv = _lite_attn(ms.to(CD).reshape(B, H * W, ld), heads2, eps)
     att = y.reshape(B, H, W, heads2 * 16).to(BF)

@@ -159,8 +159,8 @@ def test_dwconv(cuda, ks, stride, H, W, C, simple):
                                                  (3, 9, 100, 256, "hswish", False), (5, 64, 64, 384, None, True)])
 def test_dwconv_tc(cuda, ks, H, W, C, act, sliced):
     """Tensor-core depthwise kernel (diagonal bf16 tap operands, two taps per m16n8k16, tap sums preserved by es3_round_taps_sum_bf16):
-    against torch at exactly the taps it computes with, against torch with the fp32 taps, and against the CUDA-core tiled kernel;
-    `sliced`: input and output are channel windows of wider NHWC buffers."""
+    against torch at exactly the taps it computes with and against torch with the fp32 taps; `sliced`: input and output are
+    channel windows of wider NHWC buffers."""
     from efficientsam3_b200 import ops
     g = torch.Generator().manual_seed(ks * 100 + C + H)
     B = 2
@@ -170,7 +170,7 @@ def test_dwconv_tc(cuda, ks, H, W, C, act, sliced):
     b = torch.randn(C, generator=g).to(cuda) if act != "relu" else None
     wt = w.reshape(C, ks * ks).t().contiguous()
     obuf = torch.zeros(B, H, W, 2 * C if sliced else C, device=cuda, dtype=torch.bfloat16)
-    out = ops.dwconv(x, wt, b, ks, 1, act, out=obuf[..., C:] if sliced else obuf, impl="tc")
+    out = ops.dwconv(x, wt, b, ks, 1, act, out=obuf[..., C:] if sliced else obuf)
     fn = {None: lambda t: t, "hswish": F.hardswish, "gelu": F.gelu, "relu": F.relu}[act]
     taps = ops.round_taps_sum_bf16(wt)                                           # [ks*ks, C]: what the kernel multiplies with
     assert torch.equal(taps, taps.to(torch.bfloat16).float())                   # bf16-representable ...
@@ -182,8 +182,6 @@ def test_dwconv_tc(cuda, ks, H, W, C, act, sliced):
     _close(out, ref_taps, 4e-3, "dwconv_tc vs torch at the kernel's taps")
     ref = fn(F.conv2d(x.float().permute(0, 3, 1, 2), w, b, stride=1, padding=ks // 2, groups=C)).permute(0, 2, 3, 1)
     _close(out, ref, 8e-3, "dwconv_tc vs torch (fp32 taps)")
-    tiled = ops.dwconv(x, wt, b, ks, 1, act, impl="tiled")
-    _close(out, tiled.float(), 1e-2, "dwconv_tc vs tiled")
     if sliced:
         assert torch.count_nonzero(obuf[..., :C]) == 0       # the neighbouring channel window is untouched
 
@@ -250,10 +248,9 @@ def test_layout_roundtrip(cuda):
     assert torch.equal(z, x.to(torch.bfloat16).float())
 
 
-@pytest.mark.parametrize("simple", [False, True, "tc", "dwpw"])
 @pytest.mark.parametrize("H,W,heads,B", [(32, 32, 16, 2), (63, 63, 8, 1), (64, 64, 8, 2), (5, 7, 2, 3)])
-def test_litemla(cuda, H, W, heads, B, simple):
-    """aggreg + ReLU linear attention vs the textbook formulation (efficientvit/nn/ops.py:584-621)."""
+def test_litemla(cuda, H, W, heads, B):
+    """aggreg + ReLU linear attention (the tensor-core kernels) vs the textbook formulation (efficientvit/nn/ops.py:584-621)."""
     from efficientsam3_b200 import ops
     dim = 16
     td = heads * dim
@@ -265,19 +262,12 @@ def test_litemla(cuda, H, W, heads, B, simple):
     ms = torch.zeros(B, H, W, 2 * C3, device=cuda, dtype=torch.bfloat16)
     ms[..., :C3] = qkv
     wdw_t, wpw_t = wdw.reshape(C3, 25).t().contiguous(), wpw.reshape(C3, 16).contiguous()
-    if simple == "tc":
-        ops.litemla_aggreg_tc(ms, ops.litemla_wcomb(wdw_t, wpw_t), C3)
-    elif simple == "dwpw":
-        ops.litemla_aggreg_dwpw(ms, *ops.litemla_dwpw_weights(wdw_t, wpw_t), C3)
-    else:
-        ops.litemla_aggreg(ms, wdw_t, wpw_t, C3, force_simple=simple)
+    ops.litemla_aggreg_dwpw(ms, *ops.litemla_dwpw_weights(wdw_t, wpw_t), C3)
     x = qkv.float().permute(0, 3, 1, 2)
-    dw = F.conv2d(x, wdw, padding=2, groups=C3)
-    if simple != "tc":      # the FMA / dwpw kernels round the depthwise output to bf16; the tc kernel folds the weights
-        dw = dw.to(torch.bfloat16).float()
+    dw = F.conv2d(x, wdw, padding=2, groups=C3).to(torch.bfloat16).float()     # the kernel rounds the depthwise output to bf16
     agg = F.conv2d(dw, wpw, groups=3 * heads)
     _close(ms[..., C3:], agg.permute(0, 2, 3, 1), 1e-2, "aggreg")
-    att = ops.litemla_attn(ms, 2 * heads, tc=(simple in ("tc", "dwpw")))
+    att = ops.litemla_attn(ms, 2 * heads)
     full = ms.float().permute(0, 3, 1, 2).reshape(B, -1, 3 * dim, H * W)
     q, k, v = F.relu(full[:, :, :dim]), F.relu(full[:, :, dim:2 * dim]), full[:, :, 2 * dim:]
     v = F.pad(v, (0, 0, 0, 1), value=1.0)

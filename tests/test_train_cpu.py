@@ -222,13 +222,12 @@ def test_repvit_padded_patch_embed_exact(monkeypatch, name):
     assert (num / den) ** 0.5 < 2e-5, (num / den) ** 0.5
 
 
-@pytest.mark.parametrize("bn_train,exact,batched_se", [(True, True, False), (False, True, False), (False, False, False), (True, True, True)])
-def test_repvit_train_graph_matches_oracle_autograd(monkeypatch, bn_train, exact, batched_se):
+@pytest.mark.parametrize("bn_train,exact", [(True, True), (False, True), (False, False)])
+def test_repvit_train_graph_matches_oracle_autograd(monkeypatch, bn_train, exact):
     """RepViT-M1.1 training graph (un-fused RepVGGDW with batch-statistics BN, SqueezeExcite, stride-2 patch-embed conv through
     the 2x2 phase decomposition) vs autograd of the oracle; exact = fp64 emulation (logic check), else bf16 storage (frozen BN)."""
     from efficientsam3_b200 import ops
     emu_ops.install(monkeypatch)
-    monkeypatch.setattr(ops, "SE_BWD_BATCHED", batched_se)          # the one-launch SqueezeExcite backward vs the per-image loops
     if exact:
         monkeypatch.setattr(emu_ops, "BF", torch.float64)
         monkeypatch.setattr(emu_ops, "CD", torch.float64)

@@ -516,19 +516,6 @@ def test_repvit_training_step_matches_oracle_autograd(cuda, bn_train):
     assert rel_out < tol_out and rel_all < tol_all, (rel_out, rel_all)
 
 
-@pytest.mark.parametrize("B,H,W,C,ks", [(2, 16, 16, 32, 3), (1, 9, 11, 96, 5), (2, 64, 64, 384, 5), (2, 40, 37, 512, 3), (1, 7, 5, 64, 5)])
-def test_dwconv_wgrad_tiled(cuda, B, H, W, C, ks):
-    from efficientsam3_b200 import ops
-    g = _g(B * H + C + ks + 1)
-    ms = _bf(torch.randn(B, H, W, 2 * C, generator=g))
-    dz = _bf(torch.randn(B, H, W, C, generator=g))
-    ref = torch.full((C, 1, ks, ks), 0.125)
-    E.dwconv_wgrad(dz, ms[..., :C], ref, ks, 1)
-    got = torch.full((C, 1, ks, ks), 0.125, device=cuda)
-    ops.dwconv_wgrad(dz.to(cuda), ms.to(cuda)[..., :C], got, ks, 1, impl="tiled")
-    _close(got, ref, 2e-3, "dwconv_wgrad tiled")
-
-
 @pytest.mark.parametrize("B,H,W,C,ks,stride", [(2, 16, 16, 32, 3, 1), (1, 9, 11, 96, 5, 1), (2, 64, 64, 384, 5, 1), (2, 40, 37, 512, 3, 1),
                                                (1, 7, 5, 64, 5, 1), (2, 64, 64, 64, 3, 2), (1, 37, 51, 128, 3, 2), (3, 18, 70, 32, 3, 2),
                                                (1, 33, 33, 64, 5, 2), (2, 8, 100, 96, 3, 1)])

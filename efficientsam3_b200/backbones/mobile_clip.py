@@ -25,7 +25,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops, sync_bn
-from ..nn_utils import NativePlanMixin, bn_scale_bias, cached_pack
+from ..nn_utils import NativePlanMixin, StagedGraphMixin, bn_scale_bias, cached_pack
 
 
 # ----------------------------------------------------------------------------------------------- parameter containers
@@ -346,7 +346,7 @@ def host_ids(ids: torch.Tensor, vocab: int) -> torch.Tensor:
     return h
 
 
-class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
+class MobileCLIPTextTransformer(nn.Module, NativePlanMixin, StagedGraphMixin):
     def __init__(self, cfg: dict, projection_dim: int, skip_embeddings: bool = False, *args, **kwargs) -> None:
         super().__init__()
         if skip_embeddings:
@@ -424,11 +424,14 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
         return self._embed(ids)
 
     def _embed(self, ids):
-        dev = next(self.parameters()).device
         h = host_ids(ids, self.vocab_size)
+        return self._embed_ids(h.to(next(self.parameters()).device, non_blocking=True))
+
+    def _embed_ids(self, ids):
+        """The embedding of ids [B, L] int64 already on the device (validated on the host) -> fp32 [B, L, C]."""
         p = self._plan()
-        B, L = h.shape
-        x, _ = ops.text_embed(h.to(dev, non_blocking=True), p["table"], self._pos(p, L, dev))
+        B, L = ids.shape
+        x, _ = ops.text_embed(ids, p["table"], self._pos(p, L, ids.device))
         return x.view(B, L, self.model_dim)
 
     def forward_embedding(self, text_tokens: torch.Tensor) -> torch.Tensor:
@@ -440,9 +443,12 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
         check_native(self, "MobileCLIPTextTransformer", self.training)
         return self._encode(x)
 
-    def _encode(self, x):
+    def _check_embeddings(self, x):
         if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[2] == self.model_dim):
             raise ValueError(f"expected CUDA fp32 embeddings [B, L, {self.model_dim}]; the native path has no CPU fallback")
+
+    def _encode(self, x):
+        self._check_embeddings(x)
         B, L, C = x.shape
         p = self._plan()
         bn_blocks = list(self.transformer) if self.batch_stat_active() else None
@@ -453,29 +459,55 @@ class MobileCLIPTextTransformer(nn.Module, NativePlanMixin):
         return yf, yb
 
     def encode_text(self, text, key_padding_mask=None, return_all_tokens=False, input_is_embeddings=False, *args, **kwargs):
+        return self._encode_text(text, key_padding_mask, return_all_tokens, input_is_embeddings, self._graphs is not None)
+
+    @torch.no_grad()
+    def _encode_text(self, text, key_padding_mask, return_all_tokens, input_is_embeddings, graphed):
         if key_padding_mask is not None:
             raise NotImplementedError("MobileCLIPTextTransformer: key_padding_mask is not supported on the native path (no "
                                       "caller passes one: TextStudentEncoder attends over padding tokens)")
-        check_native(self, "MobileCLIPTextTransformer", self.training)
-        ids = None
+        dev = check_native(self, "MobileCLIPTextTransformer", self.training)
+        # on the host: the ids validated and the pooled rows built (EOT token = argmax of the ids or, for embeddings, the last
+        # token, mobile_clip.py:873-882); _encode_on_device runs on device copies of them
         if input_is_embeddings:
-            emb = text
+            self._check_embeddings(text)
+            B, L, _ = text.shape
+            host, dev_in, eot = [], [text], L - 1
         else:
             ids = host_ids(text, self.vocab_size)
-            emb = self._embed(ids)
+            B, L = ids.shape
+            host, dev_in, eot = [ids], [], ids.argmax(dim=-1)
+        if not return_all_tokens:
+            host.append(torch.arange(B) * L + eot)
+
+        def run(*inputs):
+            return self._encode_on_device(inputs, input_is_embeddings, return_all_tokens)
+        if graphed and not self.batch_stat_active():
+            key = (B, L, "embeddings" if input_is_embeddings else "ids", bool(return_all_tokens), dev)
+            return self._graphed(key, host, dev_in, run)
+        return run(*(h.to(dev, non_blocking=True) for h in host), *dev_in)
+
+    def _encode_on_device(self, inputs, input_is_embeddings, return_all_tokens):
+        """inputs: (ids [B, L] | embeddings [B, L, C], then the pooled rows [B] unless return_all_tokens), all on the device ->
+        fp32 [B, L, C] (return_all_tokens) or the pooled projection fp32 [B, projection_dim]."""
+        if input_is_embeddings:
+            emb, rows = inputs[-1], (None if return_all_tokens else inputs[0])
+        else:
+            emb, rows = self._embed_ids(inputs[0]), (None if return_all_tokens else inputs[1])
         B, L, C = emb.shape
         yf, yb = self._encode(emb)
         if return_all_tokens:
             return yf.view(B, L, C)
-        # pooled: EOT token (argmax of the ids) or, for embeddings, the last token (mobile_clip.py:873-882)
-        rows = torch.arange(B) * L + (ids.argmax(dim=-1) if ids is not None else L - 1)
-        pooled = yb.index_select(0, rows.to(yb.device)).contiguous()
-        with torch.no_grad():
-            return ops.gemm(pooled, self._plan()["proj"], out_dtype=torch.float32)
+        pooled = yb.index_select(0, rows).contiguous()
+        return ops.gemm(pooled, self._plan()["proj"], out_dtype=torch.float32)
 
     def forward(self, text_tokens, key_padding_mask=None, return_all_tokens=False, input_is_embeddings=False, *args, **kwargs):
         return self.encode_text(text_tokens, key_padding_mask=key_padding_mask, return_all_tokens=return_all_tokens,
                                 input_is_embeddings=input_is_embeddings)
+
+    def forward_uncaptured(self, text_tokens, key_padding_mask=None, return_all_tokens=False, input_is_embeddings=False):
+        """forward() launched kernel by kernel, whether or not CUDA graphs are enabled."""
+        return self._encode_text(text_tokens, key_padding_mask, return_all_tokens, input_is_embeddings, False)
 
 
 # ----------------------------------------------------------------------------------------------- training graph (base trunk)

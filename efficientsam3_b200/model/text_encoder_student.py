@@ -13,6 +13,8 @@ it gets no gradient, so optimisers skip it (build stage1.optim.FlatAdamW with ex
 A train-mode module under torch.no_grad() runs the eval path: the base students have no train-time behaviour besides gradients.
 MobileCLIP-S0 after enable_batch_stat_bn() with its BatchNorms in train mode normalises with batch statistics instead, with grad
 or under torch.no_grad(), and updates the running buffers on every forward (RepMixerBatchStatUnit).
+enable_cuda_graphs() replays the eval forward from CUDA graphs (nn_utils.StagedGraphMixin); the training and batch-statistics
+paths above never are.
 """
 from __future__ import annotations
 
@@ -21,7 +23,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..backbones.mobile_clip import MobileCLIPTextTransformer, TextStudentTrainGraph, check_native, check_trainable, host_ids
-from ..nn_utils import NativePlanMixin
+from ..nn_utils import NativePlanMixin, StagedGraphMixin
 from .tokenizer_ve import SimpleTokenizer
 
 
@@ -29,7 +31,7 @@ def _lin(linear: nn.Linear):
     return linear.weight.detach().to(torch.bfloat16).contiguous(), linear.bias.detach().float().contiguous()
 
 
-class TextStudentEncoder(nn.Module, NativePlanMixin):
+class TextStudentEncoder(nn.Module, NativePlanMixin, StagedGraphMixin):
     def __init__(self, cfg, context_length, output_dim, bpe_path=None):
         super().__init__()
         self.context_length = context_length
@@ -60,6 +62,13 @@ class TextStudentEncoder(nn.Module, NativePlanMixin):
     supports_direct_grads = True
 
     def forward(self, text, input_boxes=None, device=None):
+        return self._forward(text, self._graphs is not None)
+
+    def forward_uncaptured(self, text, input_boxes=None, device=None):
+        """forward() launched kernel by kernel, whether or not CUDA graphs are enabled."""
+        return self._forward(text, False)
+
+    def _forward(self, text, graphed):
         if self.training:
             dev = check_trainable(self, self.encoder, "TextStudentEncoder")
             if torch.is_grad_enabled():
@@ -67,7 +76,7 @@ class TextStudentEncoder(nn.Module, NativePlanMixin):
         else:
             dev = check_native(self, "TextStudentEncoder", self.training)
         with torch.no_grad():
-            return self._forward_eval(text, dev)
+            return self._forward_eval(text, dev, graphed)
 
     def enable_batch_stat_bn(self, enabled: bool = True):
         """Opt in to batch-statistics BatchNorm in MobileCLIP-S0's RepMixerBlocks: with every such BN in train mode, each forward
@@ -84,16 +93,24 @@ class TextStudentEncoder(nn.Module, NativePlanMixin):
             raise ValueError("TextStudentEncoder: batch-statistics BatchNorm expects more than 1 value per channel when training "
                              f"(B*L = {ids.shape[0] * ids.shape[1]})")
 
-    def _forward_eval(self, text, dev):
+    def _forward_eval(self, text, dev, graphed):
         ids = self.tokenize(text)
         self._check_batch(ids)
         mask = (ids != 0).bool().ne(1)                       # True = padding (text_encoder_student.py:56)
         B, L = ids.shape
-        emb = self.encoder._embed(ids)                       # [B, L, dim]: also the trunk's input stream
+        if graphed and not self.encoder.batch_stat_active():   # batch statistics update the running buffers: never replayed
+            memory, emb = self._graphed((B, L, "ids", True, dev), [ids], [], self._forward_ids)
+        else:
+            memory, emb = self._forward_ids(ids.to(dev, non_blocking=True))
+        return mask.to(dev), memory.transpose(0, 1), emb.transpose(0, 1)
+
+    def _forward_ids(self, ids):
+        """ids [B, L] on the device -> (memory fp32 [B, L, output_dim], input_embeds fp32 [B, L, dim])."""
+        B, L = ids.shape
+        emb = self.encoder._embed_ids(ids)                   # [B, L, dim]: also the trunk's input stream
         _, yb = self.encoder._encode(emb)
         w, b = self._plan()["proj"]
-        memory = ops.gemm(yb, w, bias=b, out_dtype=torch.float32).view(B, L, -1)
-        return mask.to(dev), memory.transpose(0, 1), emb.transpose(0, 1)
+        return ops.gemm(yb, w, bias=b, out_dtype=torch.float32).view(B, L, -1), emb
 
     def trainable_parameters(self):
         """The parameters the training graph produces gradients for (all but UNUSED_PARAMETERS)."""

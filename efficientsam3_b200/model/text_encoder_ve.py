@@ -21,7 +21,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..backbones.mobile_clip import check_native, host_ids
-from ..nn_utils import NativePlanMixin
+from ..nn_utils import NativePlanMixin, StagedGraphMixin
 
 
 def _f32(t):
@@ -90,7 +90,7 @@ class TextTransformer(nn.Module):
         nn.init.normal_(self.text_projection, std=width ** -0.5)
 
 
-class VETextEncoder(nn.Module, NativePlanMixin):
+class VETextEncoder(nn.Module, NativePlanMixin, StagedGraphMixin):
     def __init__(self, d_model: int, tokenizer: Callable, width: int = 1024, heads: int = 16, layers: int = 24,
                  context_length: int = 32, vocab_size: int = 49408, use_ln_post: bool = True, compile_mode: Optional[str] = None,
                  use_act_checkpoint: bool = True):
@@ -109,16 +109,22 @@ class VETextEncoder(nn.Module, NativePlanMixin):
                     ln=(_f32(e.ln_final.weight), _f32(e.ln_final.bias), e.ln_final.eps),
                     resizer=(self.resizer.weight.detach().to(torch.bfloat16).contiguous(), _f32(self.resizer.bias)))
 
-    @torch.no_grad()
     def forward(self, text: Union[List[str], Tuple[torch.Tensor, torch.Tensor, dict]], input_boxes: Optional[List] = None,
                 device: torch.device = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        return self._forward(text, input_boxes, self._graphs is not None)
+
+    def forward_uncaptured(self, text, input_boxes=None, device=None):
+        """forward() launched kernel by kernel, whether or not CUDA graphs are enabled."""
+        return self._forward(text, input_boxes, False)
+
+    @torch.no_grad()
+    def _forward(self, text, input_boxes, graphed):
         if not (torch.is_tensor(text) or isinstance(text[0], str)):
             # already encoded (text_encoder_ve.py:315-321)
             assert input_boxes is None or len(input_boxes) == 0, "Can't replace boxes in text if it's already encoded"
             mask, memory, tokenized = text
             return mask, memory, tokenized["inputs_embeds"].transpose(0, 1)
         assert input_boxes is None or len(input_boxes) == 0, "not supported"
-        from ..backbones.mobile_clip import run_layers
         dev = check_native(self, "VETextEncoder", self.training)
         if torch.is_tensor(text):
             ids = host_ids(text, self.encoder.vocab_size)
@@ -130,12 +136,22 @@ class VETextEncoder(nn.Module, NativePlanMixin):
         B, L = ids.shape
         if L > self.encoder.num_pos:
             raise ValueError(f"VETextEncoder: {L} tokens exceed the {self.encoder.num_pos}-entry positional table")
+        if graphed:
+            memory, emb = self._graphed((B, L, "ids", True, dev), [ids], [], self._forward_ids)
+        else:
+            memory, emb = self._forward_ids(ids.to(dev, non_blocking=True))
+        mask = (ids != 0).bool().ne(1)
+        return mask.to(dev), memory.transpose(0, 1), emb.transpose(0, 1)
+
+    def _forward_ids(self, ids):
+        """ids [B, L] on the device -> (memory fp32 [B, L, d_model], inputs_embeds fp32 [B, L, width])."""
+        from ..backbones.mobile_clip import run_layers
+        B, L = ids.shape
         p = self._plan()
         C = self.encoder.width
-        x, emb = ops.text_embed(ids.to(dev, non_blocking=True), p["table"], p["pos"][:L], emb="plain")
+        x, emb = ops.text_embed(ids, p["table"], p["pos"][:L], emb="plain")
         xs = run_layers(p["layers"], x, B, L, causal=self.encoder.causal)
         yb, _ = ops.layernorm(xs, *p["ln"])
         w, b = p["resizer"]
         memory = ops.gemm(yb, w, bias=b, out_dtype=torch.float32).view(B, L, -1)
-        mask = (ids != 0).bool().ne(1)
-        return mask.to(dev), memory.transpose(0, 1), emb.view(B, L, C).transpose(0, 1)
+        return memory, emb.view(B, L, C)

@@ -144,3 +144,84 @@ class NativePlanMixin:
             raise NotImplementedError(
                 f"{what}: this module's native sm_90a path is eval-mode only (train-mode forward / backward exist for the "
                 "stage-1 student encoders: ImageStudentEncoder; see DESIGN.md).  Call .eval() first.")
+
+
+class StagedGraphMixin:
+    """CUDA-graph replay of an eval forward whose inputs arrive from the host (the text encoders: token ids validated on the
+    host, EOT row indices).  One graph per key (shapes, input kind, device): its inputs are static device buffers, refilled
+    before each replay -- host int64 tensors through a pinned staging buffer (one asynchronous copy), CUDA tensors device to
+    device -- and its outputs are the graph's own buffers, overwritten by the next replay with the same key.
+
+    A graph reads the packed weights of every NativePlanMixin below the module by address, so it is captured again when
+    a parameter or buffer moves (params_fingerprint: optimiser steps through torch, load_state_dict, a replaced Parameter, a move
+    to another device) or a plan was invalidated (FlatAdamW's step and the batch-statistics BatchNorm reset `_plan_key`).  The
+    entry keeps the plans it was captured with alive, so a stale graph never reads freed memory.  At most `max_graphs` graphs are
+    kept; the oldest capture is evicted first."""
+
+    _graphs = None
+    graph_launches_per_step = 0     # kernels of the graph replayed last (es3 launches, as ops.launch_count counts them)
+
+    def enable_cuda_graphs(self, enabled: bool = True, max_graphs: int = 4):
+        """Replay the eval forward from CUDA graphs (off by default).  Returns self."""
+        if max_graphs < 1:
+            raise ValueError(f"max_graphs must be >= 1, got {max_graphs}")
+        self._graphs = {} if enabled else None
+        self._graph_max = max_graphs
+        return self
+
+    def _graphed(self, key, host, dev_in, fn):
+        """fn(*static inputs) -> outputs, replayed from the graph of `key` (its last element is the device).  host: CPU int64
+        tensors, dev_in: CUDA tensors; fn receives device buffers of the same shapes, host ones first."""
+        dev = key[-1]
+        fp = params_fingerprint(self)
+        ent = self._graphs.get(key)
+        with torch.cuda.device(dev):
+            if ent is None or ent["fp"] != fp or any(getattr(m, "_plan_key", None) is not k for m, k, _ in ent["plans"]):
+                del ent                             # release the stale graph's memory before capturing its successor
+                self._graphs.pop(key, None)
+                ent = self._capture(dev, host, dev_in, fn, fp)
+                while len(self._graphs) >= self._graph_max:
+                    self._graphs.pop(next(iter(self._graphs)))
+                self._graphs[key] = ent
+            else:
+                self._stage(ent, host, dev_in)
+            ent["graph"].replay()
+        self.graph_launches_per_step = ent["launches"]
+        return ent["out"]
+
+    @staticmethod
+    def _stage(ent, host, dev_in):
+        if host:
+            ent["copied"].synchronize()             # the previous replay's copy out of the pinned buffer has been read
+            o = 0
+            for h in host:
+                ent["pinned"][o:o + h.numel()].copy_(h.reshape(-1))
+                o += h.numel()
+            ent["flat"].copy_(ent["pinned"], non_blocking=True)
+            ent["copied"].record()
+        for s, t in zip(ent["dev_in"], dev_in):
+            s.copy_(t)
+
+    def _capture(self, dev, host, dev_in, fn, fp):
+        from . import ops
+        n = sum(h.numel() for h in host)
+        ent = dict(fp=fp, pinned=torch.empty(n, dtype=torch.int64, pin_memory=True),
+                   flat=torch.empty(n, dtype=torch.int64, device=dev), copied=torch.cuda.Event(),
+                   dev_in=[torch.empty(t.shape, dtype=t.dtype, device=t.device) for t in dev_in])
+        static, o = [], 0
+        for h in host:
+            static.append(ent["flat"][o:o + h.numel()].view(h.shape))
+            o += h.numel()
+        static += ent["dev_in"]
+        self._stage(ent, host, dev_in)
+        fn(*static)                                 # un-captured pass: packs weights, builds positional tables, configures kernels
+        torch.cuda.synchronize(dev)
+        graph = torch.cuda.CUDAGraph()
+        n0 = ops.launch_count
+        # thread_local: another thread may wait on CUDA events meanwhile (the embedding dump's writer thread does)
+        with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+            out = fn(*static)
+        ent.update(graph=graph, out=out, launches=ops.launch_count - n0,
+                   plans=[(m, getattr(m, "_plan_key", None), getattr(m, "_plan_cache", None)) for m in self.modules()
+                          if isinstance(m, NativePlanMixin)])
+        return ent

@@ -268,6 +268,22 @@ class SAM3TextTeacherEncoder(nn.Module):
         _, memory, _ = self.sam3.backbone.language_backbone(text, input_boxes=None, device=device)
         return memory[:self.context_length] if memory.shape[0] > self.context_length else memory
 
+    # CUDA-graph replay of the eval forward: the VETextEncoder's (StagedGraphMixin), which this module calls
+    def enable_cuda_graphs(self, enabled: bool = True, max_graphs: int = 4):
+        """Replay the forward from CUDA graphs, one per (batch, context length); the returned memory is the graph's output buffer,
+        overwritten by the next replay of the same shape.  Returns self."""
+        self.sam3.backbone.language_backbone.enable_cuda_graphs(enabled, max_graphs)
+        return self
+
+    @property
+    def graph_launches_per_step(self):
+        return self.sam3.backbone.language_backbone.graph_launches_per_step
+
+    @torch.no_grad()
+    def forward_uncaptured(self, text, device=None):
+        _, memory, _ = self.sam3.backbone.language_backbone.forward_uncaptured(text, input_boxes=None, device=device)
+        return memory[:self.context_length] if memory.shape[0] > self.context_length else memory
+
 
 def build_image_teacher_model(config):
     """stage1/model.py:168-175.  `config.MODEL.RESUME` (optional) is a reference SAM3 checkpoint."""

@@ -122,6 +122,23 @@ def _chk(t: torch.Tensor, dtype, name: str):
     return t
 
 
+_BF16_F32 = (torch.bfloat16, torch.float32)
+
+
+def _chk_any(t: torch.Tensor, dtypes, name: str):
+    """`t` is a CUDA tensor of one of `dtypes` (the kernels take a 0/1 fp32 flag: any other dtype would be read with the wrong
+    element size or bit layout)."""
+    if not t.is_cuda:
+        raise _lib.Es3Error(f"{name}: expected a CUDA tensor (the native path has no CPU fallback)")
+    if t.dtype not in dtypes:
+        raise _lib.Es3Error(f"{name}: expected one of {dtypes}, got {t.dtype}")
+    return t
+
+
+def _chk_opt(t, dtype, name: str):
+    return t if t is None else _chk(t, dtype, name)
+
+
 def _ptr(t):
     return 0 if t is None else t.data_ptr()
 
@@ -139,6 +156,7 @@ def gemm(a, w, *, scale=None, bias=None, act=None, residual=None, out=None, out_
     w: [N,K] bf16, scale/bias fp32 [N]; residual bf16 or fp32 [M,N].
     rope = (table[P,32,2] fp32, rope_cols, H, W, win): rotate columns [0, rope_cols) (see es3_gemm_bf16_ex)."""
     _chk(a, torch.bfloat16, "a"); _chk(w, torch.bfloat16, "w")
+    _chk_opt(scale, torch.float32, "scale"); _chk_opt(bias, torch.float32, "bias")
     _ensure_init(a)
     assert a.dim() == 2 and w.dim() == 2 and a.stride(1) == 1 and w.stride(1) == 1
     M, K = a.shape
@@ -146,10 +164,11 @@ def gemm(a, w, *, scale=None, bias=None, act=None, residual=None, out=None, out_
     assert w.shape[1] == K, (a.shape, w.shape)
     if out is None:
         out = torch.empty((M, N), device=a.device, dtype=out_dtype)
+    _chk_any(out, _BF16_F32, "out")
     assert out.stride(1) == 1 and out.shape == (M, N)
     res_f32 = 0
     if residual is not None:
-        assert residual.is_cuda and residual.dtype in (torch.bfloat16, torch.float32)
+        _chk_any(residual, _BF16_F32, "residual")
         assert residual.stride(1) == 1 and residual.shape == (M, N)
         res_f32 = int(residual.dtype == torch.float32)
     if (PW_SMALL and K <= 64 and N <= 64 and scale is None and bias is None and act in (None, "none") and rope is None
@@ -174,12 +193,18 @@ def gemm(a, w, *, scale=None, bias=None, act=None, residual=None, out=None, out_
 
 
 def gemm_simt(a, w, *, scale=None, bias=None, act=None, residual=None, out=None, out_dtype=torch.bfloat16):
+    """The CUDA-core GEMM (gemm_simt.cu), same epilogue as `gemm`; a, w, out and residual each bf16 or fp32."""
+    _chk_any(a, _BF16_F32, "a"); _chk_any(w, _BF16_F32, "w")
+    _chk_opt(scale, torch.float32, "scale"); _chk_opt(bias, torch.float32, "bias")
+    if residual is not None:
+        _chk_any(residual, _BF16_F32, "residual")
     _ensure_init(a)
     assert a.dim() == 2 and w.dim() == 2 and a.stride(1) == 1 and w.stride(1) == 1
     M, K = a.shape
     N = w.shape[0]
     if out is None:
         out = torch.empty((M, N), device=a.device, dtype=out_dtype)
+    _chk_any(out, _BF16_F32, "out")
     res_f32 = int(residual is not None and residual.dtype == torch.float32)
     _call("es3_gemm_simt", "gemm_simt", _nb(a, w, out, residual), 2 * M * N * K, a.data_ptr(), a.stride(0), int(a.dtype == torch.float32), w.data_ptr(), w.stride(0),
               int(w.dtype == torch.float32), out.data_ptr(), out.stride(0), int(out.dtype == torch.float32), M, N, K,
@@ -189,13 +214,22 @@ def gemm_simt(a, w, *, scale=None, bias=None, act=None, residual=None, out=None,
 
 
 def conv3x3(x, w9, *, scale=None, bias=None, act=None, residual=None, out_dtype=torch.bfloat16, bn_hint=0):
-    """x: [B,H,W,C] bf16 NHWC contiguous; w9: [N, 9*C] bf16 (tap-major k)."""
+    """x: [B,H,W,C] bf16 NHWC contiguous; w9: [N, 9*C] bf16 (tap-major k); residual: bf16 [B,H,W,N] contiguous (the kernel
+    reads it with row pitch N and has no fp32-residual flag)."""
     _chk(x, torch.bfloat16, "x"); _chk(w9, torch.bfloat16, "w9")
+    _chk_opt(scale, torch.float32, "scale"); _chk_opt(bias, torch.float32, "bias")
+    if out_dtype not in _BF16_F32:
+        raise _lib.Es3Error(f"conv3x3: out_dtype must be bf16 or fp32, got {out_dtype}")
     _ensure_init(x)
     assert x.is_contiguous() and w9.is_contiguous()
     B, H, W, Cc = x.shape
     N = w9.shape[0]
     assert w9.shape[1] == 9 * Cc
+    if residual is not None:
+        _chk(residual, torch.bfloat16, "residual")
+        if not residual.is_contiguous() or residual.shape != (B, H, W, N):
+            raise _lib.Es3Error(f"conv3x3: residual must be contiguous [{B},{H},{W},{N}], got {tuple(residual.shape)} "
+                                f"with strides {residual.stride()}")
     out = torch.empty((B, H, W, N), device=x.device, dtype=out_dtype)
     _call("es3_conv3x3_bf16", f"conv3x3_tc[C={Cc},N={N}]", _nb(x, w9, out, residual), 2 * B * H * W * N * 9 * Cc,
           x.data_ptr(), w9.data_ptr(), out.data_ptr(), int(out_dtype == torch.float32),
@@ -921,7 +955,9 @@ def cast_f32_to_f16(x, out=None):
 # ------------------------------------------------------------------------------------ SAM heads
 def convt2x2(x, wt, bias4=None, act=None, residual=None, out_dtype=torch.bfloat16, act_after_res=False):
     """ConvTranspose2d(k=2,s=2) on NHWC: x [B,H,W,Cin] bf16, wt [4*Cout, Cin] bf16 -> [B,2H,2W,Cout]."""
-    _chk(x, torch.bfloat16, "x"); _chk(wt, torch.bfloat16, "wt")
+    _chk(x, torch.bfloat16, "x"); _chk(wt, torch.bfloat16, "wt"); _chk_opt(bias4, torch.float32, "bias4")
+    if out_dtype not in _BF16_F32:
+        raise _lib.Es3Error(f"convt2x2: out_dtype must be bf16 or fp32, got {out_dtype}")
     _ensure_init(x)
     assert x.is_contiguous() and wt.is_contiguous()
     B, H, W, Cin = x.shape
@@ -929,6 +965,7 @@ def convt2x2(x, wt, bias4=None, act=None, residual=None, out_dtype=torch.bfloat1
     out = torch.empty((B, 2 * H, 2 * W, Cout), device=x.device, dtype=out_dtype)
     res_f32 = int(residual is not None and residual.dtype == torch.float32)
     if residual is not None:
+        _chk_any(residual, _BF16_F32, "residual")
         assert residual.is_contiguous() and residual.shape == out.shape
     _call("es3_convt2x2_bf16", f"convt2x2[{Cin}->{Cout}]", _nb(x, wt, out, residual), 2 * B * H * W * Cin * 4 * Cout,
           x.data_ptr(), wt.data_ptr(), out.data_ptr(), int(out_dtype == torch.float32), B, H, W, Cin, Cout, _ptr(bias4),

@@ -1,0 +1,579 @@
+"""The fused GEMM epilogue of gemm_tc.cu (1x1 convs, nn.Linear, the implicit-GEMM 3x3 conv, the 2x2 transposed conv) and the
+CUDA-core gemm_simt.cu, element by element against fp64.
+
+Operands are bf16-representable (A, W and bf16 residuals are rounded first), so the fp64 statement
+y = act(s * (A W^T) + b) (+ r), in the order the call asks for, is what the kernel would compute with exact arithmetic.  Every
+output element must lie within its own bound
+
+    |got - ref| <= L_act * (gamma_K * |s| * (|A| |W|^T) + 4u (|s acc| + |b| [+ |r| when act follows the residual]) + eps_act(x))
+                   + 4u |ref|        (+ 2^-8 |ref| for a bf16 output, the half-step of its rounding)
+
+with u = 2^-24, gamma_K = GAMMA * K * u (fp32 accumulation of K products), L_act the Lipschitz constant of the activation
+(1.5 hswish, 1.13 GELU, 0.25 sigmoid) and eps_act(x) the activation's own approximation error at its input x (the
+Abramowitz-Stegun erf of common.cuh's es3_gelu_fast, the MUFU exp of sigmoid).  A bound per element, rather than a fraction of
+the tensor's maximum, is what catches a wrong residual row or a missing scale on one 32-column chunk where the values are small.
+
+Output buffers are prefilled with NaN: every cell inside the output region must be written (a NaN fails the bound), and every cell
+outside it -- the rest of a wider buffer, or a tail past the end -- must keep its sentinel bits.  Strided operands are slices of
+NaN-padded buffers, so a read outside the slice also shows.
+
+GAMMA = 2 and the eps_act below were set from one run on an H100 80GB HBM3 (700 W power limit).  Measured maximum err/bound per
+section, fp32 outputs: (a) epilogue matrix 0.18, (c) act/residual order 0.021, (d) RoPE 0.0037, (e) conv3x3 0.019,
+(f) convt2x2 0.025, (g) gemm_simt 0.054, so the fp32 accumulation stays well inside 2 K u.  bf16 outputs: 0.87 ... 0.996 in
+every section (pw_small 0.995), because the half-step of the output rounding dominates their bound and is reached.
+(b) reaches 1.0 of its half-step tolerance by construction: the residual sits at a bf16 midpoint.
+"""
+import itertools
+import math
+import random
+import zlib
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+pytestmark = pytest.mark.gpu
+
+U = 2.0 ** -24
+GAMMA = 2.0                    # gamma_K = GAMMA * K * u
+L_ACT = {None: 1.0, "relu": 1.0, "hswish": 1.5, "gelu": 1.13, "sigmoid": 0.25}
+EPS_GELU = 3e-7                # es3_gelu_fast: 0.5 |x| * (1.5e-7 erf approximation + a few ulp of MUFU rcp / ex2), per |x|
+EPS_SIGMOID = 1e-6             # 1 / (1 + __expf(-x)): __expf is within (2 + 1.16 |x|) ulp; sigmoid' <= 1/4
+TAIL = 256                     # sentinel cells past the end of a flat output buffer
+_INT = {torch.bfloat16: torch.int16, torch.float32: torch.int32}
+_WORST: dict = {}              # section -> max err/bound over the run
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _report_worst():
+    yield
+    for k in sorted(_WORST):
+        print(f"\ngemm epilogue, section {k}: max err/bound = {_WORST[k]:.3g}", end="")
+
+
+def _pairwise(factors: dict, seed: int = 0) -> list:
+    """Rows of a strength-2 covering design: every value pair of every two factors appears in some row (greedy)."""
+    names = list(factors)
+    sizes = [len(factors[n]) for n in names]
+    nf = len(names)
+    todo = {(i, a, j, b) for i, j in itertools.combinations(range(nf), 2) for a in range(sizes[i]) for b in range(sizes[j])}
+    rng = random.Random(seed)
+    rows = []
+
+    def key(k, v, m, u):
+        return (k, v, m, u) if k < m else (m, u, k, v)
+
+    while todo:
+        i, a, j, b = min(todo)
+        row = {i: a, j: b}
+        for k in range(nf):
+            if k in row:
+                continue
+            gains = [sum(key(k, v, m, u) in todo for m, u in row.items()) for v in range(sizes[k])]
+            row[k] = rng.choice([v for v in range(sizes[k]) if gains[v] == max(gains)])
+        todo -= {(p, row[p], q, row[q]) for p, q in itertools.combinations(range(nf), 2)}
+        rows.append(tuple(factors[names[k]][row[k]] for k in range(nf)))
+    return rows
+
+
+def _bf(t):
+    return t.to(torch.bfloat16)
+
+
+def _gen(cuda, *key):
+    return torch.Generator(device=cuda).manual_seed(zlib.crc32(repr(key).encode()))
+
+
+def _act64(x, act):
+    if act is None:
+        return x
+    return {"relu": F.relu, "hswish": F.hardswish, "gelu": F.gelu, "sigmoid": torch.sigmoid}[act](x)
+
+
+def _eps_act(x, act):
+    if act == "gelu":
+        return EPS_GELU * x.abs()
+    if act == "sigmoid":
+        return EPS_SIGMOID * (1.0 + x.abs())
+    return 0.0
+
+
+def _expect(acc, absprod, K, act=None, scale=None, bias=None, res=None, after=False, out_bf16=False):
+    """fp64 reference and per-element bound (module docstring).  acc, absprod: fp64 A W^T and |A| |W|^T; scale / bias [N]
+    broadcast over the last dim; res in the output's layout."""
+    s = scale.double() if scale is not None else 1.0
+    sacc = acc * s
+    inner = GAMMA * K * U * absprod * (s.abs() if scale is not None else 1.0) + 4 * U * sacc.abs()
+    pre = sacc
+    if bias is not None:
+        pre = pre + bias.double()
+        inner = inner + 4 * U * bias.double().abs()
+    if res is None:
+        x = pre
+        ref = _act64(x, act)
+    elif after:
+        x = pre + res.double()
+        inner = inner + 4 * U * res.double().abs()
+        ref = _act64(x, act)
+    else:
+        x = pre
+        ref = _act64(x, act) + res.double()
+    bound = L_ACT[act] * (inner + _eps_act(x, act)) + 4 * U * ref.abs() + 2.0 ** -126
+    if out_bf16:
+        bound = bound * (1 + 2.0 ** -8) + 2.0 ** -8 * ref.abs()
+    return ref, bound
+
+
+def _check(section, got, ref, bound, what):
+    err = (got.double() - ref).abs()
+    bad = ~(err <= bound)                   # NaN (a cell never written) is outside any bound
+    nbad = int(bad.sum())
+    if nbad:
+        idx = tuple(bad.nonzero()[0].tolist())
+        raise AssertionError(f"{what}: {nbad} of {err.numel()} elements outside their bound ({int(torch.isnan(got).sum())} unwritten); "
+                             f"first at {idx}: got {got[idx].item():.6g}, ref {ref[idx].item():.6g}, bound {bound[idx].item():.3g}")
+    _WORST[section] = max(_WORST.get(section, 0.0), (err / bound).max().item())
+
+
+def _sentinel(dtype):
+    return torch.full((1,), float("nan"), dtype=dtype).view(_INT[dtype]).item()
+
+
+def _assert_untouched(buf, inside, what):
+    bits = buf.view(_INT[buf.dtype])[~inside]
+    changed = int((bits != _sentinel(buf.dtype)).sum())
+    assert changed == 0, f"{what}: {changed} cells outside the output region were written"
+
+
+def _flat_out(n, dtype, cuda):
+    """A NaN-filled flat buffer of n + TAIL cells; returns (buffer, inside-mask)."""
+    buf = torch.full((n + TAIL,), float("nan"), dtype=dtype, device=cuda)
+    inside = torch.zeros(n + TAIL, dtype=torch.bool, device=cuda)
+    inside[:n] = True
+    return buf, inside
+
+
+def _matrix_out(M, N, dtype, strided, cuda):
+    """(buffer, [M, N] view, inside-mask): `strided` puts the view at column 8 of a [M + 2, N + 24] buffer."""
+    if not strided:
+        buf, inside = _flat_out(M * N, dtype, cuda)
+        return buf, buf[:M * N].view(M, N), inside
+    buf = torch.full((M + 2, N + 24), float("nan"), dtype=dtype, device=cuda)
+    inside = torch.zeros(buf.shape, dtype=torch.bool, device=cuda)
+    inside[:M, 8:8 + N] = True
+    return buf, buf[:M, 8:8 + N], inside
+
+
+def _padded(t, strided):
+    """`t` itself, or the same values as a column-8 slice of a NaN-padded buffer 16 columns wider (row stride != width)."""
+    if not strided:
+        return t.contiguous()
+    big = torch.full((t.shape[0], t.shape[1] + 16), float("nan"), dtype=t.dtype, device=t.device)
+    big[:, 8:8 + t.shape[1]] = t
+    return big[:, 8:8 + t.shape[1]]
+
+
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _ptr(t):
+    return 0 if t is None else t.data_ptr()
+
+
+# ---------------------------------------------------------------------------------------------- (a) es3_gemm_bf16_ex epilogue
+GEMM_FACTORS = dict(
+    M=[1, 77, 127, 129, 231, 5184],
+    N=[8, 24, 48, 80, 96, 1024, 4736],
+    K=[8, 200, 1024],                  # one k-block / the TMA K tail / 16 k-blocks: both BN-128 stage counts
+    act=[None, "relu", "hswish", "gelu"],
+    after=[False, True],
+    scale=[False, True],
+    bias=[False, True],
+    res=[None, "bf16", "f32"],
+    out=["bf16", "f32"],
+    bn=[0, 32, 64, 128],
+    strided=[False, True],
+)
+GEMM_DESIGN = _pairwise(GEMM_FACTORS, seed=1)
+
+
+def _gemm_id(c):
+    M, N, K, act, after, sc, bi, res, out, bn, strided = c
+    return (f"M{M}-N{N}-K{K}-{act}-{'after' if after else 'before'}-{'s' if sc else ''}{'b' if bi else ''}-r{res}-{out}-bn{bn}"
+            f"{'-strided' if strided else ''}")
+
+
+def _gemm_case(cuda, M, N, K, act, after, has_s, has_b, res, out, bn, strided, seed=()):
+    from efficientsam3_b200 import ops
+    g = _gen(cuda, M, N, K, act, after, has_s, has_b, res, out, bn, strided, *seed)
+    a = _padded(_bf(torch.randn(M, K, device=cuda, generator=g)), strided)
+    w = _bf(torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K))
+    scale = (torch.rand(N, device=cuda, generator=g) + 0.5) * torch.randn(N, device=cuda, generator=g).sign() if has_s else None
+    bias = torch.randn(N, device=cuda, generator=g) if has_b else None
+    r = None
+    if res is not None:
+        r = 2 * torch.randn(M, N, device=cuda, generator=g)
+        r = _padded(_bf(r) if res == "bf16" else r, strided)
+    dt = torch.float32 if out == "f32" else torch.bfloat16
+    buf, o, inside = _matrix_out(M, N, dt, strided, cuda)
+    got = ops.gemm(a, w, scale=scale, bias=bias, act=act, residual=r, out=o, bn_hint=bn, act_after_res=after)
+    assert got.data_ptr() == o.data_ptr()
+    acc = a.double() @ w.double().t()
+    absprod = a.double().abs() @ w.double().abs().t()
+    ref, bound = _expect(acc, absprod, K, act, scale, bias, r, after, out_bf16=out == "bf16")
+    return buf, o, inside, ref, bound
+
+
+@pytest.mark.parametrize("M,N,K,act,after,has_s,has_b,res,out,bn,strided", GEMM_DESIGN, ids=[_gemm_id(c) for c in GEMM_DESIGN])
+def test_gemm_epilogue(cuda, monkeypatch, M, N, K, act, after, has_s, has_b, res, out, bn, strided):
+    """Pairwise cover of act x act-after-residual x scale x bias x residual dtype x out dtype x tile width x M x N (ragged 32-column
+    chunks at 8, 24, 48, 80) x K, contiguous and strided; always on the wgmma kernel."""
+    from efficientsam3_b200 import ops
+    monkeypatch.setattr(ops, "PW_SMALL", False)
+    buf, o, inside, ref, bound = _gemm_case(cuda, M, N, K, act, after, has_s, has_b, res, out, bn, strided)
+    what = _gemm_id((M, N, K, act, after, has_s, has_b, res, out, bn, strided))
+    _check(f"a/{out}", o, ref, bound, what)
+    _assert_untouched(buf, inside, what)
+
+
+@pytest.mark.parametrize("pw_small", [True, False])
+@pytest.mark.parametrize("M,N,K,res,strided", [(4099, 16, 16, "bf16", True), (231, 64, 32, None, False), (1, 32, 64, "bf16", False),
+                                               (129, 16, 64, None, True), (5184, 32, 16, "bf16", False)])
+def test_gemm_pw_small_route(cuda, monkeypatch, M, N, K, res, strided, pw_small):
+    """Plain narrow GEMMs (K, N <= 64, no scale / bias / act, bf16 out) on es3_pw_small_bf16 and, with the switch off, on wgmma."""
+    from efficientsam3_b200 import ops
+    monkeypatch.setattr(ops, "PW_SMALL", pw_small)
+    buf, o, inside, ref, bound = _gemm_case(cuda, M, N, K, None, False, False, False, res, "bf16", 0, strided)
+    what = f"pw_small={pw_small} {M}x{N}x{K} res={res} strided={strided}"
+    _check("pw_small", o, ref, bound, what)
+    _assert_untouched(buf, inside, what)
+
+
+# ---------------------------------------------------------------------------------------------- (b) the fp32 residual's precision
+@pytest.mark.parametrize("out", ["f32", "bf16"])
+@pytest.mark.parametrize("N", [96, 80])
+@pytest.mark.parametrize("bn", [32, 64, 128])
+def test_fp32_residual_keeps_precision(cuda, bn, N, out):
+    """|A W^T| ~ 1 on a residual near 4096, where bf16's step is 32.  fp32 out: the residual's fraction survives (|err| <= 1e-3).
+    bf16 out: the residual sits within 1 of 4112, the midpoint between two bf16 values, so a sum rounded once at the store is
+    within half a step (16) of the fp64 result, while a residual rounded to bf16 first lands on the far side.  N = 80 ends in a
+    ragged 16-column chunk."""
+    from efficientsam3_b200 import ops
+    M, K = 300, 256
+    g = _gen(cuda, "b", bn, N, out)
+    a = _bf(torch.randn(M, K, device=cuda, generator=g))
+    w = _bf(torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K))
+    u01 = torch.rand(M, N, device=cuda, generator=g)
+    r = 4096 + u01 if out == "f32" else 4112 + (2 * u01 - 1)
+    dt = torch.float32 if out == "f32" else torch.bfloat16
+    buf, o, inside = _matrix_out(M, N, dt, False, cuda)
+    ops.gemm(a, w, residual=r, out=o, bn_hint=bn)
+    ref = a.double() @ w.double().t() + r.double()
+    tol = 1e-3 if out == "f32" else 16 + 1e-3
+    err = (o.double() - ref).abs()
+    assert not torch.isnan(o).any(), "unwritten output cells"
+    assert err.max().item() <= tol, f"bn={bn} N={N} {out}: max |err| {err.max().item():.4g} > {tol}"
+    _WORST["b"] = max(_WORST.get("b", 0.0), err.max().item() / tol)
+    _assert_untouched(buf, inside, f"fp32 residual bn={bn} N={N}")
+
+
+# ---------------------------------------------------------------------------------------------- (c) activation vs residual order
+@pytest.mark.parametrize("res", ["bf16", "f32"])
+@pytest.mark.parametrize("after", [False, True])
+@pytest.mark.parametrize("N", [96, 40])
+def test_act_residual_order(cuda, N, after, res):
+    """relu on a negative pre-activation (about -2) with a positive residual (3 .. 4): relu(x) + r = r, relu(x + r) = x + r, two
+    answers about 2 apart.  N = 96 runs the vectorised chunks only, N = 40 a full chunk and a ragged 8-column one."""
+    from efficientsam3_b200 import ops
+    M, K = 200, 64
+    g = _gen(cuda, "c", N, after, res)
+    a = _bf(torch.randn(M, K, device=cuda, generator=g))
+    w = _bf(torch.randn(N, K, device=cuda, generator=g) / (4 * math.sqrt(K)))
+    bias = torch.full((N,), -2.0, device=cuda)
+    r = 3 + torch.rand(M, N, device=cuda, generator=g)
+    r = _bf(r) if res == "bf16" else r
+    buf, o, inside = _matrix_out(M, N, torch.float32, False, cuda)
+    ops.gemm(a, w, bias=bias, act="relu", residual=r, out=o, act_after_res=after)
+    acc = a.double() @ w.double().t()
+    absprod = a.double().abs() @ w.double().abs().t()
+    ref, bound = _expect(acc, absprod, K, "relu", None, bias, r, after)
+    other, _ = _expect(acc, absprod, K, "relu", None, bias, r, not after)
+    assert ((ref - other).abs() > 1).double().mean().item() > 0.99        # the two orders are far apart on this data
+    _check("c", o, ref, bound, f"act/residual order N={N} after={after} res={res}")
+    _assert_untouched(buf, inside, "act/residual order")
+
+
+# ---------------------------------------------------------------------------------------------- (d) RoPE epilogue
+@pytest.mark.parametrize("win,out,bn", [(24, "bf16", 128), (24, "f32", 64), (0, "bf16", 64), (0, "f32", 128)])
+def test_rope_epilogue_teacher_geometry(cuda, win, out, bn):
+    """The SAM3 ViT's QKV projection: 72 x 72 tokens, B = 2, C = 1024, bias; windows of 24 (576 table positions) or global (5184).
+    q | k (columns < 2C) rotated per 64-dim head; v (columns >= 2C) bit-identical to the same GEMM without RoPE."""
+    from efficientsam3_b200 import ops
+    from efficientsam3_b200.model.vitdet import compute_axial_cis
+    B, H, W, C = 2, 72, 72, 1024
+    M, N, K = B * H * W, 3 * C, C
+    g = _gen(cuda, "d", win, out, bn)
+    a = _bf(torch.randn(M, K, device=cuda, generator=g))
+    w = _bf(torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K))
+    bias = torch.randn(N, device=cuda, generator=g)
+    cis = compute_axial_cis(64, win, win) if win else compute_axial_cis(64, H, W, scale_pos=24 / H)
+    tab = torch.view_as_real(cis).float().contiguous().to(cuda)                 # [positions, 32, 2] (cos, sin)
+    assert tab.shape[0] == (win * win if win else H * W)
+    dt = torch.float32 if out == "f32" else torch.bfloat16
+    buf, o, inside = _matrix_out(M, N, dt, False, cuda)
+    ops.gemm(a, w, bias=bias, rope=(tab, 2 * C, H, W, win), out=o, bn_hint=bn)
+    plain = ops.gemm(a, w, bias=bias, out_dtype=dt, bn_hint=bn)
+    assert torch.equal(o[:, 2 * C:].view(_INT[dt]), plain[:, 2 * C:].view(_INT[dt])), "v columns differ from the GEMM without RoPE"
+
+    acc = a.double() @ w.double().t()
+    absprod = a.double().abs() @ w.double().abs().t()
+    x, xb = _expect(acc, absprod, K, bias=bias)                                  # pre-rotation value and its bound
+    t = torch.arange(M, device=cuda) % (H * W)
+    hh, ww = t // W, t % W
+    pidx = (hh % win) * win + (ww % win) if win else t
+    cs = tab.double()[pidx]                                                      # [M, 32, 2]
+    c, s = cs[..., 0].repeat(1, 2 * C // 64), cs[..., 1].repeat(1, 2 * C // 64)  # per (q | k) column pair
+    x0, x1 = x[:, 0:2 * C:2], x[:, 1:2 * C:2]
+    b0, b1 = xb[:, 0:2 * C:2], xb[:, 1:2 * C:2]
+    ref, bound = x.clone(), xb.clone()
+    ref[:, 0:2 * C:2], ref[:, 1:2 * C:2] = x0 * c - x1 * s, x0 * s + x1 * c
+    rot = c.abs() * b0 + s.abs() * b1 + 4 * U * (x0.abs() * c.abs() + x1.abs() * s.abs())
+    bound[:, 0:2 * C:2], bound[:, 1:2 * C:2] = rot, c.abs() * b1 + s.abs() * b0 + 4 * U * (x0.abs() * s.abs() + x1.abs() * c.abs())
+    bound[:, :2 * C] += 4 * U * ref[:, :2 * C].abs()
+    if out == "bf16":
+        bound = bound * (1 + 2.0 ** -8) + 2.0 ** -8 * ref.abs()
+    _check(f"d/{out}", o, ref, bound, f"rope win={win} {out} bn={bn}")
+    _assert_untouched(buf, inside, "rope")
+
+
+# ---------------------------------------------------------------------------------------------- (e) es3_conv3x3_bf16
+def _conv3x3(cuda, x, w, epi, bn=0, seed=0):
+    """Run the implicit-GEMM conv through its C entry into a NaN-prefilled buffer; check it against fp64 F.conv2d."""
+    from efficientsam3_b200 import _lib, ops
+    B, H, W, C = x.shape
+    N = w.shape[0]
+    g = _gen(cuda, "e", B, H, W, C, N, epi, seed)
+    bias = torch.randn(N, device=cuda, generator=g) if epi != "nobias" else None
+    scale = (torch.rand(N, device=cuda, generator=g) + 0.5) if epi.startswith("scale") else None
+    act = {"scale_hswish": "hswish", "scale_gelu": "gelu"}.get(epi)
+    res = _bf(torch.randn(B, H, W, N, device=cuda, generator=g)) if epi == "bias_res" else None
+    dt = torch.float32 if epi == "bias_f32" else torch.bfloat16
+    w9 = w.permute(0, 2, 3, 1).reshape(N, 9 * C).contiguous()
+    buf, inside = _flat_out(B * H * W * N, dt, cuda)
+    _lib.init(cuda.index or 0)
+    rc = _lib.call_rc("es3_conv3x3_bf16", x.data_ptr(), w9.data_ptr(), buf.data_ptr(), int(dt == torch.float32), B, H, W, C, N,
+                      _ptr(scale), _ptr(bias), ops.ACT[act], _ptr(res), bn, _stream())
+    assert rc == 0
+    xn, wd = x.double().permute(0, 3, 1, 2), w.double()
+    acc = F.conv2d(xn, wd, padding=1).permute(0, 2, 3, 1)
+    absprod = F.conv2d(xn.abs(), wd.abs(), padding=1).permute(0, 2, 3, 1)
+    ref, bound = _expect(acc, absprod, 9 * C, act, scale, bias, res, False, out_bf16=dt == torch.bfloat16)
+    what = f"conv3x3 B{B} {H}x{W} C{C}->N{N} {epi} bn{bn}"
+    _check(f"e/{'f32' if dt == torch.float32 else 'bf16'}", buf[:B * H * W * N].view(B, H, W, N), ref, bound, what)
+    _assert_untouched(buf, inside, what)
+
+
+CONV_FACTORS = dict(
+    W=[64, 48, 144, 36, 23],           # tile width 32, 16, 16, 8, 8 (W % 32, W % 16)
+    H=[13, 7, 18],                     # never a multiple of the tile height (4, 8, 16): partial row tiles
+    C=[8, 32, 96, 256, 1024],          # C % 64 != 0: a tap's last k-block runs into the next tap's weights
+    N=[32, 64, 256, 1024],
+    epi=["bias", "nobias", "scale_hswish", "scale_gelu", "bias_f32", "bias_res"],
+)
+CONV_DESIGN = _pairwise(CONV_FACTORS, seed=2)
+
+
+@pytest.mark.parametrize("W,H,C,N,epi", CONV_DESIGN, ids=[f"W{c[0]}-H{c[1]}-C{c[2]}-N{c[3]}-{c[4]}" for c in CONV_DESIGN])
+def test_conv3x3_geometry(cuda, W, H, C, N, epi):
+    g = _gen(cuda, "conv", W, H, C, N, epi)
+    x = _bf(torch.randn(3, H, W, C, device=cuda, generator=g))
+    w = _bf(torch.randn(N, C, 3, 3, device=cuda, generator=g) / math.sqrt(9 * C))
+    _conv3x3(cuda, x, w, epi)
+
+
+@pytest.mark.parametrize("B,H,W,C,N,epi", [(1, 144, 144, 256, 256, "bias_f32"), (2, 144, 144, 256, 256, "bias"),
+                                           (2, 36, 36, 256, 256, "bias"), (2, 64, 64, 1024, 1024, "bias"),
+                                           (1, 64, 64, 1024, 1024, "nobias")])
+def test_conv3x3_production_shapes(cuda, B, H, W, C, N, epi):
+    """The FPN neck's 3x3 conv at the 2x (144^2, fp32 levels too) and 0.5x (36^2) levels; the student head at 64^2 and its input
+    gradient (no bias)."""
+    g = _gen(cuda, "prod", B, H, W, C, N, epi)
+    x = _bf(torch.randn(B, H, W, C, device=cuda, generator=g))
+    w = _bf(torch.randn(N, C, 3, 3, device=cuda, generator=g) / math.sqrt(9 * C))
+    _conv3x3(cuda, x, w, epi)
+
+
+@pytest.mark.parametrize("W", [64, 48, 23])
+def test_conv3x3_halo(cuda, W):
+    """Large values (8) in the last column and last row of every image, small ones (< 1/16) elsewhere: column 0 reading its left
+    neighbour from the previous row's last column, or an image's last row reading the next image's first row (or the reverse),
+    would be far outside the bound."""
+    B, H, C, N = 3, 13, 64, 64
+    g = _gen(cuda, "halo", W)
+    x = (torch.rand(B, H, W, C, device=cuda, generator=g) - 0.5) / 8
+    sgn = torch.randn(B, H, W, C, device=cuda, generator=g).sign()
+    x[:, :, -1] = 8 * sgn[:, :, -1]
+    x[:, -1] = 8 * sgn[:, -1]
+    w = _bf(torch.randn(N, C, 3, 3, device=cuda, generator=g) / math.sqrt(9 * C))
+    _conv3x3(cuda, _bf(x), w, "bias")
+
+
+# ---------------------------------------------------------------------------------------------- (f) es3_convt2x2_bf16
+def _convt2x2(cuda, B, H, W, Cin, Cout, mode, res, out, seed=0):
+    from efficientsam3_b200 import _lib, ops
+    g = _gen(cuda, "f", B, H, W, Cin, Cout, mode, res, out, seed)
+    x = _bf(torch.randn(B, H, W, Cin, device=cuda, generator=g))
+    w = _bf(torch.randn(Cin, Cout, 2, 2, device=cuda, generator=g) / math.sqrt(Cin))      # nn.ConvTranspose2d layout
+    bias = torch.randn(Cout, device=cuda, generator=g)
+    act = None if mode == "none" else "gelu"
+    after = mode == "gelu_after"
+    r = None
+    if res is not None:
+        r = torch.randn(B, 2 * H, 2 * W, Cout, device=cuda, generator=g)
+        r = _bf(r) if res == "bf16" else r
+    dt = torch.float32 if out == "f32" else torch.bfloat16
+    wt = ops.convt2x2_weight(w)
+    bias4 = bias.repeat(4).contiguous()
+    n = B * 4 * H * W * Cout
+    buf, inside = _flat_out(n, dt, cuda)
+    _lib.init(cuda.index or 0)
+    rc = _lib.call_rc("es3_convt2x2_bf16", x.data_ptr(), wt.data_ptr(), buf.data_ptr(), int(dt == torch.float32), B, H, W, Cin,
+                      Cout, bias4.data_ptr(), ops.ACT[act], _ptr(r), int(res == "f32"), int(after), _stream())
+    assert rc == 0
+    xn = x.double().permute(0, 3, 1, 2)
+    acc = F.conv_transpose2d(xn, w.double(), stride=2).permute(0, 2, 3, 1)
+    absprod = F.conv_transpose2d(xn.abs(), w.double().abs(), stride=2).permute(0, 2, 3, 1)
+    ref, bound = _expect(acc, absprod, Cin, act, None, bias, r, after, out_bf16=out == "bf16")
+    what = f"convt2x2 B{B} {H}x{W} {Cin}->{Cout} {mode} res={res} {out}"
+    _check(f"f/{out}", buf[:n].view(B, 2 * H, 2 * W, Cout), ref, bound, what)
+    _assert_untouched(buf, inside, what)
+
+
+CONVT_FACTORS = dict(
+    Cout=[32, 64, 256, 512],
+    Cin=[64, 256, 1024],
+    mode=["none", "gelu_before", "gelu_after"],
+    res=[None, "bf16", "f32"],
+    out=["bf16", "f32"],
+    HW=[(5, 7), (9, 3), (7, 11)],
+)
+CONVT_DESIGN = _pairwise(CONVT_FACTORS, seed=3)
+
+
+@pytest.mark.parametrize("Cout,Cin,mode,res,out,HW", CONVT_DESIGN,
+                         ids=[f"{c[1]}to{c[0]}-{c[2]}-r{c[3]}-{c[4]}-{c[5][0]}x{c[5][1]}" for c in CONVT_DESIGN])
+def test_convt2x2_scatter(cuda, Cout, Cin, mode, res, out, HW):
+    """Depth-to-space scatter: every output pixel written, each with the value of its own (dy, dx) weight slice."""
+    _convt2x2(cuda, 3, HW[0], HW[1], Cin, Cout, mode, res, out)
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,mode,res,out", [(1, 72, 72, 1024, 512, "gelu_before", None, "bf16"),
+                                                         (1, 144, 144, 512, 256, "none", None, "bf16"),
+                                                         (2, 72, 72, 256, 64, "none", "f32", "f32"),
+                                                         (2, 144, 144, 64, 32, "gelu_after", "f32", "f32")])
+def test_convt2x2_production_shapes(cuda, B, H, W, Cin, Cout, mode, res, out):
+    """The FPN neck's 4x level (1024 -> 512 with GELU, 512 -> 256) and the mask decoder's upscaling (256 -> 64 on an fp32 residual,
+    64 -> 32 with GELU after the residual)."""
+    _convt2x2(cuda, B, H, W, Cin, Cout, mode, res, out)
+
+
+# ---------------------------------------------------------------------------------------------- (g) es3_gemm_simt
+SIMT_FACTORS = dict(
+    dtypes=[("bf16", "bf16"), ("f32", "f32"), ("f32", "bf16"), ("bf16", "f32")],
+    res=[None, "bf16", "f32"],
+    out=["bf16", "f32"],
+    M=[1, 3, 17],
+    K=[20, 100],
+    N=[7, 40],
+    act=["relu", "sigmoid"],
+    scale=[False, True],
+)
+SIMT_DESIGN = _pairwise(SIMT_FACTORS, seed=4)
+
+
+@pytest.mark.parametrize("dtypes,res,out,M,K,N,act,has_s", SIMT_DESIGN,
+                         ids=[f"a{c[0][0]}-w{c[0][1]}-r{c[1]}-{c[2]}-M{c[3]}-K{c[4]}-N{c[5]}-{c[6]}{'-s' if c[7] else ''}"
+                              for c in SIMT_DESIGN])
+def test_gemm_simt(cuda, dtypes, res, out, M, K, N, act, has_s):
+    """The CUDA-core GEMM (SE MLPs and their backward in fp32, the decoder's token MLPs) with every operand dtype pair."""
+    from efficientsam3_b200 import ops
+    g = _gen(cuda, "g", dtypes, res, out, M, K, N, act, has_s)
+    a = torch.randn(M, K, device=cuda, generator=g)
+    w = torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K)
+    a = _bf(a) if dtypes[0] == "bf16" else a
+    w = _bf(w) if dtypes[1] == "bf16" else w
+    scale = (torch.rand(N, device=cuda, generator=g) + 0.5) if has_s else None
+    bias = torch.randn(N, device=cuda, generator=g)
+    r = None
+    if res is not None:
+        r = torch.randn(M, N, device=cuda, generator=g)
+        r = _bf(r) if res == "bf16" else r
+    dt = torch.float32 if out == "f32" else torch.bfloat16
+    buf, o, inside = _matrix_out(M, N, dt, True, cuda)
+    ops.gemm_simt(a, w, scale=scale, bias=bias, act=act, residual=r, out=o)
+    acc = a.double() @ w.double().t()
+    absprod = a.double().abs() @ w.double().abs().t()
+    ref, bound = _expect(acc, absprod, K, act, scale, bias, r, False, out_bf16=out == "bf16")
+    what = f"gemm_simt {dtypes} res={res} {out} {M}x{N}x{K} {act}"
+    _check(f"g/{out}", o, ref, bound, what)
+    _assert_untouched(buf, inside, what)
+
+
+# ---------------------------------------------------------------------------------------------- (h) what the wrappers refuse
+@pytest.mark.parametrize("act", ["sigmoid", "relu6", "gelu_tanh"])
+def test_tc_activation_not_instantiated(cuda, act):
+    """The wgmma kernel instantiates none / relu / hswish / gelu only; any other code is an error, not a silent identity."""
+    from efficientsam3_b200 import ops
+    from efficientsam3_b200._lib import Es3Error
+    x = torch.zeros(1, 8, 8, 64, device=cuda, dtype=torch.bfloat16)
+    with pytest.raises(Es3Error):
+        ops.gemm(x.view(64, 64), torch.zeros(64, 64, device=cuda, dtype=torch.bfloat16), act=act)
+    with pytest.raises(Es3Error):
+        ops.conv3x3(x, torch.zeros(64, 9 * 64, device=cuda, dtype=torch.bfloat16), act=act)
+    with pytest.raises(Es3Error):
+        ops.convt2x2(x, torch.zeros(4 * 32, 64, device=cuda, dtype=torch.bfloat16), act=act)
+
+
+def _refusals(cuda):
+    from efficientsam3_b200 import ops
+    bf, f32, f16 = torch.bfloat16, torch.float32, torch.float16
+    a, w = torch.zeros(64, 64, device=cuda, dtype=bf), torch.zeros(32, 64, device=cuda, dtype=bf)
+    x = torch.zeros(2, 8, 8, 64, device=cuda, dtype=bf)
+    w9, wt = torch.zeros(32, 9 * 64, device=cuda, dtype=bf), torch.zeros(4 * 32, 64, device=cuda, dtype=bf)
+    return {
+        "gemm fp16 out": lambda: ops.gemm(a, w, out=torch.zeros(64, 32, device=cuda, dtype=f16)),
+        "gemm fp16 residual": lambda: ops.gemm(a, w, residual=torch.zeros(64, 32, device=cuda, dtype=f16)),
+        "gemm fp16 bias": lambda: ops.gemm(a, w, bias=torch.zeros(32, device=cuda, dtype=f16)),
+        "gemm_simt fp16 a": lambda: ops.gemm_simt(a.half(), w),
+        "gemm_simt fp16 w": lambda: ops.gemm_simt(a, w.half()),
+        "gemm_simt fp64 a": lambda: ops.gemm_simt(a.double(), w),
+        "gemm_simt fp16 residual": lambda: ops.gemm_simt(a, w, residual=torch.zeros(64, 32, device=cuda, dtype=f16)),
+        "gemm_simt fp16 out": lambda: ops.gemm_simt(a, w, out_dtype=f16),
+        "gemm_simt fp16 scale": lambda: ops.gemm_simt(a, w, scale=torch.ones(32, device=cuda, dtype=f16)),
+        "conv3x3 fp32 residual": lambda: ops.conv3x3(x, w9, residual=torch.zeros(2, 8, 8, 32, device=cuda, dtype=f32)),
+        "conv3x3 strided residual": lambda: ops.conv3x3(x, w9, residual=torch.zeros(2, 8, 8, 64, device=cuda, dtype=bf)[..., :32]),
+        "conv3x3 residual shape": lambda: ops.conv3x3(x, w9, residual=torch.zeros(2, 8, 4, 64, device=cuda, dtype=bf)),
+        "conv3x3 fp16 out": lambda: ops.conv3x3(x, w9, out_dtype=f16),
+        "conv3x3 fp16 bias": lambda: ops.conv3x3(x, w9, bias=torch.zeros(32, device=cuda, dtype=f16)),
+        "convt2x2 fp16 residual": lambda: ops.convt2x2(x, wt, residual=torch.zeros(2, 16, 16, 32, device=cuda, dtype=f16)),
+        "convt2x2 fp16 out": lambda: ops.convt2x2(x, wt, out_dtype=f16),
+        "convt2x2 fp64 bias4": lambda: ops.convt2x2(x, wt, bias4=torch.zeros(128, device=cuda, dtype=torch.float64)),
+    }
+
+
+REFUSALS = ["gemm fp16 out", "gemm fp16 residual", "gemm fp16 bias", "gemm_simt fp16 a", "gemm_simt fp16 w", "gemm_simt fp64 a",
+            "gemm_simt fp16 residual", "gemm_simt fp16 out", "gemm_simt fp16 scale", "conv3x3 fp32 residual",
+            "conv3x3 strided residual", "conv3x3 residual shape", "conv3x3 fp16 out", "conv3x3 fp16 bias",
+            "convt2x2 fp16 residual", "convt2x2 fp16 out", "convt2x2 fp64 bias4"]
+
+
+@pytest.mark.parametrize("case", REFUSALS)
+def test_wrapper_rejects_dtype_the_kernel_would_misread(cuda, case):
+    """Operand, residual and output dtypes other than the ones each kernel reads raise instead of being reinterpreted."""
+    from efficientsam3_b200 import ops
+    from efficientsam3_b200._lib import Es3Error
+    n0 = ops.launch_count
+    with pytest.raises(Es3Error):
+        _refusals(cuda)[case]()
+    assert ops.launch_count == n0

@@ -136,6 +136,11 @@ SIGNATURES: dict[str, list] = {
     "es3_bilinear_bwd": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp],
     "es3_litemla_attn_bwd_generic": [_vp, _ll, _vp, _ll, _vp, _i, _vp, _vp, _ll, _i, _i, _i, _i, _f, _vp],
     "es3_litemla_attn_bwd": [_vp, _ll, _vp, _ll, _vp, _i, _vp, _vp, _ll, _i, _i, _i, _f, _vp],
+    # opt-in FP8 route of the ViT teacher's linear layers (gemm_fp8.cu, vit_ops.cu)
+    "es3_gemm_fp8": [_vp, _ll, _vp, _vp, _ll, _vp, _vp, _ll, _i, _vp, _i, _i, _i, _vp, _i, _vp, _ll, _vp, _i, _i, _i, _i, _vp],
+    "es3_quantize_bf16_e4m3": [_vp, _ll, _vp, _vp, _ll, _i, _vp],
+    "es3_pack_weight_e4m3": [_vp, _i, _vp, _vp, _i, _i, _vp],
+    "es3_layernorm_f32_e4m3": [_vp, _vp, _vp, _f, _vp, _vp, _ll, _i, _vp],
 }
 
 # workspace-size helpers: name -> argtypes, restype long long

@@ -7,15 +7,18 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "fp8.cuh"
 
 namespace es3 {
 
 // One warp per row.  C % 128 == 0, C <= 2048.  x fp32 [M, C]; pos (optional) fp32 [ps*ps, C] tiled over an
-// (H, W) token grid; gamma/beta fp32.  Writes y_bf16 and/or y_f32 (either may be null).
-template <int VPL>  // float4 vectors per lane = C / 128
+// (H, W) token grid; gamma/beta fp32.  Writes y_bf16 and/or y_f32 (either may be null); Q8: writes y_q e4m3 [M, C] and
+// y_qs fp32 [M, C / 128] instead (fp8.cuh: vector i of every lane is 128-column block i, so a block's amax is one warp max).
+template <int VPL, bool Q8 = false>  // float4 vectors per lane = C / 128
 __global__ void layernorm_kernel(const float* __restrict__ x, const float* __restrict__ pos, int ps, int H, int W,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                                 bf16* __restrict__ y_bf16, float* __restrict__ y_f32, long long M) {
+                                 bf16* __restrict__ y_bf16, float* __restrict__ y_f32, long long M,
+                                 uint8_t* __restrict__ y_q = nullptr, float* __restrict__ y_qs = nullptr) {
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
@@ -55,6 +58,12 @@ __global__ void layernorm_kernel(const float* __restrict__ x, const float* __res
     o.y = (v[i].y - mean) * rstd * g.y + bb.y;
     o.z = (v[i].z - mean) * rstd * g.z + bb.z;
     o.w = (v[i].w - mean) * rstd * g.w + bb.w;
+    if constexpr (Q8) {
+      const float sc = e4m3_block_scale(warp_max(abs_max4(o.x, o.y, o.z, o.w)));
+      reinterpret_cast<uint32_t*>(y_q + row * C)[lane + i * 32] = e4m3x4(o.x, o.y, o.z, o.w, sc);
+      if (lane == 0) y_qs[row * VPL + i] = sc;
+      continue;
+    }
     if (y_f32) reinterpret_cast<float4*>(y_f32 + row * C)[lane + i * 32] = o;
     if (y_bf16) {
       uint2 u;
@@ -119,6 +128,24 @@ extern "C" int es3_layernorm_f32(const float* x, const float* pos, int pos_size,
   }
 #undef ES3_LN
   ES3_LAUNCH_CHECK("layernorm_kernel");
+  return 0;
+}
+
+// LayerNorm of the fp32 rows straight to the FP8 GEMM's A operand: e4m3 q [M, C] + fp32 scales [M, C / 128] (fp8.cuh).  The
+// statistics and the normalised value are the same arithmetic as es3_layernorm_f32's.
+extern "C" int es3_layernorm_f32_e4m3(const float* x, const float* gamma, const float* beta, float eps, void* q, float* scales,
+                                      long long M, int C, void* stream) {
+  ES3_REQUIRE(C % 128 == 0 && C <= 2048, "es3_layernorm_f32_e4m3: C=%d must be a multiple of 128 and <= 2048", C);
+  const int warps = 8;
+  const unsigned blocks = (unsigned)ceil_div(M, warps);
+  cudaStream_t st = (cudaStream_t)stream;
+#define ES3_LNQ(V) case V: layernorm_kernel<V, true><<<blocks, warps * 32, 0, st>>>(x, nullptr, 0, 0, 0, gamma, beta, eps, nullptr, nullptr, M, (uint8_t*)q, scales); break;
+  switch (C / 128) {
+    ES3_LNQ(8) ES3_LNQ(16)
+    default: ES3_REQUIRE(false, "es3_layernorm_f32_e4m3: C=%d not instantiated (1024, 2048)", C);
+  }
+#undef ES3_LNQ
+  ES3_LAUNCH_CHECK("layernorm_kernel<e4m3>");
   return 0;
 }
 

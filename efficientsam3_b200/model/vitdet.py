@@ -11,6 +11,11 @@ Device path per block (all libes3.so):
   LayerNorm, fc1 + GELU(erf), fc2 + fp32 residual        es3_layernorm_f32, es3_gemm_bf16_ex x2
 Patch embedding = es3_im2col_patch + GEMM; tiled abs-pos add is fused into ln_pre.
 Eval-mode only (the teacher is frozen: stage1/model.py:225-227).
+
+ViT.enable_fp8() (off by default; the strict precision mode ignores it) moves the four linear layers to block-scaled e4m3
+(gemm_fp8.cu): norm1 / norm2 write e4m3 (es3_layernorm_f32_e4m3), the attention output is quantised (es3_quantize_bf16_e4m3),
+fc1's epilogue writes fc2's e4m3 operand, and the weights are packed once per parameter version (es3_pack_weight_e4m3).  Patch
+embedding, the LayerNorm statistics, RoPE, attention and the fp32 residual stream stay as above.
 """
 from __future__ import annotations
 
@@ -90,6 +95,12 @@ def _lin(linear: nn.Linear):
             linear.bias.detach().float().contiguous() if linear.bias is not None else None)
 
 
+def _lin8(linear: nn.Linear):
+    w = linear.weight.detach()
+    return (*ops.pack_weight_e4m3(w if w.dtype in (torch.bfloat16, torch.float32) else w.float()),
+            linear.bias.detach().float().contiguous() if linear.bias is not None else None)
+
+
 class ViT(nn.Module, NativePlanMixin):
     def __init__(self, img_size=1024, patch_size=16, in_chans=3, embed_dim=768, depth=12, num_heads=12, mlp_ratio=4.0,
                  qkv_bias=True, drop_path_rate=0.0, norm_layer: Union[Callable[..., nn.Module], str] = "LayerNorm",
@@ -132,6 +143,15 @@ class ViT(nn.Module, NativePlanMixin):
                 if m.bias is not None:
                     nn.init.constant_(m.bias, 0)
 
+    _fp8 = False
+
+    def enable_fp8(self, enabled: bool = True):
+        """Run qkv, proj, fc1 and fc2 as block-scaled e4m3 GEMMs (off by default; ignored in the strict precision mode).  The
+        weights are packed to e4m3 on the next forward and again whenever a parameter changes.  Returns self."""
+        self._fp8 = bool(enabled)
+        self._plan_key = None
+        return self
+
     def _build_plan(self):
         P, C = self.patch_size, self.embed_dim
         kp = (3 * P * P + 7) // 8 * 8
@@ -147,6 +167,9 @@ class ViT(nn.Module, NativePlanMixin):
                 qkv=_lin(blk.attn.qkv), proj=_lin(blk.attn.proj), fc1=_lin(blk.mlp.fc1), fc2=_lin(blk.mlp.fc2),
                 rope=torch.view_as_real(blk.attn.freqs_cis.detach().to(torch.complex64)).float().contiguous(),
                 win=blk.window_size, scale=blk.attn.scale))
+            if self._fp8:
+                blocks[-1].update(qkv8=_lin8(blk.attn.qkv), proj8=_lin8(blk.attn.proj), fc1_8=_lin8(blk.mlp.fc1),
+                                  fc2_8=_lin8(blk.mlp.fc2))
         return dict(kp=kp, wpe=wpe, pos=tab.float().contiguous(), pos_size=int(math.isqrt(tab.shape[0])),
                     ln_pre=(self.ln_pre.weight.detach().float().contiguous(), self.ln_pre.bias.detach().float().contiguous(),
                             self.ln_pre.eps), blocks=blocks)
@@ -171,6 +194,16 @@ class ViT(nn.Module, NativePlanMixin):
         tok = ops.gemm(cols, p["wpe"], out_dtype=torch.float32)
         g, b_, eps = p["ln_pre"]
         _, xs = ops.layernorm(tok, g, b_, eps, pos=p["pos"], pos_size=p["pos_size"], H=h, W=w, out_bf16=False, out_f32=True)
+        if self._fp8:
+            for bp in p["blocks"]:
+                q, s = ops.layernorm_e4m3(xs, *bp["n1"])
+                qkv = ops.gemm_fp8(q, s, *bp["qkv8"], rope=(bp["rope"], 2 * C, h, w, bp["win"]))
+                a = ops.attention(qkv, B, h, w, C, heads, bp["win"], bp["scale"])
+                xs = ops.gemm_fp8(*ops.quantize_e4m3(a), *bp["proj8"], residual=xs, out_dtype=torch.float32)
+                q, s = ops.layernorm_e4m3(xs, *bp["n2"])
+                q, s = ops.gemm_fp8(q, s, *bp["fc1_8"], act="gelu", out_dtype=ops.E4M3)
+                xs = ops.gemm_fp8(q, s, *bp["fc2_8"], residual=xs, out_dtype=torch.float32)
+            return xs, (B, h, w)
         for bp in p["blocks"]:
             y, _ = ops.layernorm(xs, *bp["n1"])
             qkv = ops.gemm(y, bp["qkv"][0], bias=bp["qkv"][1], rope=(bp["rope"], 2 * C, h, w, bp["win"]))

@@ -952,6 +952,140 @@ def cast_f32_to_f16(x, out=None):
     return out
 
 
+# ------------------------------------------------------------------------------------ FP8 (e4m3) teacher linears
+# Block-scaled e4m3 (gemm_fp8.cu, fp8.cuh): an activation [M, K] carries fp32 scales [M, K / 128] (one per row per 128 K
+# elements), a weight [N, K] scales [ceil(N / 128), K / 128] (one per 128 x 128 block); s = amax / 448 (1 for an all-zero
+# block), q = e4m3_rn_satfinite(x / s).  Shapes, dtypes and strides are checked here and raise ValueError before anything
+# launches; a tensor off the GPU then raises Es3Error as everywhere else.
+E4M3 = torch.float8_e4m3fn
+FP8_BLOCK = 128
+
+
+def _fp8_fail(cond, msg):
+    if not cond:
+        raise ValueError(msg)
+
+
+def _fp8_2d(t, dtype, name):
+    _fp8_fail(torch.is_tensor(t) and t.dim() == 2, f"{name}: expected a 2-D tensor")
+    _fp8_fail(t.dtype == dtype, f"{name}: expected {dtype}, got {t.dtype}")
+    _fp8_fail(t.stride(1) == 1, f"{name}: columns must be contiguous")
+
+
+def _fp8_scales(s, shape, name):
+    _fp8_fail(torch.is_tensor(s) and s.dtype == torch.float32, f"{name}: expected fp32 scales")
+    _fp8_fail(tuple(s.shape) == tuple(shape) and s.is_contiguous(), f"{name}: expected contiguous scales of shape {tuple(shape)}, "
+              f"got {tuple(s.shape)}")
+
+
+def _fp8_cuda(*ts):
+    for t in ts:
+        if t is not None and not t.is_cuda:
+            raise _lib.Es3Error("FP8 ops: expected CUDA tensors (the native path has no CPU fallback)")
+
+
+def _fp8_out(M, C, dev):
+    return (torch.empty((M, C), device=dev, dtype=E4M3),
+            torch.empty((M, C // FP8_BLOCK), device=dev, dtype=torch.float32))
+
+
+def quantize_e4m3(x):
+    """bf16 [M, C] (row stride allowed), C % 128 == 0 -> (e4m3 [M, C], fp32 scales [M, C / 128])."""
+    _fp8_2d(x, torch.bfloat16, "x")
+    M, C = x.shape
+    _fp8_fail(M > 0 and C % FP8_BLOCK == 0, f"quantize_e4m3: C={C} must be a multiple of 128")
+    _fp8_fail(x.stride(0) % 4 == 0 and x.data_ptr() % 8 == 0, "quantize_e4m3: row stride must be a multiple of 4 elements")
+    _fp8_cuda(x)
+    _ensure_init(x)
+    q, s = _fp8_out(M, C, x.device)
+    _call("es3_quantize_bf16_e4m3", "quantize_e4m3", _nb(x, q, s), 2 * M * C, x.data_ptr(), x.stride(0), q.data_ptr(),
+          s.data_ptr(), M, C, _stream())
+    return q, s
+
+
+def layernorm_e4m3(x, gamma, beta, eps=1e-5):
+    """LayerNorm of fp32 rows [M, C] (C = 1024 or 2048) -> (e4m3 [M, C], fp32 scales [M, C / 128]); the same normalised values as
+    layernorm(x, ..., out_f32=True), quantised."""
+    _fp8_2d(x, torch.float32, "x")
+    M, C = x.shape
+    _fp8_fail(M > 0 and C in (1024, 2048) and x.is_contiguous(), f"layernorm_e4m3: contiguous [M, C] with C in (1024, 2048), got C={C}")
+    for t, n in ((gamma, "gamma"), (beta, "beta")):
+        _fp8_fail(t.dtype == torch.float32 and t.is_contiguous() and t.numel() == C, f"layernorm_e4m3: {n} must be fp32 [{C}]")
+    _fp8_cuda(x, gamma, beta)
+    _ensure_init(x)
+    q, s = _fp8_out(M, C, x.device)
+    _call("es3_layernorm_f32_e4m3", "layernorm_e4m3", _nb(x, q, s), 8 * M * C, x.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
+          float(eps), q.data_ptr(), s.data_ptr(), M, C, _stream())
+    return q, s
+
+
+def pack_weight_e4m3(w):
+    """Linear weight bf16 or fp32 [N, K], K % 128 == 0 -> (e4m3 [N, K], fp32 scales [ceil(N / 128), K / 128])."""
+    _fp8_fail(torch.is_tensor(w) and w.dim() == 2 and w.dtype in _BF16_F32, "pack_weight_e4m3: expected a bf16 or fp32 [N, K] weight")
+    N, K = w.shape
+    _fp8_fail(N > 0 and K % FP8_BLOCK == 0, f"pack_weight_e4m3: K={K} must be a multiple of 128")
+    _fp8_cuda(w)
+    _ensure_init(w)
+    w = w.contiguous()
+    q = torch.empty((N, K), device=w.device, dtype=E4M3)
+    s = torch.empty(((N + FP8_BLOCK - 1) // FP8_BLOCK, K // FP8_BLOCK), device=w.device, dtype=torch.float32)
+    _call("es3_pack_weight_e4m3", "pack_weight_e4m3", _nb(w, q, s), 2 * N * K, w.data_ptr(), int(w.dtype == torch.float32),
+          q.data_ptr(), s.data_ptr(), N, K, _stream())
+    return q, s
+
+
+_FP8_OUT = {torch.bfloat16: 0, torch.float32: 1, E4M3: 2}
+
+
+def gemm_fp8(a, sa, w, sw, bias=None, *, act=None, residual=None, rope=None, out_dtype=torch.bfloat16):
+    """Block-scaled e4m3 GEMM: out[m, n] = epi(sum_k dequant(a)[m, k] dequant(w)[n, k] + bias[n]).
+    a e4m3 [M, K] (row stride a multiple of 16), sa [M, K / 128]; w e4m3 [N, K], sw [N / 128, K / 128]; N, K multiples of 128.
+    Epilogues: out_dtype bf16 with optional rope = (table [P, 32, 2], rope_cols, H, W, win) (the qkv projection); fp32 with an
+    optional fp32 residual [M, N] (proj, fc2); act="gelu" to e4m3, returning (q [M, N], scales [M, N / 128]) (fc1), or to fp32."""
+    _fp8_2d(a, E4M3, "a")
+    _fp8_2d(w, E4M3, "w")
+    M, K = a.shape
+    N = w.shape[0]
+    _fp8_fail(w.shape[1] == K, f"gemm_fp8: a is [{M}, {K}] but w is {tuple(w.shape)}")
+    _fp8_fail(M > 0 and K % FP8_BLOCK == 0 and N % FP8_BLOCK == 0, f"gemm_fp8: N={N} and K={K} must be multiples of 128")
+    _fp8_fail(a.stride(0) % 16 == 0 and w.stride(0) % 16 == 0 and a.data_ptr() % 16 == 0 and w.data_ptr() % 16 == 0,
+              "gemm_fp8: operand rows must start 16-byte aligned (row strides multiples of 16)")
+    _fp8_scales(sa, (M, K // FP8_BLOCK), "sa")
+    _fp8_scales(sw, (N // FP8_BLOCK, K // FP8_BLOCK), "sw")
+    _fp8_fail(out_dtype in _FP8_OUT, f"gemm_fp8: out_dtype must be bf16, fp32 or float8_e4m3fn, got {out_dtype}")
+    _fp8_fail(act in (None, "none", "gelu"), f"gemm_fp8: act must be None or 'gelu', got {act!r}")
+    gelu = act == "gelu"
+    _fp8_fail(not (out_dtype == torch.bfloat16 and gelu), "gemm_fp8: the bf16 epilogue has no activation")
+    _fp8_fail(out_dtype != E4M3 or gelu, "gemm_fp8: the e4m3 epilogue is bias + GELU (act='gelu')")
+    if bias is not None:
+        _fp8_fail(bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == N, f"gemm_fp8: bias must be fp32 [{N}]")
+    if residual is not None:
+        _fp8_2d(residual, torch.float32, "residual")
+        _fp8_fail(out_dtype == torch.float32 and not gelu, "gemm_fp8: a residual needs out_dtype=fp32 and no activation")
+        _fp8_fail(tuple(residual.shape) == (M, N) and residual.stride(0) % 2 == 0, f"gemm_fp8: residual must be [{M}, {N}]")
+    rargs = (0, 0, 0, 0, 0)
+    if rope is not None:
+        tab, rcols, rH, rW, rwin = rope
+        _fp8_fail(out_dtype == torch.bfloat16, "gemm_fp8: the RoPE epilogue writes bf16")
+        _fp8_fail(tab.dtype == torch.float32 and tab.is_contiguous() and tab.dim() == 3 and tuple(tab.shape[1:]) == (32, 2),
+                  "gemm_fp8: rope table must be fp32 [P, 32, 2]")
+        _fp8_fail(rcols % FP8_BLOCK == 0 and 0 < rcols <= N and rH > 0 and rW > 0 and M % (rH * rW) == 0
+                  and tab.shape[0] == (rwin * rwin if rwin else rH * rW), "gemm_fp8: bad rope arguments")
+        rargs = (tab.data_ptr(), rcols, rH, rW, rwin)
+    _fp8_cuda(a, sa, w, sw, bias, residual, rope[0] if rope is not None else None)
+    _ensure_init(a)
+    scales = None
+    if out_dtype == E4M3:
+        out, scales = _fp8_out(M, N, a.device)
+    else:
+        out = torch.empty((M, N), device=a.device, dtype=out_dtype)
+    _call("es3_gemm_fp8", f"gemm_fp8[K={K},N={N}]", M * K + N * K + M * N * out.element_size() + _nb(residual), 2 * M * N * K,
+          a.data_ptr(), a.stride(0), sa.data_ptr(), w.data_ptr(), w.stride(0), sw.data_ptr(), out.data_ptr(), out.stride(0),
+          _FP8_OUT[out_dtype], _ptr(scales), M, N, K, _ptr(bias), ACT[act], _ptr(residual),
+          residual.stride(0) if residual is not None else 0, *rargs, _stream())
+    return (out, scales) if out_dtype == E4M3 else out
+
+
 # ------------------------------------------------------------------------------------ SAM heads
 def convt2x2(x, wt, bias4=None, act=None, residual=None, out_dtype=torch.bfloat16, act_after_res=False):
     """ConvTranspose2d(k=2,s=2) on NHWC: x [B,H,W,Cin] bf16, wt [4*Cout, Cin] bf16 -> [B,2H,2W,Cout]."""

@@ -333,6 +333,11 @@ class SAM3ImageTeacherEncoder(nn.Module):
             feats, _ = ops.bilinear_nchw(feats, self.embed_size, self.embed_size)
         return feats
 
+    def enable_fp8(self, enabled: bool = True):
+        """Run the trunk's linear layers as block-scaled e4m3 GEMMs (ViT.enable_fp8; off by default).  Returns self."""
+        self.sam3.backbone.vision_backbone.trunk.enable_fp8(enabled)
+        return self
+
 
 class RepViTAdapter(nn.Module):
     """stage1/model.py:287-296."""

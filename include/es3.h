@@ -174,6 +174,26 @@ int es3_tokens_f32_to_nchw(const float* in, float* out, int B, int HW, int C, vo
  * (save_embedding_image_stage1.py:92); done on the device so the D2H copy moves 2 bytes per element. */
 int es3_cast_f32_to_f16(const float* in, void* out, long long n, void* stream);
 
+/* ------------------------------------------------------------------------------------------ FP8 teacher linears (opt-in) */
+/* Block-scaled e4m3: an activation [M, K] carries one fp32 scale per row per 128 consecutive K elements ([M, K/128]), a
+ * weight [N, K] one per 128 x 128 block ([ceil(N/128), K/128]).  s = amax / 448 (s = 1 for an all-zero block),
+ * q = e4m3_rn_satfinite(x / s), both divisions IEEE round-to-nearest. */
+/* out = epi(sum_kb sA[m,kb] sW[n/128,kb] (qA qW^T)_kb + bias) on wgmma e4m3 with the per-block partial sums promoted into an fp32
+ * accumulator.  A [M][lda bytes], W [N][ldw bytes], both K-major; N % 128 == 0, K % 128 == 0.  out_kind 0 bf16 (act none,
+ * optional 2-D RoPE on columns [0, rope_cols): the rope arguments of es3_gemm_bf16_ex), 1 fp32 (act none with optional fp32
+ * residual [M][ldr], or act GELU), 2 e4m3 [M][ldo bytes] + out_scales [M, N/128] (act GELU). */
+int es3_gemm_fp8(const void* A, long long lda, const float* sA, const void* W, long long ldw, const float* sW, void* out,
+                 long long ldo, int out_kind, float* out_scales, int M, int N, int K, const float* bias, int act,
+                 const float* residual, long long ldr, const float* rope, int rope_cols, int rope_H, int rope_W, int rope_win,
+                 void* stream);
+/* bf16 [M, C] (row stride lda elements, C % 128 == 0) -> e4m3 [M, C] + scales [M, C/128]: the attention output as proj's A. */
+int es3_quantize_bf16_e4m3(const void* x, long long lda, void* q, float* scales, long long M, int C, void* stream);
+/* Weight [N, K] (bf16, or fp32 when w_f32) -> e4m3 [N, K] + scales [ceil(N/128), K/128]; K % 128 == 0. */
+int es3_pack_weight_e4m3(const void* w, int w_f32, void* q, float* scales, int N, int K, void* stream);
+/* es3_layernorm_f32 (no pos add) writing e4m3 [M, C] + scales [M, C/128] instead of bf16 / fp32; C = 1024 or 2048. */
+int es3_layernorm_f32_e4m3(const float* x, const float* gamma, const float* beta, float eps, void* q, float* scales,
+                           long long M, int C, void* stream);
+
 /* ------------------------------------------------------------------------------------------ text encoders */
 /* Causal softmax attention, head_dim 64, over B sequences of L tokens on the fused qkv activation [B*L, 3C] bf16 ->
  * [B*L, C] bf16: token l attends to tokens 0..l (the triu(-inf) additive mask of MobileCLIP-B and the SAM3 text

@@ -1,0 +1,411 @@
+"""The opt-in FP8 route of the SAM3 ViT teacher's linear layers (csrc/gemm_fp8.cu, ViT.enable_fp8).
+
+Quantisers (LayerNorm -> e4m3, bf16 -> e4m3, the weight packer) must be bit-identical to the host emulation (tests/emu_fp8.py),
+codes and scales.  The GEMM is checked element by element against fp64 of its dequantised operands, in the style of
+test_gemm_epilogue_gpu.py (NaN-prefilled outputs, strided operands cut from NaN-padded buffers), with the per-element bound
+
+    |got - ref| <= (EPS_INNER + GAMMA (K / 128 + 2) u) * (|A| |W|^T) + 4u (|acc| + |bias|) (+ epilogue terms) + 4u |ref|
+
+EPS_INNER covers the tensor core's accumulation of e4m3 products inside one 128-wide K block, which NVIDIA does not document; the
+fp32 promotion of each block's partial sum and the sum across blocks are the GAMMA term.  Measured on an H100 80GB HBM3 (700 W power
+limit), one run of this file: the largest err / (|A| |W|^T) over its GEMMs was 2.0e-4 (about 2^-12.3), so EPS_INNER = 2^-11 = 4.9e-4
+leaves a factor of 2.4.  A kernel that accumulated all of K in the tensor core fails this bound: on the `spread` operands the
+per-block scales differ by up to 2^6 along K, so no single scale per output can be right, and on the unit-scale K = 4736 operands
+the block error could compound over 37 blocks against a bound that allows 2.4 blocks' worth.
+"""
+import math
+import zlib
+
+import pytest
+import torch
+
+from emu_fp8 import BLOCK, E4M3, dequant_rows, dequant_weight, quantize_rows, quantize_weight
+from helpers import cosine, rel_l2
+
+pytestmark = pytest.mark.gpu
+
+U = 2.0 ** -24
+GAMMA = 2.0
+EPS_INNER = 2.0 ** -11
+_WORST: dict = {}
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _report_worst():
+    yield
+    for k in sorted(_WORST):
+        print(f"\nfp8 gemm {k}: max {_WORST[k]:.3g}", end="")
+
+
+def _gen(*key):
+    return torch.Generator().manual_seed(zlib.crc32(repr(key).encode()))
+
+
+def _u8(t):
+    return t.view(torch.uint8)
+
+
+def _assert_codes(got_q, got_s, want_q, want_s, what):
+    gq, wq = _u8(got_q.cpu()), _u8(want_q)
+    bad = (gq != wq).nonzero()
+    assert bad.numel() == 0, f"{what}: {bad.shape[0]} codes differ, first at {tuple(bad[0].tolist())}: " \
+                             f"{int(gq[tuple(bad[0])])} vs {int(wq[tuple(bad[0])])}"
+    assert torch.equal(got_s.cpu().view(torch.int32), want_s.view(torch.int32)), f"{what}: scales differ"
+
+
+def _rows_with_spread(M, C, g, strided_amax=True):
+    """fp32 rows whose amax sits in a different 128-block per row, one all-zero block, and tiny values that quantise to
+    e4m3 subnormals next to a large one."""
+    x = torch.randn(M, C, generator=g)
+    if strided_amax:
+        for r in range(M):
+            x[r, (r % (C // BLOCK)) * BLOCK + (r * 7) % BLOCK] = 40.0 * (1 if r % 2 else -1)
+    if M > 2:
+        x[1, :BLOCK] = 0.0
+        x[2, BLOCK:2 * BLOCK] = torch.randn(BLOCK, generator=g) * 3e-5
+        x[2, BLOCK + 5] = 3.0
+    return x
+
+
+# ---------------------------------------------------------------------------------------------- quantisers
+@pytest.mark.parametrize("M,C,strided", [(1, 128, False), (77, 1024, True), (300, 384, False), (1029, 2048, True)])
+def test_quantize_bf16_bit_exact(cuda, M, C, strided):
+    from efficientsam3_b200 import ops
+    x = _rows_with_spread(M, C, _gen("q", M, C)).to(torch.bfloat16)
+    if strided:
+        big = torch.full((M, C + 64), float("nan"), dtype=torch.bfloat16)
+        big[:, 32:32 + C] = x
+        xd = big.to(cuda)[:, 32:32 + C]
+    else:
+        xd = x.to(cuda)
+    q, s = ops.quantize_e4m3(xd)
+    wq, ws = quantize_rows(x.float())
+    c = _u8(wq)
+    assert M < 3 or (((c & 0x78) == 0) & ((c & 0x07) != 0)).any()          # e4m3 subnormal codes are exercised
+    _assert_codes(q, s, wq, ws, f"quantize_e4m3 {M}x{C}")
+
+
+@pytest.mark.parametrize("M,C", [(1, 1024), (133, 1024), (517, 2048)])
+def test_layernorm_e4m3_bit_exact(cuda, M, C):
+    """The quantised LayerNorm equals the emulation applied to es3_layernorm_f32's fp32 output (same statistics, same arithmetic)."""
+    from efficientsam3_b200 import ops
+    g = _gen("ln", M, C)
+    x = (_rows_with_spread(M, C, g) * 3 + 1).to(cuda)
+    gamma = (torch.rand(C, generator=g) + 0.5).to(cuda)
+    beta = (torch.randn(C, generator=g) * 0.1).to(cuda)
+    q, s = ops.layernorm_e4m3(x, gamma, beta, 1e-6)
+    _, y = ops.layernorm(x, gamma, beta, 1e-6, out_bf16=False, out_f32=True)
+    wq, ws = quantize_rows(y.cpu())
+    _assert_codes(q, s, wq, ws, f"layernorm_e4m3 {M}x{C}")
+
+
+@pytest.mark.parametrize("N,K,dtype", [(128, 128, torch.float32), (200, 384, torch.float32), (3072, 1024, torch.bfloat16),
+                                       (4736, 1024, torch.float32), (77, 256, torch.bfloat16)])
+def test_pack_weight_bit_exact(cuda, N, K, dtype):
+    from efficientsam3_b200 import ops
+    g = _gen("w", N, K)
+    w = torch.randn(N, K, generator=g) * 0.02
+    w[min(5, N - 1), 130 % K] = 0.5
+    if K > 128:
+        w[:min(N, 128), :128] = 0.0                                           # an all-zero block
+    w = w.to(dtype)
+    q, s = ops.pack_weight_e4m3(w.to(cuda))
+    wq, ws = quantize_weight(w.float())
+    _assert_codes(q, s, wq, ws, f"pack_weight_e4m3 {N}x{K} {dtype}")
+
+
+# ---------------------------------------------------------------------------------------------- GEMM vs fp64
+def _operands(cuda, M, N, K, spread, strided, g):
+    """Quantised operands on the device and their fp64 dequantised values.  spread: activation blocks scaled by 2^(kb mod 5),
+    weight blocks by 2^-(kb mod 3) (per-block scales that differ along K); otherwise unit scales (|x| <= 448 e4m3 values with a
+    448 in every block)."""
+    if spread:
+        x = torch.randn(M, K, generator=g) * torch.tensor([2.0 ** (kb % 5) for kb in range(K // BLOCK)]).repeat_interleave(BLOCK)
+        w = torch.randn(N, K, generator=g) / math.sqrt(K) * torch.tensor([2.0 ** -(kb % 3) for kb in range(K // BLOCK)]).repeat_interleave(BLOCK)
+        qa, sa = quantize_rows(x)
+        qw, sw = quantize_weight(w)
+    else:
+        qa = e4m3_values(M, K, g)
+        qw = e4m3_values(N, K, g)
+        sa, sw = torch.ones(M, K // BLOCK), torch.ones(N // BLOCK, K // BLOCK)
+    a64, w64 = dequant_rows(qa, sa).double(), dequant_weight(qw, sw).double()
+    if strided:
+        big = torch.full((M, K + 64), float("nan")).to(E4M3)
+        big[:, 32:32 + K] = qa
+        qa_d = big.to(cuda)[:, 32:32 + K]
+    else:
+        qa_d = qa.to(cuda)
+    return qa_d, sa.to(cuda), qw.to(cuda), sw.to(cuda), a64, w64
+
+
+PAD = 16                 # output rows are N + PAD wide; the pad columns and a tail row keep their NaN sentinel
+
+
+def _run(cuda, qa, sa, qw, sw, bias=None, out=torch.float32, act=None, residual=None, rope=None):
+    """es3_gemm_fp8 into a NaN-prefilled output [M + 1, N + PAD] (and NaN-prefilled scales); returns the [M, N] results after
+    checking that no cell outside them was written."""
+    from efficientsam3_b200 import _lib, ops
+    M, N, K = qa.shape[0], qw.shape[0], qa.shape[1]
+    kind = {torch.bfloat16: 0, torch.float32: 1, E4M3: 2}[out]
+    buf = torch.full((M + 1, N + PAD), float("nan"), device=cuda).to(out)
+    sbuf = torch.full((M + 1, N // BLOCK), float("nan"), device=cuda)
+    ibits = {torch.bfloat16: torch.int16, torch.float32: torch.int32, E4M3: torch.uint8}[out]
+    sentinel = buf.view(ibits)[0, 0].item()
+    rargs = (0, 0, 0, 0, 0) if rope is None else (rope[0].data_ptr(), *rope[1:])
+    _lib.init(cuda.index or 0)
+    rc = _lib.call_rc("es3_gemm_fp8", qa.data_ptr(), qa.stride(0), sa.data_ptr(), qw.data_ptr(), qw.stride(0), sw.data_ptr(),
+                      buf.data_ptr(), buf.stride(0), kind, sbuf.data_ptr() if kind == 2 else 0, M, N, K,
+                      0 if bias is None else bias.data_ptr(), ops.ACT[act], 0 if residual is None else residual.data_ptr(),
+                      0 if residual is None else residual.stride(0), *rargs, torch.cuda.current_stream().cuda_stream)
+    assert rc == 0
+    torch.cuda.synchronize()
+    bits = buf.view(ibits).cpu()
+    outside = torch.ones(bits.shape, dtype=torch.bool)
+    outside[:M, :N] = False
+    assert bool((bits[outside] == sentinel).all()), "cells outside the output were written"
+    if kind == 2:
+        sb = sbuf.cpu()
+        assert torch.isnan(sb[M]).all(), "scales past row M were written"
+        return buf[:M, :N].cpu(), sb[:M]
+    return buf[:M, :N].cpu()
+
+
+def e4m3_values(R, K, g):
+    q = (torch.randn(R, K, generator=g) * 64).clamp(-448, 448).to(E4M3)
+    q[:, ::BLOCK] = torch.tensor(448.0).to(E4M3)
+    return q
+
+
+def _bound(absprod, acc, K, bias):
+    return (EPS_INNER + GAMMA * (K // BLOCK + 2) * U) * absprod + 4 * U * (acc.abs() + bias.abs())
+
+
+def _check(section, got, ref, bound, what):
+    err = (got.double() - ref).abs()
+    bad = ~(err <= bound)
+    if int(bad.sum()):
+        idx = tuple(bad.nonzero()[0].tolist())
+        raise AssertionError(f"{what}: {int(bad.sum())} of {err.numel()} outside the bound ({int(torch.isnan(got).sum())} NaN); first "
+                             f"at {idx}: got {got[idx].item():.6g}, ref {ref[idx].item():.6g}, bound {bound[idx].item():.3g}")
+    _WORST[section + " err/bound"] = max(_WORST.get(section + " err/bound", 0.0), (err / bound).max().item())
+
+
+def _gelu64(x):
+    return 0.5 * x * (1 + torch.erf(x / math.sqrt(2)))
+
+
+EPS_GELU = 3e-7          # es3_gelu_fast's own error per |x| (test_gemm_epilogue_gpu.py)
+
+
+@pytest.mark.parametrize("M,N,K,spread,strided", [(77, 128, 128, True, False), (300, 1024, 1024, True, True),
+                                                  (1029, 3072, 1024, False, False), (257, 1024, 4736, False, True),
+                                                  (5184, 1024, 4736, True, False)])
+def test_gemm_fp8_residual_f32(cuda, M, N, K, spread, strided):
+    """proj / fc2: bias + fp32 residual -> fp32, and the same without residual; M not a multiple of 128."""
+    from efficientsam3_b200 import ops
+    g = _gen("res", M, N, K, spread, strided)
+    qa, sa, qw, sw, a64, w64 = _operands(cuda, M, N, K, spread, strided, g)
+    bias = torch.randn(N, generator=g)
+    res = torch.randn(M, N, generator=g) * 4
+    acc = a64 @ w64.t()
+    absprod = a64.abs() @ w64.abs().t()
+    bound = _bound(absprod, acc, K, bias.double())
+    for r in (res, None):
+        got = _run(cuda, qa, sa, qw, sw, bias.to(cuda), residual=None if r is None else r.to(cuda))
+        ref = acc + bias.double() + (0 if r is None else r.double())
+        b = bound + 4 * U * ((0 if r is None else r.double().abs()) + ref.abs())
+        _check("f32", got, ref, b, f"fp32 M{M} N{N} K{K} spread={spread} strided={strided} res={r is not None}")
+        _WORST["err / absprod"] = max(_WORST.get("err / absprod", 0.0), ((got.double() - ref).abs() / absprod.clamp_min(1e-30)).max().item())
+
+
+@pytest.mark.parametrize("win,M_img", [(24, 2), (0, 1)])
+def test_gemm_fp8_rope_bf16(cuda, win, M_img):
+    """qkv: bias + 2-D axial RoPE on q | k -> bf16 at the teacher's geometry (72 x 72 tokens, C = 1024), windowed and global;
+    v columns unrotated."""
+    from efficientsam3_b200 import ops
+    from efficientsam3_b200.model.vitdet import compute_axial_cis
+    H = W = 72
+    C = 1024
+    M, N, K = M_img * H * W, 3 * C, C
+    g = _gen("rope", win)
+    qa, sa, qw, sw, a64, w64 = _operands(cuda, M, N, K, True, False, g)
+    bias = torch.randn(N, generator=g)
+    cis = compute_axial_cis(64, win, win) if win else compute_axial_cis(64, H, W, scale_pos=24 / H)
+    tab = torch.view_as_real(cis).float().contiguous()
+    got = _run(cuda, qa, sa, qw, sw, bias.to(cuda), out=torch.bfloat16, rope=(tab.to(cuda), 2 * C, H, W, win))
+    acc = a64 @ w64.t()
+    x = acc + bias.double()
+    xb = _bound(a64.abs() @ w64.abs().t(), acc, K, bias.double()) + 4 * U * x.abs()
+    t = torch.arange(M) % (H * W)
+    pidx = (t // W % win) * win + (t % W % win) if win else t
+    cs = tab.double()[pidx]
+    c, s = cs[..., 0].repeat(1, 2 * C // 64), cs[..., 1].repeat(1, 2 * C // 64)
+    x0, x1 = x[:, 0:2 * C:2], x[:, 1:2 * C:2]
+    b0, b1 = xb[:, 0:2 * C:2], xb[:, 1:2 * C:2]
+    ref, bound = x.clone(), xb.clone()
+    ref[:, 0:2 * C:2], ref[:, 1:2 * C:2] = x0 * c - x1 * s, x0 * s + x1 * c
+    bound[:, 0:2 * C:2] = c.abs() * b0 + s.abs() * b1 + 4 * U * (x0.abs() * c.abs() + x1.abs() * s.abs())
+    bound[:, 1:2 * C:2] = c.abs() * b1 + s.abs() * b0 + 4 * U * (x0.abs() * s.abs() + x1.abs() * c.abs())
+    bound = bound * (1 + 2.0 ** -8) + 2.0 ** -8 * ref.abs()
+    _check("bf16 rope", got, ref, bound, f"rope win={win}")
+
+
+@pytest.mark.parametrize("M,N,K", [(77, 128, 128), (1029, 4736, 1024), (300, 1024, 4736)])
+def test_gemm_fp8_gelu_e4m3(cuda, M, N, K):
+    """fc1: bias + GELU(erf).  The fp32 epilogue is checked against fp64; the e4m3 epilogue's codes and per-row / 128-column
+    scales must equal the emulation's quantisation of that fp32 result, except where a value lies within one fp32 ulp of an
+    e4m3 rounding boundary (none is expected: both epilogues run the same arithmetic)."""
+    from efficientsam3_b200 import ops
+    g = _gen("gelu", M, N, K)
+    qa, sa, qw, sw, a64, w64 = _operands(cuda, M, N, K, True, False, g)
+    bias = torch.randn(N, generator=g)
+    f32 = _run(cuda, qa, sa, qw, sw, bias.to(cuda), act="gelu")
+    acc = a64 @ w64.t()
+    pre = acc + bias.double()
+    ref = _gelu64(pre)
+    bound = 1.13 * (_bound(a64.abs() @ w64.abs().t(), acc, K, bias.double()) + EPS_GELU * pre.abs()) + 4 * U * ref.abs()
+    _check("f32 gelu", f32, ref, bound, f"gelu fp32 M{M} N{N} K{K}")
+
+    q, s = _run(cuda, qa, sa, qw, sw, bias.to(cuda), out=E4M3, act="gelu")
+    wq, ws = quantize_rows(f32)
+    near = torch.zeros(M, N, dtype=torch.bool)
+    for d in (float("inf"), float("-inf")):
+        nq, _ = quantize_rows(torch.nextafter(f32, torch.tensor(d)))
+        near |= _u8(nq) != _u8(wq)
+    assert torch.equal(s.cpu().view(torch.int32), ws.view(torch.int32)), "fc1 e4m3 scales differ from the quantised fp32 result"
+    diff = (_u8(q.cpu()) != _u8(wq)) & ~near
+    assert not diff.any(), f"fc1 e4m3 codes: {int(diff.sum())} differ away from a rounding boundary"
+    assert int(((_u8(q.cpu()) != _u8(wq))).sum()) <= int(near.sum())
+
+
+def test_gemm_fp8_fc2_reads_fc1_output(cuda):
+    """fc1 -> fc2 as the teacher chains them: fc2's A operand is fc1's e4m3 output and scales, straight from HBM."""
+    from efficientsam3_b200 import ops
+    M, C, Hd = 300, 1024, 4736
+    g = _gen("chain")
+    qa, sa, qw1, sw1, _, _ = _operands(cuda, M, Hd, C, True, False, g)
+    qw2, sw2 = ops.pack_weight_e4m3((torch.randn(C, Hd, generator=g) / math.sqrt(Hd)).to(cuda))
+    b1, b2 = torch.randn(Hd, generator=g).to(cuda), torch.randn(C, generator=g).to(cuda)
+    h, hs = ops.gemm_fp8(qa, sa, qw1, sw1, b1, act="gelu", out_dtype=E4M3)
+    got = ops.gemm_fp8(h, hs, qw2, sw2, b2, out_dtype=torch.float32).cpu()
+    a64, w64 = dequant_rows(h.cpu(), hs.cpu()).double(), dequant_weight(qw2.cpu(), sw2.cpu()).double()
+    acc = a64 @ w64.t()
+    ref = acc + b2.cpu().double()
+    _check("f32", got, ref, _bound(a64.abs() @ w64.abs().t(), acc, Hd, b2.cpu().double()) + 4 * U * ref.abs(), "fc1 -> fc2")
+
+
+# ---------------------------------------------------------------------------------------------- the teacher end to end
+def _teacher(over, seed, cuda):
+    from efficientsam3_b200.stage1.model import SAM3ImageTeacherEncoder
+    from oracle.weights import fill_state_dict
+    t = SAM3ImageTeacherEncoder(embed_size=72, vit_overrides=over)
+    vit = t.sam3.backbone.vision_backbone.trunk
+    sd = {k: v for k, v in fill_state_dict(vit.state_dict(), seed).items() if not v.is_complex()}
+    vit.load_state_dict(sd, strict=False)
+    return t.to(cuda), sd
+
+
+def test_fp8_teacher_geometry_vs_oracle(cuda):
+    """Full-width teacher geometry (1008 px, 72 x 72 tokens, 24-windows + one global block, dim 1024, 16 heads, depth 3,
+    re-randomised weights) with the FP8 linears, against the fp32 CPU oracle: minimum per-token cosine >= 0.99 and rel-L2 <= 5e-2
+    (from e4m3's 2^-4 relative rounding), mean per-token cosine >= 0.998.
+
+    Measured on an H100 80GB HBM3 (700 W): FP8 mean cosine 0.998905, minimum 0.998616, rel-L2 4.68e-2; the bf16 path on the same
+    input 0.999994 / 0.999991 / 3.56e-3.  The mean-cosine threshold is 0.998, not 0.999: for errors spread evenly over the tokens
+    cosine = 1 - rel^2 / 2, so rel-L2 at its 5e-2 limit means a mean cosine of 0.99875, and 0.999 would demand rel-L2 <= 4.47e-2.
+    The bf16 path's figures on the same input are printed."""
+    from efficientsam3_b200.model.vitdet import SAM3_VIT_KWARGS
+    from oracle import vitdet as O
+    over = dict(depth=3, global_att_blocks=(2,))
+    t, sd = _teacher(over, 35, cuda)
+    x = torch.randn(1, 3, 1008, 1008, generator=_gen("teacher"))
+    with torch.no_grad():
+        ref = O.vit_trunk(sd, "", x, dict(SAM3_VIT_KWARGS, **over))
+    bf = t(x.to(cuda)).cpu()
+    out = t.enable_fp8()(x.to(cuda)).cpu()
+    tok = lambda y: y.double().flatten(2).transpose(1, 2).reshape(-1, y.shape[1])
+    def stats(y):
+        a, b = tok(y), tok(ref)
+        cos = (a * b).sum(1) / (a.norm(dim=1) * b.norm(dim=1))
+        return cos.mean().item(), cos.min().item(), rel_l2(y, ref)
+    c8, b16 = stats(out), stats(bf)
+    print(f"\nteacher depth 3 vs oracle: fp8 cos mean {c8[0]:.6f} min {c8[1]:.6f} rel-L2 {c8[2]:.3e}; "
+          f"bf16 cos mean {b16[0]:.6f} min {b16[1]:.6f} rel-L2 {b16[2]:.3e}")
+    assert out.shape == ref.shape and torch.isfinite(out).all()
+    assert c8[0] >= 0.998 and c8[1] >= 0.99 and c8[2] <= 5e-2, c8
+
+
+# ---------------------------------------------------------------------------------------------- consumers
+SMALL = dict(img_size=336, depth=2, global_att_blocks=(1,))      # 24 x 24 tokens: one window and one global block
+
+
+def test_switch_off_is_bit_identical_and_parameters_repack(cuda):
+    from efficientsam3_b200.stage1.model import SAM3ImageTeacherEncoder
+    t, _ = _teacher(SMALL, 7, cuda)
+    t.embed_size = 24
+    x = torch.randn(2, 3, 336, 336, generator=_gen("sw")).to(cuda)
+    base = t(x)
+    f8 = t.enable_fp8()(x)
+    assert not torch.equal(f8, base) and cosine(f8.cpu(), base.cpu()) > 0.999
+    assert torch.equal(t.enable_fp8(False)(x), base), "switching FP8 off must reproduce the bf16 output bit for bit"
+    fresh = SAM3ImageTeacherEncoder(embed_size=24, vit_overrides=SMALL).to(cuda)
+    fresh.load_state_dict(t.state_dict())
+    assert torch.equal(fresh(x), base)
+
+    t.enable_fp8()
+    assert torch.equal(t(x), f8)
+    vit = t.sam3.backbone.vision_backbone.trunk
+    with torch.no_grad():
+        vit.blocks[0].mlp.fc1.weight[:128, :128] *= 4             # one 128 x 128 block: its scale must change
+    moved = t(x)
+    fresh.load_state_dict(t.state_dict())
+    assert not torch.equal(moved, f8)
+    assert torch.equal(fresh.enable_fp8()(x), moved), "a parameter change under the switch must repack the e4m3 weights"
+
+
+def test_strict_precision_ignores_fp8(cuda):
+    from efficientsam3_b200 import ops
+    t, _ = _teacher(SMALL, 8, cuda)
+    t.embed_size = 24
+    x = torch.randn(1, 3, 336, 336, generator=_gen("strict")).to(cuda)
+    with ops.strict_precision():
+        a = t(x)
+        b = t.enable_fp8()(x)
+    assert torch.equal(a, b)
+
+
+def test_embedding_dump_with_fp8_teacher(cuda, tmp_path):
+    """save_embeddings_one_epoch with an FP8 teacher writes records of the unchanged format: fp16 [1024, E, E], equal to the FP8
+    teacher's own output rounded to fp16."""
+    import numpy as np
+    from efficientsam3_b200.stage1 import embeddings as E
+    t, _ = _teacher(dict(depth=1, global_att_blocks=()), 9, cuda)
+    t.enable_fp8()
+    xs = [torch.randn(2, 3, 1008, 1008, generator=_gen("dump", b)) for b in range(2)]
+    keys = [[f"img_{b}_{i}" for i in range(2)] for b in range(2)]
+    loader = [((list(x), None), (keys[b], np.array([b, b + 10], dtype=np.int32))) for b, x in enumerate(xs)]
+    path = str(tmp_path / "emb")
+    assert E.save_embeddings_one_epoch(t, loader, path, rank=0) == 4
+    rd = E.EmbeddingStoreReader(path, E.item_size(1024, 72 * 72), 0)
+    for b, x in enumerate(xs):
+        want = t(x.to(cuda)).half().cpu().numpy()
+        for i in range(2):
+            seed, emb = rd.read_embedding(keys[b][i], (1024, 72, 72))
+            assert seed == [b, b + 10][i] and emb.dtype == np.float16
+            assert np.array_equal(emb, want[i])
+
+
+def test_online_kd_step_with_fp8_teacher(cuda):
+    from types import SimpleNamespace as NS
+    from efficientsam3_b200.stage1.losses import kd_train_step_online
+    from efficientsam3_b200.stage1.model import build_image_student_model
+    from efficientsam3_b200.stage1.optim import FlatAdamW
+    t, _ = _teacher(dict(depth=1, global_att_blocks=()), 11, cuda)
+    t.enable_fp8()
+    cfg = NS(MODEL=NS(BACKBONE="efficientvit_b1"), DATA=NS(IMG_SIZE=1008), DISTILL=NS(EMBED_DIM=1024, EMBED_SIZE=72))
+    m = build_image_student_model(cfg).to(cuda).train()
+    opt = FlatAdamW(m, lr=1e-4, weight_decay=0.01)
+    x = torch.randn(2, 3, 1008, 1008, generator=_gen("kd")).to(cuda)
+    sizes = [(3, 1008, 756), (3, 672, 1008)]
+    losses = [float(kd_train_step_online(m, t, opt, x, sizes, 1.0, 5.0).item()) for _ in range(2)]
+    assert all(math.isfinite(v) for v in losses), losses

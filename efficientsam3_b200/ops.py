@@ -199,7 +199,8 @@ def gemm_simt(a, w, *, scale=None, bias=None, act=None, residual=None, out=None,
     if residual is not None:
         _chk_any(residual, _BF16_F32, "residual")
     _ensure_init(a)
-    assert a.dim() == 2 and w.dim() == 2 and a.stride(1) == 1 and w.stride(1) == 1
+    # a single column has no column stride: x.t().contiguous() of a [1, C] tensor is a [C, 1] view of column stride C (SE backward, B = 1)
+    assert a.dim() == 2 and w.dim() == 2 and (a.stride(1) == 1 or a.shape[1] == 1) and (w.stride(1) == 1 or w.shape[1] == 1)
     M, K = a.shape
     N = w.shape[0]
     if out is None:

@@ -17,85 +17,33 @@ Output buffers are prefilled with NaN: every cell inside the output region must 
 outside it -- the rest of a wider buffer, or a tail past the end -- must keep its sentinel bits.  Strided operands are slices of
 NaN-padded buffers, so a read outside the slice also shows.
 
-GAMMA = 2 and the eps_act below were set from one run on an H100 80GB HBM3 (700 W power limit).  Measured maximum err/bound per
+GAMMA = 2 and the eps_act of tests/bounds.py were set from one run on an H100 80GB HBM3 (700 W power limit).  Measured maximum err/bound per
 section, fp32 outputs: (a) epilogue matrix 0.18, (c) act/residual order 0.021, (d) RoPE 0.0037, (e) conv3x3 0.019,
 (f) convt2x2 0.025, (g) gemm_simt 0.054, so the fp32 accumulation stays well inside 2 K u.  bf16 outputs: 0.87 ... 0.996 in
 every section (pw_small 0.995), because the half-step of the output rounding dominates their bound and is reached.
 (b) reaches 1.0 of its half-step tolerance by construction: the residual sits at a bf16 midpoint.
 """
-import itertools
 import math
-import random
-import zlib
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+from bounds import (L_ACT, U, _INT, _act64, _assert_untouched, _bf, _check, _eps_act, _flat_out, _gen, _matrix_out, _padded,
+                    _pairwise, report_worst, WORST)
+
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24
 GAMMA = 2.0                    # gamma_K = GAMMA * K * u
-L_ACT = {None: 1.0, "relu": 1.0, "hswish": 1.5, "gelu": 1.13, "sigmoid": 0.25}
-EPS_GELU = 3e-7                # es3_gelu_fast: 0.5 |x| * (1.5e-7 erf approximation + a few ulp of MUFU rcp / ex2), per |x|
-EPS_SIGMOID = 1e-6             # 1 / (1 + __expf(-x)): __expf is within (2 + 1.16 |x|) ulp; sigmoid' <= 1/4
-TAIL = 256                     # sentinel cells past the end of a flat output buffer
-_INT = {torch.bfloat16: torch.int16, torch.float32: torch.int32}
-_WORST: dict = {}              # section -> max err/bound over the run
+_report_worst = report_worst("gemm epilogue")
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _report_worst():
-    yield
-    for k in sorted(_WORST):
-        print(f"\ngemm epilogue, section {k}: max err/bound = {_WORST[k]:.3g}", end="")
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
 
 
-def _pairwise(factors: dict, seed: int = 0) -> list:
-    """Rows of a strength-2 covering design: every value pair of every two factors appears in some row (greedy)."""
-    names = list(factors)
-    sizes = [len(factors[n]) for n in names]
-    nf = len(names)
-    todo = {(i, a, j, b) for i, j in itertools.combinations(range(nf), 2) for a in range(sizes[i]) for b in range(sizes[j])}
-    rng = random.Random(seed)
-    rows = []
-
-    def key(k, v, m, u):
-        return (k, v, m, u) if k < m else (m, u, k, v)
-
-    while todo:
-        i, a, j, b = min(todo)
-        row = {i: a, j: b}
-        for k in range(nf):
-            if k in row:
-                continue
-            gains = [sum(key(k, v, m, u) in todo for m, u in row.items()) for v in range(sizes[k])]
-            row[k] = rng.choice([v for v in range(sizes[k]) if gains[v] == max(gains)])
-        todo -= {(p, row[p], q, row[q]) for p, q in itertools.combinations(range(nf), 2)}
-        rows.append(tuple(factors[names[k]][row[k]] for k in range(nf)))
-    return rows
-
-
-def _bf(t):
-    return t.to(torch.bfloat16)
-
-
-def _gen(cuda, *key):
-    return torch.Generator(device=cuda).manual_seed(zlib.crc32(repr(key).encode()))
-
-
-def _act64(x, act):
-    if act is None:
-        return x
-    return {"relu": F.relu, "hswish": F.hardswish, "gelu": F.gelu, "sigmoid": torch.sigmoid}[act](x)
-
-
-def _eps_act(x, act):
-    if act == "gelu":
-        return EPS_GELU * x.abs()
-    if act == "sigmoid":
-        return EPS_SIGMOID * (1.0 + x.abs())
-    return 0.0
+def _ptr(t):
+    return 0 if t is None else t.data_ptr()
 
 
 def _expect(acc, absprod, K, act=None, scale=None, bias=None, res=None, after=False, out_bf16=False):
@@ -122,63 +70,6 @@ def _expect(acc, absprod, K, act=None, scale=None, bias=None, res=None, after=Fa
     if out_bf16:
         bound = bound * (1 + 2.0 ** -8) + 2.0 ** -8 * ref.abs()
     return ref, bound
-
-
-def _check(section, got, ref, bound, what):
-    err = (got.double() - ref).abs()
-    bad = ~(err <= bound)                   # NaN (a cell never written) is outside any bound
-    nbad = int(bad.sum())
-    if nbad:
-        idx = tuple(bad.nonzero()[0].tolist())
-        raise AssertionError(f"{what}: {nbad} of {err.numel()} elements outside their bound ({int(torch.isnan(got).sum())} unwritten); "
-                             f"first at {idx}: got {got[idx].item():.6g}, ref {ref[idx].item():.6g}, bound {bound[idx].item():.3g}")
-    _WORST[section] = max(_WORST.get(section, 0.0), (err / bound).max().item())
-
-
-def _sentinel(dtype):
-    return torch.full((1,), float("nan"), dtype=dtype).view(_INT[dtype]).item()
-
-
-def _assert_untouched(buf, inside, what):
-    bits = buf.view(_INT[buf.dtype])[~inside]
-    changed = int((bits != _sentinel(buf.dtype)).sum())
-    assert changed == 0, f"{what}: {changed} cells outside the output region were written"
-
-
-def _flat_out(n, dtype, cuda):
-    """A NaN-filled flat buffer of n + TAIL cells; returns (buffer, inside-mask)."""
-    buf = torch.full((n + TAIL,), float("nan"), dtype=dtype, device=cuda)
-    inside = torch.zeros(n + TAIL, dtype=torch.bool, device=cuda)
-    inside[:n] = True
-    return buf, inside
-
-
-def _matrix_out(M, N, dtype, strided, cuda):
-    """(buffer, [M, N] view, inside-mask): `strided` puts the view at column 8 of a [M + 2, N + 24] buffer."""
-    if not strided:
-        buf, inside = _flat_out(M * N, dtype, cuda)
-        return buf, buf[:M * N].view(M, N), inside
-    buf = torch.full((M + 2, N + 24), float("nan"), dtype=dtype, device=cuda)
-    inside = torch.zeros(buf.shape, dtype=torch.bool, device=cuda)
-    inside[:M, 8:8 + N] = True
-    return buf, buf[:M, 8:8 + N], inside
-
-
-def _padded(t, strided):
-    """`t` itself, or the same values as a column-8 slice of a NaN-padded buffer 16 columns wider (row stride != width)."""
-    if not strided:
-        return t.contiguous()
-    big = torch.full((t.shape[0], t.shape[1] + 16), float("nan"), dtype=t.dtype, device=t.device)
-    big[:, 8:8 + t.shape[1]] = t
-    return big[:, 8:8 + t.shape[1]]
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _ptr(t):
-    return 0 if t is None else t.data_ptr()
 
 
 # ---------------------------------------------------------------------------------------------- (a) es3_gemm_bf16_ex epilogue
@@ -274,7 +165,7 @@ def test_fp32_residual_keeps_precision(cuda, bn, N, out):
     err = (o.double() - ref).abs()
     assert not torch.isnan(o).any(), "unwritten output cells"
     assert err.max().item() <= tol, f"bn={bn} N={N} {out}: max |err| {err.max().item():.4g} > {tol}"
-    _WORST["b"] = max(_WORST.get("b", 0.0), err.max().item() / tol)
+    WORST["b"] = max(WORST.get("b", 0.0), err.max().item() / tol)
     _assert_untouched(buf, inside, f"fp32 residual bn={bn} N={N}")
 
 

@@ -141,6 +141,8 @@ SIGNATURES: dict[str, list] = {
     "es3_quantize_bf16_e4m3": [_vp, _ll, _vp, _vp, _ll, _i, _vp],
     "es3_pack_weight_e4m3": [_vp, _i, _vp, _vp, _i, _i, _vp],
     "es3_layernorm_f32_e4m3": [_vp, _vp, _vp, _f, _vp, _vp, _ll, _i, _vp],
+    # opt-in FP8 attention of the ViT teacher (attention_fp8.cu)
+    "es3_attention_fp8": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
 }
 
 # workspace-size helpers: name -> argtypes, restype long long
@@ -155,6 +157,7 @@ SIZE_HELPERS: dict[str, list] = {
     "es3_repmixer_bwd_ws_floats": [_i, _i],
     "es3_repmixer_bn_ws_floats": [_i, _i],
     "es3_colsum_f32_ws_floats": [_ll, _i],
+    "es3_attention_fp8_ws_floats": [_i, _i, _i, _i, _i],
     "es3_wgrad_tc_ws_floats": [_ll, _i, _i],
     "es3_litemla_attn_f32_ws_floats": [_i, _i, _i, _i],
     "es3_stem_wgrad_ws_floats": [_i, _i, _i, _i],

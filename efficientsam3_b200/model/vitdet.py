@@ -16,6 +16,7 @@ ViT.enable_fp8() (off by default; the strict precision mode ignores it) moves th
 (gemm_fp8.cu): norm1 / norm2 write e4m3 (es3_layernorm_f32_e4m3), the attention output is quantised (es3_quantize_bf16_e4m3),
 fc1's epilogue writes fc2's e4m3 operand, and the weights are packed once per parameter version (es3_pack_weight_e4m3).  Patch
 embedding, the LayerNorm statistics, RoPE, attention and the fp32 residual stream stay as above.
+ViT.enable_fp8(attention=True) moves attention to e4m3 as well (es3_attention_fp8: Q, K, V and P quantised on the device).
 """
 from __future__ import annotations
 
@@ -144,11 +145,16 @@ class ViT(nn.Module, NativePlanMixin):
                     nn.init.constant_(m.bias, 0)
 
     _fp8 = False
+    _fp8_attn = False
 
-    def enable_fp8(self, enabled: bool = True):
+    def enable_fp8(self, enabled: bool = True, attention: bool = False):
         """Run qkv, proj, fc1 and fc2 as block-scaled e4m3 GEMMs (off by default; ignored in the strict precision mode).  The
-        weights are packed to e4m3 on the next forward and again whenever a parameter changes.  Returns self."""
+        weights are packed to e4m3 on the next forward and again whenever a parameter changes.  attention=True also runs every
+        block's attention as FP8 flash attention (ops.attention_fp8); it needs enabled=True.  Returns self."""
+        if attention and not enabled:
+            raise ValueError("enable_fp8: attention=True needs the FP8 linear layers (enabled=True)")
         self._fp8 = bool(enabled)
+        self._fp8_attn = bool(attention)
         self._plan_key = None
         return self
 
@@ -198,7 +204,8 @@ class ViT(nn.Module, NativePlanMixin):
             for bp in p["blocks"]:
                 q, s = ops.layernorm_e4m3(xs, *bp["n1"])
                 qkv = ops.gemm_fp8(q, s, *bp["qkv8"], rope=(bp["rope"], 2 * C, h, w, bp["win"]))
-                a = ops.attention(qkv, B, h, w, C, heads, bp["win"], bp["scale"])
+                attn = ops.attention_fp8 if self._fp8_attn else ops.attention
+                a = attn(qkv, B, h, w, C, heads, bp["win"], bp["scale"])
                 xs = ops.gemm_fp8(*ops.quantize_e4m3(a), *bp["proj8"], residual=xs, out_dtype=torch.float32)
                 q, s = ops.layernorm_e4m3(xs, *bp["n2"])
                 q, s = ops.gemm_fp8(q, s, *bp["fc1_8"], act="gelu", out_dtype=ops.E4M3)

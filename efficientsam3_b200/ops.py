@@ -5,6 +5,8 @@ dtype / contiguity and raises (no CPU fallback -- a CPU tensor is an error, SURV
 """
 from __future__ import annotations
 
+import math
+
 import torch
 
 from . import _lib
@@ -47,7 +49,7 @@ class strict_precision:
 
 # ------------------------------------------------------------------------------------ accounting
 # kernels launched per C-ABI call (memsets excluded) -- bench.py reports the sum as `gpu_launches`.
-KERNELS_PER_CALL = {"es3_colsum_f32": 2, "es3_layernorm_bwd": 2, "es3_litemla_attn_generic": 2, "es3_fill_small_components": 4, "es3_grad_norm": 2, "es3_adamw_flat": 2, "es3_litemla_attn_tc": 2, "es3_kd_loss_fwd": 2, "es3_channel_mean": 2}
+KERNELS_PER_CALL = {"es3_colsum_f32": 2, "es3_layernorm_bwd": 2, "es3_litemla_attn_generic": 2, "es3_fill_small_components": 4, "es3_grad_norm": 2, "es3_adamw_flat": 2, "es3_litemla_attn_tc": 2, "es3_kd_loss_fwd": 2, "es3_channel_mean": 2, "es3_attention_fp8": 2}
 launch_count = 0
 
 
@@ -1033,6 +1035,28 @@ def pack_weight_e4m3(w):
     _call("es3_pack_weight_e4m3", "pack_weight_e4m3", _nb(w, q, s), 2 * N * K, w.data_ptr(), int(w.dtype == torch.float32),
           q.data_ptr(), s.data_ptr(), N, K, _stream())
     return q, s
+
+
+def attention_fp8(qkv, B, H, W, C, num_heads, win, scale):
+    """FP8 flash attention with the contract of attention(): qkv [B*H*W, 3C] bf16 -> [B*H*W, C] bf16, head_dim 64, win = 0
+    (global) or a window that divides H and W, scale > 0.  Q, K, V and P are quantised to e4m3 on the device with power-of-two
+    block scales (attention_fp8.cu: a pre-pass quantises K and V once per key tile into a workspace allocated here).  Shapes, dtypes
+    and the scale are checked here and raise ValueError before anything launches."""
+    _fp8_fail(torch.is_tensor(qkv) and qkv.dtype == torch.bfloat16, "attention_fp8: qkv must be a bf16 tensor")
+    _fp8_fail(qkv.is_contiguous(), "attention_fp8: qkv must be contiguous")
+    _fp8_fail(min(B, H, W, C, num_heads) > 0 and win >= 0, f"attention_fp8: bad shape B={B} H={H} W={W} C={C} heads={num_heads}")
+    _fp8_fail(C == 64 * num_heads, f"attention_fp8: head_dim must be 64 (C={C}, num_heads={num_heads})")
+    _fp8_fail(win == 0 or (H % win == 0 and W % win == 0), f"attention_fp8: window {win} must divide H={H} and W={W}")
+    _fp8_fail(tuple(qkv.shape) == (B * H * W, 3 * C), f"attention_fp8: qkv must be [{B * H * W}, {3 * C}], got {tuple(qkv.shape)}")
+    _fp8_fail(math.isfinite(scale) and scale > 0, f"attention_fp8: scale must be positive and finite, got {scale}")
+    _fp8_cuda(qkv)
+    _ensure_init(qkv)
+    out = torch.empty((B * H * W, C), device=qkv.device, dtype=torch.bfloat16)
+    ws = _f32ws(_lib.size("es3_attention_fp8_ws_floats", B, H, W, num_heads, win), qkv.device)
+    L = win * win if win else H * W
+    _call("es3_attention_fp8", f"attention_fp8[L={L}]", _nb(qkv, out), 4 * B * H * W * L * C, qkv.data_ptr(), out.data_ptr(),
+          ws.data_ptr(), B, H, W, C, num_heads, win, float(scale), _stream())
+    return out
 
 
 _FP8_OUT = {torch.bfloat16: 0, torch.float32: 1, E4M3: 2}

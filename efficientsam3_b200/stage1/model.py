@@ -333,9 +333,10 @@ class SAM3ImageTeacherEncoder(nn.Module):
             feats, _ = ops.bilinear_nchw(feats, self.embed_size, self.embed_size)
         return feats
 
-    def enable_fp8(self, enabled: bool = True):
-        """Run the trunk's linear layers as block-scaled e4m3 GEMMs (ViT.enable_fp8; off by default).  Returns self."""
-        self.sam3.backbone.vision_backbone.trunk.enable_fp8(enabled)
+    def enable_fp8(self, enabled: bool = True, attention: bool = False):
+        """Run the trunk's linear layers as block-scaled e4m3 GEMMs, and with attention=True its attention as FP8 flash attention
+        too (ViT.enable_fp8; off by default).  Returns self."""
+        self.sam3.backbone.vision_backbone.trunk.enable_fp8(enabled, attention=attention)
         return self
 
 

@@ -193,6 +193,13 @@ int es3_pack_weight_e4m3(const void* w, int w_f32, void* q, float* scales, int N
 /* es3_layernorm_f32 (no pos add) writing e4m3 [M, C] + scales [M, C/128] instead of bf16 / fp32; C = 1024 or 2048. */
 int es3_layernorm_f32_e4m3(const float* x, const float* gamma, const float* beta, float eps, void* q, float* scales,
                            long long M, int C, void* stream);
+/* FP8 flash attention with the data contract of es3_attention_tc_bf16 (bf16 qkv in, bf16 out, head_dim 64, the window divides H
+ * and W; scale > 0): Q, K, V and P quantised to e4m3 on the device with power-of-two block scales (Q, K per token and head; V per
+ * key tile, head and channel; P as e4m3(p * 2^8)), QK^T and PV on e4m3 wgmma.  K and V are quantised once per key tile into ws
+ * (es3_attention_fp8_ws_floats floats, 16-byte aligned) by a pre-pass; the attention kernel reads them from there. */
+int es3_attention_fp8(const void* qkv, void* out, void* ws, int B, int H, int W, int C, int num_heads, int win, float scale,
+                      void* stream);
+long long es3_attention_fp8_ws_floats(int B, int H, int W, int num_heads, int win);
 
 /* ------------------------------------------------------------------------------------------ text encoders */
 /* Causal softmax attention, head_dim 64, over B sequences of L tokens on the fused qkv activation [B*L, 3C] bf16 ->

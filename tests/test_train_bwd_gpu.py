@@ -38,6 +38,7 @@ import torch
 import torch.nn.functional as F
 
 import ref_train_bwd as R
+from es3_recorder import STUDENTS, training_step_calls
 from bounds import (_INT, TAIL, _assert_untouched, _bf, _check, _flat_out, _gen, _pairwise, _sentinel, report_worst)
 
 pytestmark = pytest.mark.gpu
@@ -939,42 +940,9 @@ def covered_keys():
     return keys
 
 
-STUDENTS = ["efficientvit_b0", "efficientvit_b1", "efficientvit_b2", "repvit_m0_9", "repvit_m1_1", "repvit_m2_3", "tiny_vit_5m",
-            "tiny_vit_11m", "tiny_vit_21m"]
-
-
 def record_training_step(cuda, monkeypatch, name, frozen_bn, img=1024, embed=64, B=1):
     """The route keys of one native KD training step (forward, loss, backward) of `name`, from its es3_* calls."""
-    from types import SimpleNamespace as NS
-    from efficientsam3_b200 import _lib as L
-    from efficientsam3_b200.stage1.model import build_image_student_model
-    from efficientsam3_b200.stage1.optim import KDLossFunction
-    from oracle.weights import fill_state_dict
-    cfg = NS(MODEL=NS(BACKBONE=name), DATA=NS(IMG_SIZE=img), DISTILL=NS(EMBED_DIM=1024, EMBED_SIZE=embed))
-    m = build_image_student_model(cfg)
-    m.load_state_dict(fill_state_dict(m.state_dict(), 3))
-    m = m.to(cuda).train()
-    if frozen_bn:
-        for mod in m.modules():
-            if isinstance(mod, torch.nn.modules.batchnorm._BatchNorm):
-                mod.eval()
-    calls = []
-    real_call, real_rc = L.call, L.call_rc
-
-    def rc_rec(n, *a):
-        rc = real_rc(n, *a)
-        if rc == 0:
-            calls.append((n, a))
-        return rc
-    monkeypatch.setattr(L, "call", lambda n, *a: (calls.append((n, a)), real_call(n, *a))[1])
-    monkeypatch.setattr(L, "call_rc", rc_rec)
-    g = torch.Generator(device=cuda).manual_seed(0)
-    x = torch.randn(B, 3, img, img, device=cuda, generator=g)
-    teacher = torch.randn(B, 1024, embed, embed, device=cuda, generator=g)
-    sz = torch.tensor([[img, img]] * B, dtype=torch.int32, device=cuda)
-    KDLossFunction.apply(m(x), teacher, sz, img, 1.0).backward()
-    torch.cuda.synchronize()
-    monkeypatch.undo()
+    calls = training_step_calls(cuda, monkeypatch, name, frozen_bn, img, embed, B)
     return {k for k in (route_key(n, a) for n, a in calls) if k is not None}
 
 

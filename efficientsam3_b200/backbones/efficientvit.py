@@ -4,7 +4,9 @@ reference checkpoints load unchanged, but every forward runs on the hand-written
 
   input stem (conv 3x3 s2 + residual DSConv)         -> es3_stem_fused_c16 (b1; other widths: es3_stem_conv3x3_s2 + es3_dsconv_res_bf16)
   MBConv blocks, stages 1-2 and the stage openers    -> es3_mbconv_tc_bf16 / es3_mbconv_tc_s2_bf16 (wgmma, whole block on the SM)
-  MBConv blocks, stages 3-4                          -> es3_gemm_bf16 (expand) + es3_dwproj_tc_bf16 (depthwise + project + residual)
+  MBConv blocks 128->512->128 (b1 stage 3, b0 stage 4)
+    and the b1 stage-4 opener 128->512->256          -> es3_mbconv_tc_wide_bf16 (wgmma, whole block on the SM)
+  other MBConv blocks of stages 3-4                  -> es3_gemm_bf16 (expand) + es3_dwproj_tc_bf16 (depthwise + project + residual)
   LiteMLA (ops.py:521-671)                           -> es3_gemm_bf16 (qkv, proj) + es3_litemla_aggreg_dwpw + es3_litemla_attn_tc
   anything not instantiated                          -> es3_gemm_bf16 / es3_dwconv_tiled_bf16 / es3_mbconv_fused_bf16 (all native)
 

@@ -4,7 +4,7 @@
 // Why a second fused kernel: in mbconv_fused.cu all three contractions run on mma.sync, with every phase separated by
 // __syncthreads.  Here the two pointwise GEMMs are warpgroup MMAs (wgmma) from TMA-staged, 128B-swizzled operands:
 //
-//   TMA (4-D map, halo + zero fill)  ->  s_in  [10x18 px][64 ch]  128B-swizzled K-major A operand
+//   TMA (4-D map, halo + zero fill)  ->  s_in  CIN/64 slabs of [10x18 px][64 ch]  128B-swizzled K-major A operand
 //   per 64-channel chunk of the expanded tensor:
 //     expand   D_exp[192 x 64] = s_in (three 64-row blocks) x W1c^T             wgmma, SS, fp32 in registers
 //     epilogue BN1 + act (+ zero outside the image = the depthwise's padding) -> bf16 s_mid (pixel-major)
@@ -55,10 +55,13 @@ constexpr int MT_MC = 64;                                // expanded-channel chu
 constexpr int MT_RS_MID = MT_MC * 2 + 16;                // s_mid row stride (bytes)
 constexpr int MT_THREADS = 384;                          // two compute warpgroups + one TMA warpgroup
 
-template <int MID, int COUT>
+template <int CIN, int MID, int COUT, int MINB>
 struct MTSmem {
-  static constexpr int IN = 3 * 64 * 128;   // the three 64-row expand blocks (rows 180..191 are padding, never written by TMA)
-  static constexpr int W1 = 2 * MT_MC * 128;
+  static constexpr int SLABS = (CIN + 63) / 64;   // 64-channel K-slabs of the input tile and of a W1 chunk
+  static constexpr int IN_SLAB = 3 * 64 * 128;    // the three 64-row expand blocks (rows 180..191 are padding, never written by TMA)
+  static constexpr int IN = SLABS * IN_SLAB;
+  static constexpr int W1_SLAB = MT_MC * 128, W1_STAGE = SLABS * W1_SLAB;
+  static constexpr int W1 = 2 * W1_STAGE;
   static constexpr int W3 = 2 * COUT * 128;
   static constexpr int DW = 128 * 128;
   static constexpr int MIDB = (MT_PIN + 1) * MT_RS_MID;   // + row MT_PIN: scratch for the expand's padding rows, never read
@@ -67,7 +70,7 @@ struct MTSmem {
   static constexpr int OFF_PAR = OFF_WDW + 9 * MID * 2;              // fp32 s1[MID] b1[MID] b2[MID] s3[COUT] b3[COUT]
   static constexpr int OFF_BAR = OFF_PAR + (3 * MID + 2 * COUT) * 4;
   static constexpr int TOTAL = OFF_BAR + 128;   // 9 mbarriers
-  static_assert(IN >= MT_PIN * 128 && 2 * (TOTAL + 1024) <= 233472, "input tile / two CTAs per SM");
+  static_assert(IN_SLAB >= MT_PIN * 128 && MINB * (TOTAL + 1024) <= 233472, "input tile / MINB CTAs per SM");
 };
 
 struct MTArgs {
@@ -93,9 +96,10 @@ template <int CIN, int MID, int COUT, int ACT, int MINB>
 __global__ void __launch_bounds__(MT_THREADS, MINB)
 mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w1,
                  const __grid_constant__ CUtensorMap tm_w3, const MTArgs a) {
-  using L = MTSmem<MID, COUT>;
+  using L = MTSmem<CIN, MID, COUT, MINB>;
   constexpr int NC = MID / MT_MC;
-  static_assert(CIN == COUT && CIN % 16 == 0 && CIN <= 64 && MID % 64 == 0 && NC >= 2 && (COUT == 32 || COUT == 64), "shape");
+  static_assert(CIN == COUT && CIN % 16 == 0 && (CIN <= 64 || CIN % 64 == 0) && MID % 64 == 0 && NC >= 2 &&
+                (COUT == 32 || COUT == 64 || COUT == 128), "shape");
   // (no integer round trip on the pointer: the compiler must keep seeing shared-space addresses, or every access below
   //  turns into a generic LD/ST -- the first version of this kernel spent its time in long-scoreboard stalls on those)
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -141,16 +145,21 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
     // ------------------------------------------------------------------------------------ control: TMA (warp 8 lane 0)
     ptx::setmaxnreg_dec<MTRegs<MINB>::TMA>();
     if (warp == 8 && lane == 0 && my_tiles > 0) {
-      constexpr uint32_t W1_BYTES = MT_MC * 128, W3_BYTES = COUT * 128;
+      constexpr uint32_t W1_BYTES = L::W1_STAGE, W3_BYTES = COUT * 128;
+      // one box per 64-channel slab, all on the same barrier
       auto load_in = [&](int t) {
         const int bb = t / tiles_per_img, r = t % tiles_per_img;
-        ptx::mbar_arrive_expect_tx(bar_in, MT_PIN * 128);
-        ptx::tma_load_4d(&tm_in, bar_in, s_in, 0, (r % a.tiles_x) * MT_TW - 1, (r / a.tiles_x) * MT_TH - 1, bb);
+        ptx::mbar_arrive_expect_tx(bar_in, L::SLABS * MT_PIN * 128);
+#pragma unroll
+        for (int sl = 0; sl < L::SLABS; ++sl)
+          ptx::tma_load_4d(&tm_in, bar_in, s_in + sl * L::IN_SLAB, sl * 64, (r % a.tiles_x) * MT_TW - 1, (r / a.tiles_x) * MT_TH - 1, bb);
       };
       auto load_w1 = [&](int gc) {
         const int s = gc & 1;
         ptx::mbar_arrive_expect_tx(bar_w1 + s, W1_BYTES);
-        ptx::tma_load_2d(&tm_w1, bar_w1 + s, s_w1 + s * W1_BYTES, 0, (gc % NC) * MT_MC);
+#pragma unroll
+        for (int sl = 0; sl < L::SLABS; ++sl)
+          ptx::tma_load_2d(&tm_w1, bar_w1 + s, s_w1 + s * W1_BYTES + sl * L::W1_SLAB, sl * 64, (gc % NC) * MT_MC);
       };
       auto load_w3 = [&](int gc) {
         const int s = gc & 1;
@@ -175,7 +184,8 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
     }
   } else {
     // ------------------------------------------------------------------------------------ compute warps 0..7 (two warpgroups)
-    // warpgroup hsel: expand columns hsel*32 .. +32 of the chunk; project columns hsel*32 .. (COUT 64) or rows hsel*64 .. (COUT 32)
+    // warpgroup hsel: expand columns hsel*32 .. +32 of the chunk; project columns hsel*COUT/2 .. (COUT >= 64) or rows hsel*64 ..
+    // (COUT 32)
     ptx::setmaxnreg_inc<MTRegs<MINB>::MMA>();
     const int q = warp & 3, hsel = warp >> 2;            // warp inside the warpgroup; warpgroup = column half / m-tile parity (dw)
     const int g = lane >> 2, t4 = lane & 3;
@@ -183,10 +193,11 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
     const uint32_t u_mid = ptx::smem_u32(s_mid), u_in = ptx::smem_u32(s_in), u_dw = ptx::smem_u32(s_dw);
     const uint32_t dshift = (g & 1) ? 16u : 0u;
     const bool dvalid = (g >> 1) == t4;
-    constexpr uint32_t W1_BYTES = MT_MC * 128, W3_BYTES = COUT * 128;
-    constexpr int PRB = COUT == 64 ? 2 : 1;               // 64-row blocks of the project accumulator this warpgroup holds
-    const int prb0 = COUT == 64 ? 0 : hsel, pcol0 = COUT == 64 ? hsel * 32 : 0;
-    float proj[PRB][16];
+    constexpr uint32_t W1_BYTES = L::W1_STAGE, W3_BYTES = COUT * 128;
+    constexpr int PRB = COUT >= 64 ? 2 : 1;               // 64-row blocks of the project accumulator this warpgroup holds
+    constexpr int PN = COUT >= 64 ? COUT / 2 : 32;        // and its columns
+    const int prb0 = COUT >= 64 ? 0 : hsel, pcol0 = COUT >= 64 ? hsel * PN : 0;
+    float proj[PRB][PN / 2];
     int gc = 0;
     // descriptors of the operands' first K-step; every other one is a constant offset from these (ptx::desc_advance)
     const uint64_t d_in = ptx::make_desc_sw128(u_in), d_dw = ptx::make_desc_sw128(u_dw + prb0 * 8192);
@@ -232,9 +243,11 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         ptx::wg_fence();
 #pragma unroll
         for (int k = 0; k < CIN / 16; ++k) {
-          const uint64_t db = ptx::desc_advance(d_w1, st * W1_BYTES + k * 32);
+          const int sl = k / 4, kk = k % 4;                // K-slab and K-step inside it
+          const uint64_t db = ptx::desc_advance(d_w1, st * W1_BYTES + sl * L::W1_SLAB + kk * 32);
 #pragma unroll
-          for (int mb = 0; mb < 3; ++mb) ptx::wgmma_m64n32<0, 0>(ex[mb], ptx::desc_advance(d_in, mb * 8192 + k * 32), db, k != 0);
+          for (int mb = 0; mb < 3; ++mb)
+            ptx::wgmma_m64n32<0, 0>(ex[mb], ptx::desc_advance(d_in, sl * L::IN_SLAB + mb * 8192 + kk * 32), db, k != 0);
         }
         ptx::wg_commit();
         ptx::wg_wait<0>();                                 // also retires project(gc-1), still in flight unless c == 0
@@ -328,13 +341,15 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         for (int k = 0; k < MT_MC / 16; ++k) {
           const uint64_t db = ptx::desc_advance(d_w3, st * W3_BYTES + k * 32);
 #pragma unroll
-          for (int rb = 0; rb < PRB; ++rb)
-            ptx::wgmma_m64n32<0, 0>(proj[rb], ptx::desc_advance(d_dw, rb * 8192 + k * 32), db, (c | k) != 0);
+          for (int rb = 0; rb < PRB; ++rb) {
+            if constexpr (PN == 64) ptx::wgmma_m64n64<0, 0>(proj[rb], ptx::desc_advance(d_dw, rb * 8192 + k * 32), db, (c | k) != 0);
+            else ptx::wgmma_m64n32<0, 0>(proj[rb], ptx::desc_advance(d_dw, rb * 8192 + k * 32), db, (c | k) != 0);
+          }
         }
         ptx::wg_commit();                                // retired by the next chunk's expand wait, or below
       }
       ptx::wg_wait<0>();                                 // the tile's last project: the final epilogue reads the accumulators
-      ptx::wg_fence_regs<PRB * 16>(&proj[0][0]);
+      ptx::wg_fence_regs<PRB * PN / 2>(&proj[0][0]);
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(bar_w3free + ((gc - 1) & 1));
 
@@ -345,9 +360,9 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
         const long long tile0 = (((long long)b * a.H + oy0) * a.W + ox0) * COUT + pcol0 + 2 * t4;
         const bf16* xt = a.x + tile0;
         bf16* yt = a.y + tile0;
-        float2 s3[4], b3[4];
+        float2 s3[PN / 8], b3[PN / 8];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < PN / 8; ++j) {
           s3[j] = *reinterpret_cast<const float2*>(s_s3 + pcol0 + 8 * j + 2 * t4);
           b3[j] = *reinterpret_cast<const float2*>(s_b3 + pcol0 + 8 * j + 2 * t4);
         }
@@ -359,7 +374,7 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
             if (oy0 + ly < a.H && ox0 + lx < a.W) {
               const int off = (ly * a.W + lx) * COUT;
 #pragma unroll
-              for (int j = 0; j < 4; ++j) {
+              for (int j = 0; j < PN / 8; ++j) {
                 const float* p = &proj[rb][4 * j + 2 * h];
                 const float2 xr = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(xt + off + 8 * j)));
                 const float f0 = fmaf(p[0], s3[j].x, b3[j].x) + xr.x;
@@ -375,7 +390,7 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
 
 template <int CIN, int MID, int COUT, int MINB>
 static int launch_mbconv_tc(const void* x, void* y, const void* w1, const void* w3, const MTArgs& a, int B, cudaStream_t st) {
-  using L = MTSmem<MID, COUT>;
+  using L = MTSmem<CIN, MID, COUT, MINB>;
   CUtensorMap tm_in, tm_w1, tm_w3;
   {
     uint64_t dims[4] = {(uint64_t)CIN, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)B};
@@ -413,6 +428,19 @@ static int launch_mbconv_tc(const void* x, void* y, const void* w1, const void* 
   return 0;
 }
 
+static MTArgs mt_args(const void* x, void* y, const float* s1, const float* b1, const float* wdw, const float* b2, const float* s3,
+                      const float* b3, int B, int H, int W) {
+  MTArgs a;
+  a.x = (const bf16*)x; a.y = (bf16*)y; a.s1 = s1; a.b1 = b1; a.wdw = wdw; a.b2 = b2; a.s3 = s3; a.b3 = b3;
+  a.H = H; a.W = W; a.tiles_x = ceil_div(W, MT_TW); a.tiles_y = ceil_div(H, MT_TH);
+  a.total_tiles = B * a.tiles_x * a.tiles_y;
+  return a;
+}
+
+// mbconv_tc_s2.cu: the stride-2 kernel for (Cin, Mid, Cout) in {(16,64,32), (32,128,64), (64,256,128), (128,512,256)}
+int mbconv_tc_s2(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw, const float* b2,
+                 const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin, cudaStream_t st);
+
 }  // namespace es3
 
 using namespace es3;
@@ -425,13 +453,25 @@ extern "C" int es3_mbconv_tc_bf16(const void* x, void* y, const void* w1, const 
   if (!(stride == 1 && residual && act == ACT_HSWISH && Cin == Cout && Mid == 4 * Cin && (Cin == 32 || Cin == 64))) return -1;
   ES3_REQUIRE(B > 0 && H > 0 && W > 0, "es3_mbconv_tc_bf16: bad shape");
   ES3_REQUIRE((((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w3 | (uintptr_t)y) & 15) == 0, "es3_mbconv_tc_bf16: 16-byte alignment");
-  MTArgs a;
-  a.x = (const bf16*)x; a.y = (bf16*)y; a.s1 = s1; a.b1 = b1; a.wdw = wdw; a.b2 = b2; a.s3 = s3; a.b3 = b3;
-  a.H = H; a.W = W; a.tiles_x = ceil_div(W, MT_TW); a.tiles_y = ceil_div(H, MT_TH);
-  a.total_tiles = B * a.tiles_x * a.tiles_y;
+  const MTArgs a = mt_args(x, y, s1, b1, wdw, b2, s3, b3, B, H, W);
   cudaStream_t st = (cudaStream_t)stream;
   // (32, 128, 32) fits 104 registers and runs faster with a second CTA per SM to overlap its phases; (64, 256, 64) needs more
   // than 104 (it spills and ptxas serialises its wgmma) and runs at one CTA per SM
   if (Cin == 32) return launch_mbconv_tc<32, 128, 32, 2>(x, y, w1, w3, a, B, st);
   return launch_mbconv_tc<64, 256, 64, 1>(x, y, w1, w3, a, B, st);
+}
+
+// Same contract as es3_mbconv_fused_bf16 for the Cin-128 hardswish blocks: (128, 512, 128) stride 1 with residual (this file's
+// kernel with two 64-channel input slabs) and (128, 512, 256) stride 2 without (mbconv_tc_s2.cu), both at one CTA per SM.
+// Returns -1 (no error set) for any other shape.
+extern "C" int es3_mbconv_tc_wide_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
+                                       const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W,
+                                       int Cin, int Mid, int Cout, int stride, int residual, int act, void* stream) {
+  const bool s1_res = stride == 1 && residual && Cout == 128, s2_open = stride == 2 && !residual && Cout == 256;
+  if (!(act == ACT_HSWISH && Cin == 128 && Mid == 512 && (s1_res || s2_open))) return -1;
+  ES3_REQUIRE(B > 0 && H > 0 && W > 0, "es3_mbconv_tc_wide_bf16: bad shape");
+  ES3_REQUIRE((((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w3 | (uintptr_t)y) & 15) == 0, "es3_mbconv_tc_wide_bf16: 16-byte alignment");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (s2_open) return mbconv_tc_s2(x, y, w1, s1, b1, wdw, b2, w3, s3, b3, B, H, W, Cin, st);
+  return launch_mbconv_tc<128, 512, 128, 1>(x, y, w1, w3, mt_args(x, y, s1, b1, wdw, b2, s3, b3, B, H, W), B, st);
 }

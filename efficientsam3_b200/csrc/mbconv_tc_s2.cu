@@ -1,10 +1,10 @@
-// Fused stride-2 MBConv on wgmma (the stage-opening blocks 16->64->32 @512^2, 32->128->64 @256^2, 64->256->128 @128^2 of
-// efficientvit_b1: y = BN3(pw2(act(BN2(dw3x3_s2(act(BN1(pw1(x)))))))), no residual; reference efficientvit/nn/ops.py:315-367).
+// Fused stride-2 MBConv on wgmma (the stage-opening blocks 16->64->32 @512^2, 32->128->64 @256^2, 64->256->128 @128^2,
+// 128->512->256 @64^2 of efficientvit_b1: y = BN3(pw2(act(BN2(dw3x3_s2(act(BN1(pw1(x)))))))), no residual; reference efficientvit/nn/ops.py:315-367).
 // Same machinery as mbconv_tc.cu (TMA-staged swizzled input tile, wgmma expand into registers, BN+act epilogue into a
 // pixel-major smem tile, diagonal m16n8k8 depthwise into the swizzled A operand of the projecting wgmma that accumulates over
 // chunks), with the geometry of a stride-2 block: a 4 x 16 output tile needs a 9 x 33 input tile = 297 pixels = five 64-row
 // wgmma blocks, so the expanded tensor is processed in 32-channel chunks to keep its tile (297 x 32 bf16) at 24 KB and two
-// CTAs on an SM.  Project K-steps per chunk: 2 (32 channels); the W3 box still loads 64 K-columns (128-byte swizzled rows), the
+// CTAs on an SM (one at Cin 128, whose input tile is two 64-channel slabs).  Project K-steps per chunk: 2 (32 channels); the W3 box still loads 64 K-columns (128-byte swizzled rows), the
 // upper half is simply not referenced.
 #include <cuda.h>
 
@@ -46,13 +46,17 @@ constexpr int S2_ODD = 20, S2_PW = S2_ODD + S2_TW;           // slots per input 
 constexpr int S2_SCRATCH = 17;                              // unused slot 17 of input row 0: the expand's padding rows write it
 constexpr int S2_THREADS = 384;                           // two compute warpgroups + one TMA warpgroup
 
-template <int MID, int COUT, int WSTAGES>
+template <int CIN, int MID, int COUT, int WSTAGES, int MINB>
 struct S2Smem {
-  // 38912: the 297 input rows.  The expand reads five 64-row blocks (320 rows): rows 304..319 fall on the depthwise weights and
-  // per-channel parameters that follow, which are written once before the main loop and read-only after (a whole 320-row
-  // buffer would not leave room for two CTAs per SM at (64, 256, 128)).
-  static constexpr int IN = (S2_PIN * 128 + 1023) / 1024 * 1024;
-  static constexpr int W1 = 2 * S2_MC * 128;
+  // 38912 per 64-channel slab: the 297 input rows.  The expand reads five 64-row blocks (320 rows) of every slab: past the
+  // last slab, rows 304..319 fall on the depthwise weights and per-channel parameters that follow, which are written once
+  // before the main loop and read-only after (a whole 320-row buffer would not leave room for two CTAs per SM at
+  // (64, 256, 128)); past an earlier slab they fall on the next slab, which TMA writes only between tiles, as it does this one.
+  static constexpr int SLABS = (CIN + 63) / 64;
+  static constexpr int IN_SLAB = (S2_PIN * 128 + 1023) / 1024 * 1024;
+  static constexpr int IN = SLABS * IN_SLAB;
+  static constexpr int W1_SLAB = S2_MC * 128, W1_STAGE = SLABS * W1_SLAB;
+  static constexpr int W1 = 2 * W1_STAGE;
   static constexpr int W3_STAGE = COUT * 128;
   static constexpr int OFF_WDW = IN;                                   // bf16 [MID/32][9][32]
   static constexpr int OFF_PAR = OFF_WDW + 9 * MID * 2;
@@ -60,8 +64,8 @@ struct S2Smem {
   static constexpr int OFF_W1 = (OFF_BAR + 128 + 1023) / 1024 * 1024;
   static constexpr int OFF_W3 = OFF_W1 + W1, OFF_DW = OFF_W3 + WSTAGES * W3_STAGE, OFF_MID = OFF_DW + 128 * 128;
   static constexpr int TOTAL = OFF_MID + (S2_IH * S2_PW * S2_RS_MID + 15) / 16 * 16;
-  static_assert(5 * 64 * 128 <= OFF_BAR, "the padding rows of the A operand must fall on the read-only parameters");
-  static_assert(2 * (TOTAL + 1024) <= 233472, "two CTAs per SM");
+  static_assert((SLABS - 1) * IN_SLAB + 5 * 64 * 128 <= OFF_BAR, "the padding rows of the A operand must fall on the read-only parameters");
+  static_assert(MINB * (TOTAL + 1024) <= 233472, "MINB CTAs per SM");
 };
 
 struct S2Args {
@@ -85,9 +89,10 @@ template <int CIN, int MID, int COUT, int WSTAGES, int ACT, int MINB>
 __global__ void __launch_bounds__(S2_THREADS, MINB)
 mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w1,
                     const __grid_constant__ CUtensorMap tm_w3, const S2Args a) {
-  using L = S2Smem<MID, COUT, WSTAGES>;
+  using L = S2Smem<CIN, MID, COUT, WSTAGES, MINB>;
   constexpr int NC = MID / S2_MC;
-  static_assert(CIN % 16 == 0 && CIN <= 64 && MID % 32 == 0 && NC >= 2 && (COUT == 32 || COUT == 64 || COUT == 128), "shape");
+  static_assert(CIN % 16 == 0 && (CIN <= 64 || CIN % 64 == 0) && MID % 32 == 0 && NC >= 2 &&
+                (COUT == 32 || COUT == 64 || COUT == 128 || COUT == 256), "shape");
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* s_in = smem;
   uint8_t* s_w1 = smem + L::OFF_W1;
@@ -124,21 +129,27 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
   }
   __syncthreads();
   const int tiles_per_img = a.tiles_x * a.tiles_y;
-  constexpr uint32_t W1_BYTES = S2_MC * 128, W3_BYTES = L::W3_STAGE;
+  constexpr uint32_t W1_BYTES = L::W1_STAGE, W3_BYTES = L::W3_STAGE;
 
   if (warp >= 8) {
     // ------------------------------------------------------------------------------------ control: TMA (warp 8 lane 0)
     ptx::setmaxnreg_dec<S2Regs<MINB>::TMA>();
     if (warp == 8 && lane == 0 && my_tiles > 0) {
+      // one box per 64-channel slab, all on the same barrier
       auto load_in = [&](int t) {
         const int bb = t / tiles_per_img, r = t % tiles_per_img;
-        ptx::mbar_arrive_expect_tx(bar_in, S2_PIN * 128);
-        ptx::tma_load_4d(&tm_in, bar_in, s_in, 0, 2 * (r % a.tiles_x) * S2_TW - 1, 2 * (r / a.tiles_x) * S2_TH - 1, bb);
+        ptx::mbar_arrive_expect_tx(bar_in, L::SLABS * S2_PIN * 128);
+#pragma unroll
+        for (int sl = 0; sl < L::SLABS; ++sl)
+          ptx::tma_load_4d(&tm_in, bar_in, s_in + sl * L::IN_SLAB, sl * 64, 2 * (r % a.tiles_x) * S2_TW - 1,
+                           2 * (r / a.tiles_x) * S2_TH - 1, bb);
       };
       auto load_w1 = [&](int g) {
         const int s = g & 1;
         ptx::mbar_arrive_expect_tx(bar_w1 + s, W1_BYTES);
-        ptx::tma_load_2d(&tm_w1, bar_w1 + s, s_w1 + s * W1_BYTES, 0, (g % NC) * S2_MC);
+#pragma unroll
+        for (int sl = 0; sl < L::SLABS; ++sl)
+          ptx::tma_load_2d(&tm_w1, bar_w1 + s, s_w1 + s * W1_BYTES + sl * L::W1_SLAB, sl * 64, (g % NC) * S2_MC);
       };
       auto load_w3 = [&](int g) {
         const int s = (WSTAGES == 2) ? (g & 1) : 0;
@@ -226,12 +237,13 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
         ptx::wg_fence();
 #pragma unroll
         for (int k = 0; k < CIN / 16; ++k) {
-          const uint64_t db = ptx::desc_advance(d_w1, st * W1_BYTES + k * 32);
+          const int sl = k / 4, kk = k % 4;                  // K-slab and K-step inside it
+          const uint64_t db = ptx::desc_advance(d_w1, st * W1_BYTES + sl * L::W1_SLAB + kk * 32);
 #pragma unroll
           for (int j = 0; j < 3; ++j) {
             // warpgroup 1 has two blocks; its third MMA repeats block 3 and is discarded, so no wgmma sits on a divergent path
             const int mb_off = (j == 2 && hsel == 1) ? 2 : 2 * j;   // block 2 j + hsel, relative to d_in's block hsel
-            ptx::wgmma_m64n32<0, 0>(ex[j], ptx::desc_advance(d_in, mb_off * 8192 + k * 32), db, k != 0);
+            ptx::wgmma_m64n32<0, 0>(ex[j], ptx::desc_advance(d_in, sl * L::IN_SLAB + mb_off * 8192 + kk * 32), db, k != 0);
           }
         }
         ptx::wg_commit();
@@ -320,7 +332,8 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
         for (int k = 0; k < S2_MC / 16; ++k) {
           const uint64_t da = ptx::desc_advance(d_dw, k * 32);
           const uint64_t db = ptx::desc_advance(d_w3, ws * W3_BYTES + k * 32);
-          if constexpr (PN == 64) ptx::wgmma_m64n64<0, 0>(proj, da, db, (c | k) != 0);
+          if constexpr (PN == 128) ptx::wgmma_m64n128<0, 0>(proj, da, db, (c | k) != 0);
+          else if constexpr (PN == 64) ptx::wgmma_m64n64<0, 0>(proj, da, db, (c | k) != 0);
           else ptx::wgmma_m64n32<0, 0>(proj, da, db, (c | k) != 0);
         }
         ptx::wg_commit();                                  // retired by the next chunk's expand wait, or below
@@ -355,7 +368,7 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
 
 template <int CIN, int MID, int COUT, int WSTAGES, int MINB>
 static int launch_mbconv_tc_s2(const void* x, const void* w1, const void* w3, const S2Args& a, int B, cudaStream_t st) {
-  using L = S2Smem<MID, COUT, WSTAGES>;
+  using L = S2Smem<CIN, MID, COUT, WSTAGES, MINB>;
   CUtensorMap tm_in, tm_w1, tm_w3;
   {
     uint64_t dims[4] = {(uint64_t)CIN, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)B};
@@ -393,6 +406,23 @@ static int launch_mbconv_tc_s2(const void* x, const void* w1, const void* w3, co
   return 0;
 }
 
+// The stride-2 kernel for (Cin, Mid, Cout) in {(16,64,32), (32,128,64), (64,256,128), (128,512,256)}, Cin selecting the
+// instantiation; shared with es3_mbconv_tc_wide_bf16 (mbconv_tc.cu), which owns the Cin-128 block.
+int mbconv_tc_s2(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw, const float* b2,
+                 const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin, cudaStream_t st) {
+  S2Args a;
+  a.y = (bf16*)y; a.s1 = s1; a.b1 = b1; a.wdw = wdw; a.b2 = b2; a.s3 = s3; a.b3 = b3;
+  a.H = H; a.W = W; a.Ho = (H - 1) / 2 + 1; a.Wo = (W - 1) / 2 + 1;
+  a.tiles_x = ceil_div(a.Wo, S2_TW); a.tiles_y = ceil_div(a.Ho, S2_TH);
+  a.total_tiles = B * a.tiles_x * a.tiles_y;
+  // two CTAs per SM (104 registers) where that does not spill, one (232 registers) for (64, 256, 128) and (128, 512, 256); the
+  // latter's 32 KB W3 box (256 rows) leaves room for one W3 stage only
+  if (Cin == 16) return launch_mbconv_tc_s2<16, 64, 32, 2, 2>(x, w1, w3, a, B, st);
+  if (Cin == 32) return launch_mbconv_tc_s2<32, 128, 64, 2, 2>(x, w1, w3, a, B, st);
+  if (Cin == 64) return launch_mbconv_tc_s2<64, 256, 128, 1, 1>(x, w1, w3, a, B, st);
+  return launch_mbconv_tc_s2<128, 512, 256, 1, 1>(x, w1, w3, a, B, st);
+}
+
 }  // namespace es3
 
 using namespace es3;
@@ -407,14 +437,5 @@ extern "C" int es3_mbconv_tc_s2_bf16(const void* x, void* y, const void* w1, con
   if (!ok) return -1;
   ES3_REQUIRE(B > 0 && H > 0 && W > 0, "es3_mbconv_tc_s2_bf16: bad shape");
   ES3_REQUIRE((((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w3 | (uintptr_t)y) & 15) == 0, "es3_mbconv_tc_s2_bf16: 16-byte alignment");
-  S2Args a;
-  a.y = (bf16*)y; a.s1 = s1; a.b1 = b1; a.wdw = wdw; a.b2 = b2; a.s3 = s3; a.b3 = b3;
-  a.H = H; a.W = W; a.Ho = (H - 1) / 2 + 1; a.Wo = (W - 1) / 2 + 1;
-  a.tiles_x = ceil_div(a.Wo, S2_TW); a.tiles_y = ceil_div(a.Ho, S2_TH);
-  a.total_tiles = B * a.tiles_x * a.tiles_y;
-  cudaStream_t st = (cudaStream_t)stream;
-  // two CTAs per SM (104 registers) where that does not spill, one (232 registers) for (64, 256, 128)
-  if (Cin == 16) return launch_mbconv_tc_s2<16, 64, 32, 2, 2>(x, w1, w3, a, B, st);
-  if (Cin == 32) return launch_mbconv_tc_s2<32, 128, 64, 2, 2>(x, w1, w3, a, B, st);
-  return launch_mbconv_tc_s2<64, 256, 128, 1, 1>(x, w1, w3, a, B, st);
+  return mbconv_tc_s2(x, y, w1, s1, b1, wdw, b2, w3, s3, b3, B, H, W, Cin, (cudaStream_t)stream);
 }

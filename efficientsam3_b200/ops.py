@@ -417,6 +417,8 @@ def mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, residual, act, impl
         rc = _call_rc("es3_mbconv_tc_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
         if rc < 0:
             rc = _call_rc("es3_mbconv_tc_s2_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
+        if rc < 0:
+            rc = _call_rc("es3_mbconv_tc_wide_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
     if rc < 0 and impl != "tc":
         rc = _call_rc("es3_mbconv_fused_bf16", "mbconv_fused" + shape, nbytes, flops, *args)
     return y if rc == 0 else None

@@ -113,6 +113,12 @@ int es3_mbconv_tc_bf16(const void* x, void* y, const void* w1, const float* s1, 
 int es3_mbconv_tc_s2_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
                           const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
                           int Mid, int Cout, int stride, int residual, int act, void* stream);
+/* Same contract on the same two kernels for the Cin-128 hardswish blocks: (128, 512, 128) stride 1 with residual and
+ * (128, 512, 256) stride 2 without (efficientvit_b1 stage 3 and the stage-4 opener, efficientvit_b0 stage 4), their input tile
+ * held as two 64-channel slabs, one CTA per SM.  Returns -1 for any other shape. */
+int es3_mbconv_tc_wide_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
+                            const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
+                            int Mid, int Cout, int stride, int residual, int act, void* stream);
 /* Depthwise 3x3 (stride 1) + bias + hardswish + pointwise projection + BN (+ residual) in one wgmma kernel, for MBConv blocks
  * whose expanded tensor is too wide for the fully fused kernels (EfficientViT stages 3/4): mid [B,H,W,Mid] bf16 is TMA-staged in
  * 64-channel chunks with its halo, the depthwise runs as diagonal m16n8k8 MMAs, its output goes straight into the swizzled A

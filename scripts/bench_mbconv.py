@@ -43,6 +43,8 @@ def cases(img):
             ("mbconv_tc_s2<32,128,64>", "mbconv", 32, 128, 64, 2, s // 2),
             ("mbconv_tc<64,256,64>", "mbconv", 64, 256, 64, 1, s // 4),
             ("mbconv_tc_s2<64,256,128>", "mbconv", 64, 256, 128, 2, s // 4),
+            ("mbconv_tc<128,512,128>", "mbconv", 128, 512, 128, 1, s // 8),
+            ("mbconv_tc_s2<128,512,256>", "mbconv", 128, 512, 256, 2, s // 8),
             ("dwproj_tc<512,128>", "dwproj", 0, 512, 128, 1, s // 8),
             ("dwproj_tc<1024,256>", "dwproj", 0, 1024, 256, 1, s // 16)]
 

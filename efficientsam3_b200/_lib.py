@@ -74,10 +74,7 @@ SIGNATURES: dict[str, list] = {
     "es3_stem_conv3x3_s2": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp],
     "es3_dwconv_bf16": [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _i, _vp],
     "es3_dwconv_tiled_bf16": [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _i, _vp],
-    "es3_mbconv_fused_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
-    "es3_mbconv_tc_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
-    "es3_mbconv_tc_s2_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
-    "es3_mbconv_tc_wide_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "es3_mbconv_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp],
     "es3_dwproj_tc_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp],
     "es3_stem_fused_c16": [_vp] * 10 + [_i, _i, _i, _vp],
     "es3_dsconv_res_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp],

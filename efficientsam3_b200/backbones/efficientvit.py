@@ -3,12 +3,10 @@ state_dict keys) of the reference `sam3/sam3/backbones/efficientvit/{backbone.py
 reference checkpoints load unchanged, but every forward runs on the hand-written kernels of libes3.so:
 
   input stem (conv 3x3 s2 + residual DSConv)         -> es3_stem_fused_c16 (b1; other widths: es3_stem_conv3x3_s2 + es3_dsconv_res_bf16)
-  MBConv blocks, stages 1-2 and the stage openers    -> es3_mbconv_tc_bf16 / es3_mbconv_tc_s2_bf16 (wgmma, whole block on the SM)
-  MBConv blocks 128->512->128 (b1 stage 3, b0 stage 4)
-    and the b1 stage-4 opener 128->512->256          -> es3_mbconv_tc_wide_bf16 (wgmma, whole block on the SM)
+  MBConv blocks of b0 / b1 up to Cin 128             -> es3_mbconv_bf16 (wgmma, whole block on the SM)
   other MBConv blocks of stages 3-4                  -> es3_gemm_bf16 (expand) + es3_dwproj_tc_bf16 (depthwise + project + residual)
   LiteMLA (ops.py:521-671)                           -> es3_gemm_bf16 (qkv, proj) + es3_litemla_aggreg_dwpw + es3_litemla_attn_tc
-  anything not instantiated                          -> es3_gemm_bf16 / es3_dwconv_tiled_bf16 / es3_mbconv_fused_bf16 (all native)
+  anything not instantiated                          -> es3_gemm_bf16 / es3_dwconv_tiled_bf16 (all native)
 
 Activations live in HBM as NHWC bf16; accumulation is fp32.  Eval-mode only (see NativePlanMixin).
 """
@@ -163,7 +161,7 @@ def _zeros(n, dev):
 
 
 class _MBConvPlan:
-    """MBConv (+ identity shortcut).  Tries the single-kernel fused path (es3_mbconv_fused_bf16) and falls
+    """MBConv (+ identity shortcut).  Tries the single-kernel fused path (es3_mbconv_bf16) and falls
     back to gemm_tc -> dwconv -> gemm_tc (all native kernels) for shapes it is not instantiated for."""
 
     def __init__(self, m: MBConv, residual: bool, device):

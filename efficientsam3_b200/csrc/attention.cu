@@ -11,24 +11,14 @@
 // double-buffered in shared memory; S = QK^T and O += PV run on mma.sync.m16n8k16 (bf16 in, fp32
 // accumulate), the online softmax lives in registers, P is re-used from the S accumulators as the A
 // operand (no smem round trip).  The wgmma flash attention (attention_tc.cu) serves sequences of >= 128 tokens.
-#include "common.cuh"
+#include "ptx.cuh"
 
 namespace es3 {
 
 namespace {
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
 __device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 __device__ __forceinline__ void cpa16(uint32_t saddr, const void* g, bool valid) {
   const int sz = valid ? 16 : 0;
@@ -139,8 +129,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
       for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks)
-          ldsm4(u_q + ((warp * MT + mt) * 16 + a_row) * AT_RS + (ks * 16 + a_kh * 8) * 2, qf[mt][ks][0], qf[mt][ks][1],
-                qf[mt][ks][2], qf[mt][ks][3]);
+          ptx::ldsm_x4(u_q + ((warp * MT + mt) * 16 + a_row) * AT_RS + (ks * 16 + a_kh * 8) * 2, qf[mt][ks][0], qf[mt][ks][1],
+                       qf[mt][ks][2], qf[mt][ks][3]);
     }
     // ---- S = Q K^T (K fragments shared by the MT query tiles)
     float s[MT][8][4];
@@ -154,11 +144,11 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
 #pragma unroll
       for (int np = 0; np < 4; ++np) {
         uint32_t b0, b1, b2, b3;
-        ldsm4(kb + (np * 16 + b_n) * AT_RS + (ks * 16 + b_kh * 8) * 2, b0, b1, b2, b3);
+        ptx::ldsm_x4(kb + (np * 16 + b_n) * AT_RS + (ks * 16 + b_kh * 8) * 2, b0, b1, b2, b3);
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) {
-          mma16816(s[mt][2 * np], qf[mt][ks], b0, b1);
-          mma16816(s[mt][2 * np + 1], qf[mt][ks], b2, b3);
+          ptx::mma_16816(s[mt][2 * np], qf[mt][ks], b0, b1);
+          ptx::mma_16816(s[mt][2 * np + 1], qf[mt][ks], b2, b3);
         }
       }
     }
@@ -218,8 +208,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
         ldsm4t(vb + (ks * 16 + v_k) * AT_RS + (np * 16 + v_n) * 2, b0, b1, b2, b3);
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) {
-          mma16816(o[mt][2 * np], pf[mt][ks], b0, b1);
-          mma16816(o[mt][2 * np + 1], pf[mt][ks], b2, b3);
+          ptx::mma_16816(o[mt][2 * np], pf[mt][ks], b0, b1);
+          ptx::mma_16816(o[mt][2 * np + 1], pf[mt][ks], b2, b3);
         }
       }
     }

@@ -76,7 +76,7 @@ template <int ACT>
 __device__ __forceinline__ float es3_act_t(float x) {
   if constexpr (ACT == ACT_RELU) return fmaxf(x, 0.f);
   // x * relu6(x + 3) / 6 == x * sat(x / 6 + 0.5): FFMA.SAT + FMUL instead of FADD, 2 FMNMX, 2 FMUL (the
-  // 5-op form was a large share of mbconv_fused's instructions)
+  // 5-op form was a large share of a fused MBConv kernel's instructions)
   else if constexpr (ACT == ACT_HSWISH) return x * __saturatef(fmaf(x, 1.f / 6.f, 0.5f));
   else if constexpr (ACT == ACT_GELU) return es3_gelu_fast(x);
   else if constexpr (ACT == ACT_GELU_TANH) {

@@ -21,26 +21,10 @@
 // (zero fill = the convolution's padding).  Warp -> (16-channel sub-group, half of the tile's rows).
 #include <cstdlib>
 
-#include "common.cuh"
+#include "ptx.cuh"
 
 namespace es3 {
 namespace {
-__device__ __forceinline__ void tc_ldsm4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void tc_mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void tc_mma1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(b0));
-}
 __device__ __forceinline__ void tc_cpa16(uint32_t saddr, const void* g, bool valid) {
   const int sz = valid ? 16 : 0;
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(g), "r"(sz) : "memory");
@@ -151,19 +135,19 @@ dw_tc_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict_
         uint32_t af[ROWS + KS - 1][4];                        // the input rows this warp's ROWS output rows touch, column offset kx
 #pragma unroll
         for (int r = 0; r < ROWS + KS - 1; ++r)
-          tc_ldsm4(u_tile + ((rb * ROWS + r) * T::IW + xh * 16 + a_row + kx) * T::PS + (sub * 16 + a_kh * 8) * 2, af[r][0], af[r][1], af[r][2],
-                   af[r][3]);
+          ptx::ldsm_x4(u_tile + ((rb * ROWS + r) * T::IW + xh * 16 + a_row + kx) * T::PS + (sub * 16 + a_kh * 8) * 2, af[r][0], af[r][1], af[r][2],
+                       af[r][3]);
 #pragma unroll
         for (int m = 0; m < ROWS; ++m) {
 #pragma unroll
           for (int kp = 0; kp < KS / 2; ++kp) {               // tap pairs (2 kp, kx) + (2 kp + 1, kx) in one k16 MMA
             const uint32_t a_lo[4] = {af[m + 2 * kp][0], af[m + 2 * kp][1], af[m + 2 * kp + 1][0], af[m + 2 * kp + 1][1]};
             const uint32_t a_hi[4] = {af[m + 2 * kp][2], af[m + 2 * kp][3], af[m + 2 * kp + 1][2], af[m + 2 * kp + 1][3]};
-            tc_mma16816(acc[m][0], a_lo, b_lo[(2 * kp) * KS + kx], b_lo[(2 * kp + 1) * KS + kx]);
-            tc_mma16816(acc[m][1], a_hi, b_hi[(2 * kp) * KS + kx], b_hi[(2 * kp + 1) * KS + kx]);
+            ptx::mma_16816(acc[m][0], a_lo, b_lo[(2 * kp) * KS + kx], b_lo[(2 * kp + 1) * KS + kx]);
+            ptx::mma_16816(acc[m][1], a_hi, b_hi[(2 * kp) * KS + kx], b_hi[(2 * kp + 1) * KS + kx]);
           }
-          tc_mma1688(acc[m][0], af[m + KS - 1][0], af[m + KS - 1][1], b_lo[(KS - 1) * KS + kx]);   // the odd tap row
-          tc_mma1688(acc[m][1], af[m + KS - 1][2], af[m + KS - 1][3], b_hi[(KS - 1) * KS + kx]);
+          ptx::mma_1688(acc[m][0], af[m + KS - 1][0], af[m + KS - 1][1], b_lo[(KS - 1) * KS + kx]);   // the odd tap row
+          ptx::mma_1688(acc[m][1], af[m + KS - 1][2], af[m + KS - 1][3], b_hi[(KS - 1) * KS + kx]);
         }
       }
 #pragma unroll

@@ -17,27 +17,6 @@
 
 namespace es3 {
 
-int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b, const uint32_t* box);
-
-namespace {
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma_16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(b0));
-}
-}  // namespace
-
 constexpr int DP_TH = 8, DP_TW = 16, DP_HH = DP_TH + 2, DP_HW = DP_TW + 2, DP_PIN = DP_HH * DP_HW;   // 8x16 tile, 10x18 halo
 constexpr int DP_MC = 64, DP_THREADS = 384;   // two compute warpgroups + one TMA warpgroup
 
@@ -169,7 +148,7 @@ dwproj_tc_kernel(const __grid_constant__ CUtensorMap tm_mid, const __grid_consta
 #pragma unroll
           for (int r = 0; r < 6; ++r) {
             const int row = (hsel * 4 + r) * DP_HW + a_row + kx;                // pixel row of the swizzled tile
-            ldsm_x4(u_a + row * 128 + (((cg * 2 + a_kh) ^ (row & 7)) << 4), af[r][0], af[r][1], af[r][2], af[r][3]);
+            ptx::ldsm_x4(u_a + row * 128 + (((cg * 2 + a_kh) ^ (row & 7)) << 4), af[r][0], af[r][1], af[r][2], af[r][3]);
           }
           // taps (0, kx) and (1, kx) in one m16n8k16 (same issue rate as m16n8k8), (2, kx) as a k8 MMA: 12 MMAs per m-tile instead of 18
           uint32_t b_lo[3], b_hi[3];
@@ -184,10 +163,10 @@ dwproj_tc_kernel(const __grid_constant__ CUtensorMap tm_mid, const __grid_consta
           for (int m = 0; m < 4; ++m) {
             const uint32_t a_lo[4] = {af[m][0], af[m][1], af[m + 1][0], af[m + 1][1]};
             const uint32_t a_hi[4] = {af[m][2], af[m][3], af[m + 1][2], af[m + 1][3]};
-            mma_16816(dacc[m][0], a_lo, b_lo[0], b_lo[1]);
-            mma_16816(dacc[m][1], a_hi, b_hi[0], b_hi[1]);
-            mma_1688(dacc[m][0], af[m + 2][0], af[m + 2][1], b_lo[2]);
-            mma_1688(dacc[m][1], af[m + 2][2], af[m + 2][3], b_hi[2]);
+            ptx::mma_16816(dacc[m][0], a_lo, b_lo[0], b_lo[1]);
+            ptx::mma_16816(dacc[m][1], a_hi, b_hi[0], b_hi[1]);
+            ptx::mma_1688(dacc[m][0], af[m + 2][0], af[m + 2][1], b_lo[2]);
+            ptx::mma_1688(dacc[m][1], af[m + 2][2], af[m + 2][3], b_hi[2]);
           }
         }
         // The mid stage was read through the generic proxy (ldmatrix) and TMA (async proxy) refills it once bar_afree completes:

@@ -24,9 +24,6 @@
 #include "ptx.cuh"
 
 namespace es3 {
-
-int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b, const uint32_t* box);
-
 namespace fp8 {
 
 constexpr int BM = 128, BN = 128, BK = 128;  // BK: 128 e4m3 = 128 B = one swizzle row = one scale block

@@ -13,23 +13,13 @@
 //           ones row (ops.py:613 F.pad value=1) via a constant A fragment.  Deterministic two-stage reduce.
 //  apply  : out[p][d] = sum_j KV[d][j] relu(q[p][j]) / (KV[16] . relu(q[p]) + eps)
 //           (M=pixels, N=17->24, K=16), KV split hi+lo bf16 so the fp32 state keeps ~16 mantissa bits.
-#include "common.cuh"
+#include "ptx.cuh"
 
 namespace es3 {
 namespace {
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
 __device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 __device__ __forceinline__ void cpa16(uint32_t saddr, const void* g, bool valid) {
   const int sz = valid ? 16 : 0;
@@ -53,12 +43,6 @@ constexpr int AG_TILE_BYTES = AG_IH * AG_IW * AG_PS;      // 34560
 // ms: [B,H,W,ld] bf16.  Reads channels [grp*16, +16) (qkv), writes channels [C3 + grp*16, +16).
 // wdw: [C3/16][25][16] bf16 (group, tap, channel);  wpw: [C3][16] bf16 (output channel, input channel within its group).
 constexpr int AG2_SMEM = AG_TILE_BYTES + 25 * 16 * 2 + 16 * AG_PS;
-__device__ __forceinline__ void mma1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(b0));
-}
 __global__ void __launch_bounds__(256, 3) litemla_aggreg_dwpw_kernel(const bf16* ms_in, bf16* ms_out, long long ld,
                                                                   const bf16* __restrict__ wdw, const bf16* __restrict__ wpw,
                                                                   int H, int W, int tiles_x) {
@@ -105,7 +89,7 @@ __global__ void __launch_bounds__(256, 3) litemla_aggreg_dwpw_kernel(const bf16*
     uint32_t af[8][4];
 #pragma unroll
     for (int r = 0; r < 8; ++r)
-      ldsm4(u_tile + ((y0 + r) * AG_IW + xh * 16 + a_row + kx) * AG_PS + a_kh * 16, af[r][0], af[r][1], af[r][2], af[r][3]);
+      ptx::ldsm_x4(u_tile + ((y0 + r) * AG_IW + xh * 16 + a_row + kx) * AG_PS + a_kh * 16, af[r][0], af[r][1], af[r][2], af[r][3]);
     // two taps per MMA (m16n8k16 issues at the rate of m16n8k8): (0, kx)+(1, kx), (2, kx)+(3, kx) as k16, (4, kx) as k8 -- 30 MMAs per
     // m-tile instead of 50; the legacy-MMA pipe was this kernel's limiter (60 % busy)
     uint32_t b_lo[5], b_hi[5];
@@ -122,15 +106,15 @@ __global__ void __launch_bounds__(256, 3) litemla_aggreg_dwpw_kernel(const bf16*
       for (int kp = 0; kp < 2; ++kp) {
         const uint32_t a_lo[4] = {af[m + 2 * kp][0], af[m + 2 * kp][1], af[m + 2 * kp + 1][0], af[m + 2 * kp + 1][1]};
         const uint32_t a_hi[4] = {af[m + 2 * kp][2], af[m + 2 * kp][3], af[m + 2 * kp + 1][2], af[m + 2 * kp + 1][3]};
-        mma16816(acc[m][0], a_lo, b_lo[2 * kp], b_lo[2 * kp + 1]);
-        mma16816(acc[m][1], a_hi, b_hi[2 * kp], b_hi[2 * kp + 1]);
+        ptx::mma_16816(acc[m][0], a_lo, b_lo[2 * kp], b_lo[2 * kp + 1]);
+        ptx::mma_16816(acc[m][1], a_hi, b_hi[2 * kp], b_hi[2 * kp + 1]);
       }
-      mma1688(acc[m][0], af[m + 4][0], af[m + 4][1], b_lo[4]);
-      mma1688(acc[m][1], af[m + 4][2], af[m + 4][3], b_hi[4]);
+      ptx::mma_1688(acc[m][0], af[m + 4][0], af[m + 4][1], b_lo[4]);
+      ptx::mma_1688(acc[m][1], af[m + 4][2], af[m + 4][3], b_hi[4]);
     }
   }
   uint32_t p0, p1, p2, p3;
-  ldsm4(u_wp + b_n * AG_PS + b_kh * 16, p0, p1, p2, p3);
+  ptx::ldsm_x4(u_wp + b_n * AG_PS + b_kh * 16, p0, p1, p2, p3);
   bf16* ob = ms_out + (long long)b * H * W * ld + grp * 16;
 #pragma unroll
   for (int m = 0; m < 4; ++m) {
@@ -138,8 +122,8 @@ __global__ void __launch_bounds__(256, 3) litemla_aggreg_dwpw_kernel(const bf16*
     const uint32_t pa[4] = {pack_bf16x2(acc[m][0][0], acc[m][0][1]), pack_bf16x2(acc[m][0][2], acc[m][0][3]),
                             pack_bf16x2(acc[m][1][0], acc[m][1][1]), pack_bf16x2(acc[m][1][2], acc[m][1][3])};
     float o[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-    mma16816(o[0], pa, p0, p1);
-    mma16816(o[1], pa, p2, p3);
+    ptx::mma_16816(o[0], pa, p0, p1);
+    ptx::mma_16816(o[1], pa, p2, p3);
     const int oy = oy0 + y0 + m;
     if (oy >= H) continue;
 #pragma unroll
@@ -193,10 +177,10 @@ __global__ void __launch_bounds__(256) litemla_kv_tc_kernel(const bf16* __restri
     ldsm4t(u + (p0 + av_p) * KV_RS + av_c, af[0], af[1], af[2], af[3]);
     ldsm4t(u + (p0 + bk_p) * KV_RS + bk_c, b0, b1, b2, b3);
     b0 = relu_bf16x2(b0); b1 = relu_bf16x2(b1); b2 = relu_bf16x2(b2); b3 = relu_bf16x2(b3);
-    mma16816(acc[0], af, b0, b1);
-    mma16816(acc[1], af, b2, b3);
-    mma16816(ones[0], a_ones, b0, b1);
-    mma16816(ones[1], a_ones, b2, b3);
+    ptx::mma_16816(acc[0], af, b0, b1);
+    ptx::mma_16816(acc[1], af, b2, b3);
+    ptx::mma_16816(ones[0], a_ones, b0, b1);
+    ptx::mma_16816(ones[1], a_ones, b2, b3);
   }
   __syncthreads();  // tile no longer needed: reuse smem as red[8 warps][17][16]
   float* red = reinterpret_cast<float*>(s_kv);
@@ -276,8 +260,8 @@ __global__ void __launch_bounds__(128) litemla_apply_tc_kernel(const bf16* __res
 #pragma unroll
     for (int nt = 0; nt < 3; ++nt) {
       acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-      mma16816(acc[nt], af, bl[nt][0], bl[nt][1]);
-      mma16816(acc[nt], af, bh[nt][0], bh[nt][1]);
+      ptx::mma_16816(acc[nt], af, bl[nt][0], bl[nt][1]);
+      ptx::mma_16816(acc[nt], af, bh[nt][0], bh[nt][1]);
     }
     // denominators: column 16 (n-tile 2, col 0) lives in lane g*4
     const float den_a = __shfl_sync(0xffffffffu, acc[2][0], g * 4);

@@ -1,8 +1,11 @@
 // Fused MBConv on wgmma (stride 1, residual): y = x + BN3(pw2(act(BN2(dw3x3(act(BN1(pw1(x)))))))) with the 4x-expanded
 // tensor kept on the SM (reference efficientvit/nn/ops.py:315-367 MBConv inside ResidualBlock :740-770).
 //
-// Why a second fused kernel: in mbconv_fused.cu all three contractions run on mma.sync, with every phase separated by
-// __syncthreads.  Here the two pointwise GEMMs are warpgroup MMAs (wgmma) from TMA-staged, 128B-swizzled operands:
+// The two pointwise GEMMs are warpgroup MMAs (wgmma) from TMA-staged, 128B-swizzled operands; the depthwise between them runs
+// on mma.sync.  For a 16-channel group the 3x3 depthwise is 9 MMAs with DIAGONAL B matrices, D[px][c] += A[px + tap][c] w[tap][c]:
+// a diagonal B fragment has at most one non-zero bf16 per lane (lane g = lane / 4, t4 = lane % 4 holds w[tap][g] where
+// g / 2 == t4, in the low half when g is even and the high half when odd), so each lane builds its B registers from the taps
+// alone and A comes straight from ldmatrix.
 //
 //   TMA (4-D map, halo + zero fill)  ->  s_in  CIN/64 slabs of [10x18 px][64 ch]  128B-swizzled K-major A operand
 //   per 64-channel chunk of the expanded tensor:
@@ -25,26 +28,7 @@
 
 namespace es3 {
 
-int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b, const uint32_t* box);
-
 namespace {
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma_16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-// m16n8k8: a diagonal 8x8 B has no structural zeros to multiply (the k16 form wasted half of every MMA)
-__device__ __forceinline__ void mma_1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(b0));
-}
 __device__ __forceinline__ void compute_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 }  // namespace
 
@@ -291,7 +275,7 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
             uint32_t af[6][4];
 #pragma unroll
             for (int r = 0; r < 6; ++r)
-              ldsm_x4(u_mid + ((hsel * 4 + r) * MT_HW + a_row + kx) * MT_RS_MID + (cg * 16 + a_kh * 8) * 2, af[r][0], af[r][1], af[r][2], af[r][3]);
+              ptx::ldsm_x4(u_mid + ((hsel * 4 + r) * MT_HW + a_row + kx) * MT_RS_MID + (cg * 16 + a_kh * 8) * 2, af[r][0], af[r][1], af[r][2], af[r][3]);
             // two taps per MMA: m16n8k16 issues at the rate of m16n8k8, so the taps (0, kx) and
             // (1, kx) share one instruction -- A = [tap-0 fragment | tap-1 fragment] along k, B = [diag(w0) ; diag(w1)] -- and (2, kx)
             // stays a k8 MMA: 12 MMAs per 16 pixels x 16 channels instead of 18
@@ -307,10 +291,10 @@ mbconv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constan
             for (int m = 0; m < 4; ++m) {
               const uint32_t a_lo[4] = {af[m][0], af[m][1], af[m + 1][0], af[m + 1][1]};
               const uint32_t a_hi[4] = {af[m][2], af[m][3], af[m + 1][2], af[m + 1][3]};
-              mma_16816(dacc[m][0], a_lo, b_lo[0], b_lo[1]);                   // channels cg*16 + 0..7, taps ky = 0, 1
-              mma_16816(dacc[m][1], a_hi, b_hi[0], b_hi[1]);                   // channels cg*16 + 8..15
-              mma_1688(dacc[m][0], af[m + 2][0], af[m + 2][1], b_lo[2]);       // tap ky = 2
-              mma_1688(dacc[m][1], af[m + 2][2], af[m + 2][3], b_hi[2]);
+              ptx::mma_16816(dacc[m][0], a_lo, b_lo[0], b_lo[1]);                   // channels cg*16 + 0..7, taps ky = 0, 1
+              ptx::mma_16816(dacc[m][1], a_hi, b_hi[0], b_hi[1]);                   // channels cg*16 + 8..15
+              ptx::mma_1688(dacc[m][0], af[m + 2][0], af[m + 2][1], b_lo[2]);       // tap ky = 2
+              ptx::mma_1688(dacc[m][1], af[m + 2][2], af[m + 2][3], b_hi[2]);
             }
           }
           float2 bb[2];                                   // bias of channels cg * 16 + nt * 8 + 2 t4
@@ -437,7 +421,8 @@ static MTArgs mt_args(const void* x, void* y, const float* s1, const float* b1, 
   return a;
 }
 
-// mbconv_tc_s2.cu: the stride-2 kernel for (Cin, Mid, Cout) in {(16,64,32), (32,128,64), (64,256,128), (128,512,256)}
+// mbconv_tc_s2.cu: the stride-2 kernel for (Cin, Mid, Cout) in {(16,64,32), (32,128,64), (64,256,128), (128,512,256)}, Cin
+// selecting the instantiation
 int mbconv_tc_s2(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw, const float* b2,
                  const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin, cudaStream_t st);
 
@@ -445,33 +430,31 @@ int mbconv_tc_s2(const void* x, void* y, const void* w1, const float* s1, const 
 
 using namespace es3;
 
-// Same contract as es3_mbconv_fused_bf16 for the stride-1 residual blocks (Cin == Cout in {32, 64}, Mid = 4 Cin, hardswish).
-// Returns -1 (no error set) for any other shape.
-extern "C" int es3_mbconv_tc_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
-                                  const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
-                                  int Mid, int Cout, int stride, int residual, int act, void* stream) {
-  if (!(stride == 1 && residual && act == ACT_HSWISH && Cin == Cout && Mid == 4 * Cin && (Cin == 32 || Cin == 64))) return -1;
-  ES3_REQUIRE(B > 0 && H > 0 && W > 0, "es3_mbconv_tc_bf16: bad shape");
-  ES3_REQUIRE((((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w3 | (uintptr_t)y) & 15) == 0, "es3_mbconv_tc_bf16: 16-byte alignment");
+// The fused MBConv blocks: mbconv_tc_kernel for the stride-1 blocks with residual, mbconv_tc_s2_kernel for the stride-2 stage
+// openers without, hardswish only.  Returns -1 (no error set, nothing written) for any other shape or activation.
+extern "C" int es3_mbconv_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
+                               const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
+                               int Mid, int Cout, int stride, int residual, int act, void* stream) {
+  auto is = [&](int ci, int mi, int co, int s) {
+    return Cin == ci && Mid == mi && Cout == co && stride == s && (residual != 0) == (s == 1);
+  };
+  // (.local: the MBConv of an EfficientViTBlock, op_list.i.local_module.main)
+  const bool tc32 = is(32, 128, 32, 1);     // efficientvit_b1 stages.0.op_list.1, b0 stages.1.op_list.1
+  const bool tc64 = is(64, 256, 64, 1);     // b1 stages.1.op_list.1-2, b0 stages.2.op_list.1-2.local
+  const bool tc128 = is(128, 512, 128, 1);  // b1 stages.2.op_list.1-3.local, b0 stages.3.op_list.1-2.local
+  const bool s2 = is(16, 64, 32, 2) ||      // b1 stages.0.op_list.0, b0 stages.1.op_list.0
+                  is(32, 128, 64, 2) ||     // b1 stages.1.op_list.0, b0 stages.2.op_list.0
+                  is(64, 256, 128, 2) ||    // b1 stages.2.op_list.0, b0 stages.3.op_list.0
+                  is(128, 512, 256, 2);     // b1 stages.3.op_list.0
+  if (act != ACT_HSWISH || !(tc32 || tc64 || tc128 || s2)) return -1;
+  ES3_REQUIRE(B > 0 && H > 0 && W > 0, "es3_mbconv_bf16: bad shape");
+  ES3_REQUIRE((((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w3 | (uintptr_t)y) & 15) == 0, "es3_mbconv_bf16: 16-byte alignment");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (s2) return mbconv_tc_s2(x, y, w1, s1, b1, wdw, b2, w3, s3, b3, B, H, W, Cin, st);
   const MTArgs a = mt_args(x, y, s1, b1, wdw, b2, s3, b3, B, H, W);
-  cudaStream_t st = (cudaStream_t)stream;
   // (32, 128, 32) fits 104 registers and runs faster with a second CTA per SM to overlap its phases; (64, 256, 64) needs more
-  // than 104 (it spills and ptxas serialises its wgmma) and runs at one CTA per SM
-  if (Cin == 32) return launch_mbconv_tc<32, 128, 32, 2>(x, y, w1, w3, a, B, st);
-  return launch_mbconv_tc<64, 256, 64, 1>(x, y, w1, w3, a, B, st);
-}
-
-// Same contract as es3_mbconv_fused_bf16 for the Cin-128 hardswish blocks: (128, 512, 128) stride 1 with residual (this file's
-// kernel with two 64-channel input slabs) and (128, 512, 256) stride 2 without (mbconv_tc_s2.cu), both at one CTA per SM.
-// Returns -1 (no error set) for any other shape.
-extern "C" int es3_mbconv_tc_wide_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
-                                       const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W,
-                                       int Cin, int Mid, int Cout, int stride, int residual, int act, void* stream) {
-  const bool s1_res = stride == 1 && residual && Cout == 128, s2_open = stride == 2 && !residual && Cout == 256;
-  if (!(act == ACT_HSWISH && Cin == 128 && Mid == 512 && (s1_res || s2_open))) return -1;
-  ES3_REQUIRE(B > 0 && H > 0 && W > 0, "es3_mbconv_tc_wide_bf16: bad shape");
-  ES3_REQUIRE((((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w3 | (uintptr_t)y) & 15) == 0, "es3_mbconv_tc_wide_bf16: 16-byte alignment");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (s2_open) return mbconv_tc_s2(x, y, w1, s1, b1, wdw, b2, w3, s3, b3, B, H, W, Cin, st);
-  return launch_mbconv_tc<128, 512, 128, 1>(x, y, w1, w3, mt_args(x, y, s1, b1, wdw, b2, s3, b3, B, H, W), B, st);
+  // than 104 (it spills and ptxas serialises its wgmma) and (128, 512, 128) 170 KB of shared memory: one CTA per SM
+  if (tc32) return launch_mbconv_tc<32, 128, 32, 2>(x, y, w1, w3, a, B, st);
+  if (tc64) return launch_mbconv_tc<64, 256, 64, 1>(x, y, w1, w3, a, B, st);
+  return launch_mbconv_tc<128, 512, 128, 1>(x, y, w1, w3, a, B, st);
 }

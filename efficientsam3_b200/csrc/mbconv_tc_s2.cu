@@ -12,25 +12,7 @@
 
 namespace es3 {
 
-int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b, const uint32_t* box);
-
 namespace {
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma_16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(b0));
-}
 __device__ __forceinline__ void compute_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 }  // namespace
 
@@ -282,8 +264,8 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
           auto frag = [&](int tap, uint32_t* af) {
             const int ky = tap / 3, kx = tap - ky * 3;
             // input column 2 * a_row + kx: kx = 0 / 2 -> even slots a_row / a_row + 1, kx = 1 -> odd slot a_row
-            ldsm_x4(u_mid + ((2 * mt + ky) * S2_PW + a_row + (kx == 1 ? S2_ODD : (kx >> 1))) * S2_RS_MID + (cg * 16 + a_kh * 8) * 2,
-                    af[0], af[1], af[2], af[3]);
+            ptx::ldsm_x4(u_mid + ((2 * mt + ky) * S2_PW + a_row + (kx == 1 ? S2_ODD : (kx >> 1))) * S2_RS_MID + (cg * 16 + a_kh * 8) * 2,
+                         af[0], af[1], af[2], af[3]);
           };
           auto bfrag = [&](int tap, uint32_t& b_lo, uint32_t& b_hi) {
             const uint32_t w_lo = (uint32_t)__bfloat16_as_ushort(wd[tap * S2_MC]);
@@ -298,14 +280,14 @@ mbconv_tc_s2_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_cons
             bfrag(2 * tp, la, ha); bfrag(2 * tp + 1, lb, hb);
             const uint32_t a_lo[4] = {fa[0], fa[1], fb[0], fb[1]};
             const uint32_t a_hi[4] = {fa[2], fa[3], fb[2], fb[3]};
-            mma_16816(dacc[0], a_lo, la, lb);
-            mma_16816(dacc[1], a_hi, ha, hb);
+            ptx::mma_16816(dacc[0], a_lo, la, lb);
+            ptx::mma_16816(dacc[1], a_hi, ha, hb);
           }
           {
             uint32_t fa[4], la, ha;
             frag(8, fa); bfrag(8, la, ha);
-            mma_1688(dacc[0], fa[0], fa[1], la);
-            mma_1688(dacc[1], fa[2], fa[3], ha);
+            ptx::mma_1688(dacc[0], fa[0], fa[1], la);
+            ptx::mma_1688(dacc[1], fa[2], fa[3], ha);
           }
           float2 bb[2];                                     // bias of channels cg * 16 + nt * 8 + 2 t4
 #pragma unroll
@@ -407,7 +389,7 @@ static int launch_mbconv_tc_s2(const void* x, const void* w1, const void* w3, co
 }
 
 // The stride-2 kernel for (Cin, Mid, Cout) in {(16,64,32), (32,128,64), (64,256,128), (128,512,256)}, Cin selecting the
-// instantiation; shared with es3_mbconv_tc_wide_bf16 (mbconv_tc.cu), which owns the Cin-128 block.
+// instantiation; es3_mbconv_bf16 (mbconv_tc.cu) accepts the shape and checks the arguments.
 int mbconv_tc_s2(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw, const float* b2,
                  const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin, cudaStream_t st) {
   S2Args a;
@@ -424,18 +406,3 @@ int mbconv_tc_s2(const void* x, void* y, const void* w1, const float* s1, const 
 }
 
 }  // namespace es3
-
-using namespace es3;
-
-// Same contract as es3_mbconv_fused_bf16 for the stride-2, no-residual, hardswish blocks with (Cin, Mid, Cout) in
-// {(16,64,32), (32,128,64), (64,256,128)}.  Returns -1 (no error set) for any other shape.
-extern "C" int es3_mbconv_tc_s2_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
-                                     const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
-                                     int Mid, int Cout, int stride, int residual, int act, void* stream) {
-  const bool ok = stride == 2 && !residual && act == ACT_HSWISH &&
-                  ((Cin == 16 && Mid == 64 && Cout == 32) || (Cin == 32 && Mid == 128 && Cout == 64) || (Cin == 64 && Mid == 256 && Cout == 128));
-  if (!ok) return -1;
-  ES3_REQUIRE(B > 0 && H > 0 && W > 0, "es3_mbconv_tc_s2_bf16: bad shape");
-  ES3_REQUIRE((((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w3 | (uintptr_t)y) & 15) == 0, "es3_mbconv_tc_s2_bf16: 16-byte alignment");
-  return mbconv_tc_s2(x, y, w1, s1, b1, wdw, b2, w3, s3, b3, B, H, W, Cin, (cudaStream_t)stream);
-}

@@ -1,12 +1,39 @@
-// Thin inline-PTX wrappers for the Hopper (sm_90a) async machinery:
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors), fences.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) async machinery and the warp-level tensor-core instructions:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors), fences, ldmatrix, mma.sync.
 #pragma once
 #include "common.cuh"
+
+namespace es3 {
+// Rank-N bf16 TMA tensor map with the 128-byte swizzle and zero out-of-bounds fill (defined in gemm_tc.cu): dims innermost
+// first, strides in bytes for dims 1..rank-1.  Returns non-zero, with the error set, on failure.
+int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b, const uint32_t* box);
+}  // namespace es3
 
 namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+
+// ---------------------------------------------------------------------------------------- ldmatrix / mma.sync
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+// D[16 x 8] += A[16 x 16] * B[16 x 8], bf16 in, fp32 accumulate.
+__device__ __forceinline__ void mma_16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// D[16 x 8] += A[16 x 8] * B[8 x 8]: a diagonal 8x8 B (the depthwise convolutions' taps) has no structural zeros to multiply,
+// where the k16 form would waste half of every MMA.
+__device__ __forceinline__ void mma_1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a0), "r"(a1), "r"(b0));
 }
 
 // ---------------------------------------------------------------------------------------- mbarrier

@@ -4,20 +4,10 @@
 //     stride-2 pixel addressing, MMA) per 16 output pixels
 //   * SqueezeExcite pieces (timm.layers.SqueezeExcite; repvit.py:136,150): per-image channel means
 //     (deterministic two-stage) and the channel-gate multiply.  The two tiny FCs run on es3_gemm_simt.
-#include "common.cuh"
+#include "ptx.cuh"
 
 namespace es3 {
 namespace {
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ void cpa16(uint32_t saddr, const void* g, bool valid) {
   const int sz = valid ? 16 : 0;
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(g), "r"(sz) : "memory");
@@ -69,13 +59,13 @@ __global__ void __launch_bounds__(256) conv3x3_s2_c32_kernel(const bf16* __restr
 #pragma unroll
     for (int ks = 0; ks < S2_CIN / 16; ++ks) {
       uint32_t af[4];
-      ldsm4(u_tile + ((2 * warp + ky) * S2_IW + 2 * a_row + kx) * S2_RS + (ks * 16 + a_kh * 8) * 2, af[0], af[1], af[2], af[3]);
+      ptx::ldsm_x4(u_tile + ((2 * warp + ky) * S2_IW + 2 * a_row + kx) * S2_RS + (ks * 16 + a_kh * 8) * 2, af[0], af[1], af[2], af[3]);
 #pragma unroll
       for (int np = 0; np < COUT / 16; ++np) {
         uint32_t b0, b1, b2, b3;
-        ldsm4(u_w + (tap * COUT + np * 16 + b_n) * S2_RS + (ks * 16 + b_kh * 8) * 2, b0, b1, b2, b3);
-        mma16816(acc[2 * np], af, b0, b1);
-        mma16816(acc[2 * np + 1], af, b2, b3);
+        ptx::ldsm_x4(u_w + (tap * COUT + np * 16 + b_n) * S2_RS + (ks * 16 + b_kh * 8) * 2, b0, b1, b2, b3);
+        ptx::mma_16816(acc[2 * np], af, b0, b1);
+        ptx::mma_16816(acc[2 * np + 1], af, b2, b3);
       }
     }
   }

@@ -9,31 +9,15 @@
 //            kept in smem as bf16 (the same rounding the unfused path applies when it stores x1)
 //   phase 3  depthwise 3x3 as 9 diagonal-B MMAs, BN + hardswish, result re-used in registers as the A operand of the
 //            16x16 pointwise MMA, + BN + residual(x1) -> global (NHWC bf16)
-#include "common.cuh"
+#include "ptx.cuh"
 
 namespace es3 {
 namespace {
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
 __device__ __forceinline__ void cpa4(uint32_t saddr, const void* g, uint32_t sz) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(saddr), "l"(g), "r"(sz) : "memory");
 }
 __device__ __forceinline__ void cpa16(uint32_t saddr, const void* g, uint32_t sz) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(g), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma1688(float* d, uint32_t a0, uint32_t a1, uint32_t b0) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(b0));
 }
 }  // namespace
 
@@ -123,7 +107,7 @@ __global__ void __launch_bounds__(256) stem_fused_kernel(const StemArgs a) {
   {
     uint32_t wf[2][4];
 #pragma unroll
-    for (int ks = 0; ks < 2; ++ks) ldsm4(u_w0 + b_n * SF_ARS + (ks * 16 + b_kh * 8) * 2, wf[ks][0], wf[ks][1], wf[ks][2], wf[ks][3]);
+    for (int ks = 0; ks < 2; ++ks) ptx::ldsm_x4(u_w0 + b_n * SF_ARS + (ks * 16 + b_kh * 8) * 2, wf[ks][0], wf[ks][1], wf[ks][2], wf[ks][3]);
     int koff[8];
     bool kval[8];
 #pragma unroll
@@ -149,8 +133,8 @@ __global__ void __launch_bounds__(256) stem_fused_kernel(const StemArgs a) {
         }
         // A fragment: {row g, k lo pair}, {row g+8, k lo pair}, {row g, k hi pair}, {row g+8, k hi pair}
         const uint32_t af[4] = {pack_bf16x2(v[0], v[1]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[6], v[7])};
-        mma16816(d[0], af, wf[ks][0], wf[ks][1]);
-        mma16816(d[1], af, wf[ks][2], wf[ks][3]);
+        ptx::mma_16816(d[0], af, wf[ks][0], wf[ks][1]);
+        ptx::mma_16816(d[1], af, wf[ks][2], wf[ks][3]);
       }
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
@@ -172,7 +156,7 @@ __global__ void __launch_bounds__(256) stem_fused_kernel(const StemArgs a) {
 
   // ---- phase 3: depthwise (diagonal-B MMAs) -> hswish -> pointwise MMA -> + residual
   {
-    // diagonal B fragments of the 9 taps for this lane (see mbconv_fused.cu): non-zero only where k == n
+    // diagonal B fragments of the 9 taps for this lane (explained at the top of mbconv_tc.cu): non-zero only where k == n
     uint32_t dlo[9], dhi[9];
 #pragma unroll
     for (int t = 0; t < 9; ++t) {
@@ -186,7 +170,7 @@ __global__ void __launch_bounds__(256) stem_fused_kernel(const StemArgs a) {
       dlo[t] = lo; dhi[t] = hi;
     }
     uint32_t pwf[4];
-    ldsm4(u_wp + b_n * SF_XRS + b_kh * 16, pwf[0], pwf[1], pwf[2], pwf[3]);
+    ptx::ldsm_x4(u_wp + b_n * SF_XRS + b_kh * 16, pwf[0], pwf[1], pwf[2], pwf[3]);
     bf16* ob = a.out + (long long)b * a.Ho * a.Wo * SF_C;
     for (int mt = warp; mt < SF_TH * (SF_TW / 16); mt += 8) {
       const int ry = mt >> 1, rx0 = (mt & 1) * 16;   // output row / first column inside the tile
@@ -195,7 +179,7 @@ __global__ void __launch_bounds__(256) stem_fused_kernel(const StemArgs a) {
       // of k8), tap 8 as m16n8k8: 10 MMAs per m-tile instead of 18
       auto frag = [&](int tap, uint32_t* af) {
         const int ky = tap / 3, kx = tap - ky * 3;
-        ldsm4(u_x + ((ry + ky) * SF_XW + rx0 + a_row + kx) * SF_XRS + a_kh * 16, af[0], af[1], af[2], af[3]);
+        ptx::ldsm_x4(u_x + ((ry + ky) * SF_XW + rx0 + a_row + kx) * SF_XRS + a_kh * 16, af[0], af[1], af[2], af[3]);
       };
 #pragma unroll
       for (int tp = 0; tp < 4; ++tp) {
@@ -203,14 +187,14 @@ __global__ void __launch_bounds__(256) stem_fused_kernel(const StemArgs a) {
         frag(2 * tp, fa); frag(2 * tp + 1, fb);
         const uint32_t a_lo[4] = {fa[0], fa[1], fb[0], fb[1]};
         const uint32_t a_hi[4] = {fa[2], fa[3], fb[2], fb[3]};
-        mma16816(d[0], a_lo, dlo[2 * tp], dlo[2 * tp + 1]);
-        mma16816(d[1], a_hi, dhi[2 * tp], dhi[2 * tp + 1]);
+        ptx::mma_16816(d[0], a_lo, dlo[2 * tp], dlo[2 * tp + 1]);
+        ptx::mma_16816(d[1], a_hi, dhi[2 * tp], dhi[2 * tp + 1]);
       }
       {
         uint32_t fa[4];
         frag(8, fa);
-        mma1688(d[0], fa[0], fa[1], dlo[8]);
-        mma1688(d[1], fa[2], fa[3], dhi[8]);
+        ptx::mma_1688(d[0], fa[0], fa[1], dlo[8]);
+        ptx::mma_1688(d[1], fa[2], fa[3], dhi[8]);
       }
       // hswish(dw + bias) -> A fragment of the pointwise MMA (C-fragment layout == A-fragment layout)
       uint32_t pa[4];
@@ -221,8 +205,8 @@ __global__ void __launch_bounds__(256) stem_fused_kernel(const StemArgs a) {
         pa[nt * 2 + 1] = pack_bf16x2(es3_act_t<ACT_HSWISH>(d[nt][2] + s_bdw[c]), es3_act_t<ACT_HSWISH>(d[nt][3] + s_bdw[c + 1]));
       }
       float o[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-      mma16816(o[0], pa, pwf[0], pwf[1]);
-      mma16816(o[1], pa, pwf[2], pwf[3]);
+      ptx::mma_16816(o[0], pa, pwf[0], pwf[1]);
+      ptx::mma_16816(o[1], pa, pwf[2], pwf[3]);
       const int oy = oy0 + ry;
 #pragma unroll
       for (int half = 0; half < 2; ++half) {

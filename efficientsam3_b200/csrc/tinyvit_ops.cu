@@ -7,23 +7,13 @@
 //   * LayerNorm over bf16 rows with arbitrary C % 8 == 0 (C = 448 is not a multiple of 128).
 #include <cuda_fp16.h>
 
-#include "common.cuh"
+#include "ptx.cuh"
 
 namespace es3 {
 namespace {
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
 __device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 }  // namespace
 
@@ -97,7 +87,7 @@ __global__ void __launch_bounds__(NT16 * 32 > 256 ? NT16 * 32 : 256) win_attn_bi
   uint32_t qf[2][4];
 #pragma unroll
   for (int ks = 0; ks < 2; ++ks)
-    ldsm4(u_q + (warp * 16 + a_row) * WA_RS + (ks * 16 + a_kh * 8) * 2, qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
+    ptx::ldsm_x4(u_q + (warp * 16 + a_row) * WA_RS + (ks * 16 + a_kh * 8) * 2, qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
   float s[2 * NT16][4];
 #pragma unroll
   for (int i = 0; i < 2 * NT16; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
@@ -106,9 +96,9 @@ __global__ void __launch_bounds__(NT16 * 32 > 256 ? NT16 * 32 : 256) win_attn_bi
 #pragma unroll
     for (int ks = 0; ks < 2; ++ks) {
       uint32_t b0, b1, b2, b3;
-      ldsm4(u_k + (np * 16 + b_n) * WA_RS + (ks * 16 + b_kh * 8) * 2, b0, b1, b2, b3);
-      mma16816(s[2 * np], qf[ks], b0, b1);
-      mma16816(s[2 * np + 1], qf[ks], b2, b3);
+      ptx::ldsm_x4(u_k + (np * 16 + b_n) * WA_RS + (ks * 16 + b_kh * 8) * 2, b0, b1, b2, b3);
+      ptx::mma_16816(s[2 * np], qf[ks], b0, b1);
+      ptx::mma_16816(s[2 * np + 1], qf[ks], b2, b3);
     }
   }
   // ---- + bias, mask, softmax (rows g, g+8)
@@ -164,8 +154,8 @@ __global__ void __launch_bounds__(NT16 * 32 > 256 ? NT16 * 32 : 256) win_attn_bi
     for (int np = 0; np < 2; ++np) {
       uint32_t b0, b1, b2, b3;
       ldsm4t(u_v + (ks * 16 + v_k) * WA_RS + (np * 16 + v_n) * 2, b0, b1, b2, b3);
-      mma16816(o[2 * np], pf[ks], b0, b1);
-      mma16816(o[2 * np + 1], pf[ks], b2, b3);
+      ptx::mma_16816(o[2 * np], pf[ks], b0, b1);
+      ptx::mma_16816(o[2 * np + 1], pf[ks], b2, b3);
     }
   }
   const float i0 = 1.f / l0, i1 = 1.f / l1;

@@ -21,6 +21,7 @@
 // Gradients of activations are bf16 (the reference's AMP path keeps them fp16), parameter gradients fp32 and ACCUMULATED
 // (+=) into their destination, all reductions are two-stage with a fixed order: no atomics, bit-reproducible.
 #include "col_reduce.cuh"
+#include "ptx.cuh"
 
 namespace es3 {
 namespace {
@@ -55,12 +56,6 @@ __device__ __forceinline__ void cpa_wait_all() { asm volatile("cp.async.commit_g
 __device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // ------------------------------------------------------------------------------------------ per-channel column reductions
@@ -405,8 +400,8 @@ __global__ void __launch_bounds__(256) wgrad_pw_kernel(const bf16* __restrict__ 
         ldsm4t(u + (p0 + bk_p) * Cfg::RS + Cfg::TN * 2 + np * 32 + bk_cb, b0, b1, b2, b3);
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) {
-          mma16816(acc[mt][2 * np], af[mt], b0, b1);
-          mma16816(acc[mt][2 * np + 1], af[mt], b2, b3);
+          ptx::mma_16816(acc[mt][2 * np], af[mt], b0, b1);
+          ptx::mma_16816(acc[mt][2 * np + 1], af[mt], b2, b3);
         }
       }
     }

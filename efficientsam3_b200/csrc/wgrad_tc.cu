@@ -21,8 +21,6 @@
 
 namespace es3 {
 
-int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b, const uint32_t* box);
-
 constexpr int WG_PX = 64;                 // pixels per stage (4 wgmma k-steps)
 constexpr int WG_TILE = WG_PX * 128;      // one [64 px][64 ch] tile: 8 KB
 constexpr int WG_STAGES = 4;

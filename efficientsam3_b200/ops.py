@@ -397,9 +397,8 @@ def litemla_attn_generic(ms, heads2, dim, eps=1e-15, return_kv=False):
     return (att, kv) if return_kv else att
 
 
-def mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, residual, act, impl=None):
-    """Fused MBConv (expand -> dw3x3 -> project [+x]); returns None when the shape is not instantiated.
-    impl: None = wgmma kernel where it applies, else the mma.sync kernel; "tc" / "mma" force one (None if not instantiated)."""
+def mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, residual, act):
+    """Fused MBConv (expand -> dw3x3 -> project [+x]) in one wgmma kernel; returns None when the shape is not instantiated."""
     _chk(x, torch.bfloat16, "x")
     _ensure_init(x)
     assert x.is_contiguous()
@@ -411,16 +410,8 @@ def mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, residual, act, impl
     args = (x.data_ptr(), y.data_ptr(), w1.data_ptr(), s1.data_ptr(), b1.data_ptr(), wdw.data_ptr(), b2.data_ptr(),
             w3.data_ptr(), s3.data_ptr(), b3.data_ptr(), B, H, W, Cin, Mid, Cout, stride, int(residual), ACT[act],
             _stream())
-    shape, nbytes, flops = f"[{Cin}-{Mid}-{Cout},s{stride}]", _nb(x, y), 2 * B * (H * W * Cin * Mid + Ho * Wo * Mid * (9 + Cout))
-    rc = -1
-    if impl in (None, "tc"):
-        rc = _call_rc("es3_mbconv_tc_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
-        if rc < 0:
-            rc = _call_rc("es3_mbconv_tc_s2_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
-        if rc < 0:
-            rc = _call_rc("es3_mbconv_tc_wide_bf16", "mbconv_tc" + shape, nbytes, flops, *args)
-    if rc < 0 and impl != "tc":
-        rc = _call_rc("es3_mbconv_fused_bf16", "mbconv_fused" + shape, nbytes, flops, *args)
+    rc = _call_rc("es3_mbconv_bf16", f"mbconv_tc[{Cin}-{Mid}-{Cout},s{stride}]", _nb(x, y),
+                  2 * B * (H * W * Cin * Mid + Ho * Wo * Mid * (9 + Cout)), *args)
     return y if rc == 0 else None
 
 

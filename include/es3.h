@@ -94,31 +94,17 @@ int es3_stem_fused_c16(const float* img, const void* w0, const float* s0, const 
                        int W, void* stream);
 
 /* Whole MBConv block in one kernel: y = [x +] BN3(pw2(act(BN2(dw3x3_s(act(BN1(pw1(x)))))))) with the 4x-expanded
- * tensor kept in shared memory (mma.sync expand/project around an fp32 depthwise).  w1 [Mid][Cin], w3 [Cout][Mid]
- * bf16; s1,b1,b2 [Mid], s3,b3 [Cout] fp32 (BN folded; ones/zeros where the reference has bias-only convs);
- * wdw [9][Mid] fp32.  Returns -1 (no error set) when the shape is not instantiated -- the caller then runs
- * es3_gemm_bf16 + es3_dwconv_tc_bf16 / es3_dwconv_tiled_bf16.  Replaces MBConv inside ResidualBlock (efficientvit/nn/ops.py:315-367,
- * 740-770) for efficientvit_b1 stages 1-3 heads. */
-int es3_mbconv_fused_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
-                          const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W,
-                          int Cin, int Mid, int Cout, int stride, int residual, int act, void* stream);
-/* Same contract on wgmma for the stride-1 residual blocks (Cin == Cout in {32, 64}, Mid = 4 Cin, hardswish): the two
- * pointwise GEMMs are warpgroup MMAs (TMA-staged 128B-swizzled operands, register accumulators, project accumulating over
- * 64-channel chunks), the depthwise stays on mma.sync with diagonal B fragments.  Returns -1 for any other shape. */
-int es3_mbconv_tc_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
-                       const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin, int Mid,
-                       int Cout, int stride, int residual, int act, void* stream);
-/* Same contract on wgmma for the stride-2, no-residual blocks (Cin, Mid, Cout) in {(16,64,32), (32,128,64), (64,256,128)}:
- * 4 x 16 output tiles, 9 x 33 input tiles = five 64-row wgmma blocks, 32-channel chunks.  Returns -1 for any other shape. */
-int es3_mbconv_tc_s2_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
-                          const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
-                          int Mid, int Cout, int stride, int residual, int act, void* stream);
-/* Same contract on the same two kernels for the Cin-128 hardswish blocks: (128, 512, 128) stride 1 with residual and
- * (128, 512, 256) stride 2 without (efficientvit_b1 stage 3 and the stage-4 opener, efficientvit_b0 stage 4), their input tile
- * held as two 64-channel slabs, one CTA per SM.  Returns -1 for any other shape. */
-int es3_mbconv_tc_wide_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
-                            const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
-                            int Mid, int Cout, int stride, int residual, int act, void* stream);
+ * tensor kept on the SM: the two pointwise GEMMs are warpgroup MMAs (TMA-staged 128B-swizzled operands, register accumulators,
+ * project accumulating over chunks of the expanded channels), the depthwise runs on mma.sync with diagonal B fragments.
+ * w1 [Mid][Cin], w3 [Cout][Mid] bf16; s1,b1,b2 [Mid], s3,b3 [Cout] fp32 (BN folded; ones/zeros where the reference has
+ * bias-only convs); wdw [9][Mid] fp32.  Instantiated for hardswish and (Cin, Mid, Cout) in {(32,128,32), (64,256,64),
+ * (128,512,128)} at stride 1 with residual, {(16,64,32), (32,128,64), (64,256,128), (128,512,256)} at stride 2 without.
+ * Returns -1 (no error set, nothing written) for any other shape or act -- the caller then runs es3_gemm_bf16 +
+ * es3_dwproj_tc_bf16 / es3_dwconv_tc_bf16 / es3_dwconv_tiled_bf16.  Replaces MBConv inside ResidualBlock
+ * (efficientvit/nn/ops.py:315-367, 740-770) for the efficientvit_b0 / b1 blocks up to Cin 128. */
+int es3_mbconv_bf16(const void* x, void* y, const void* w1, const float* s1, const float* b1, const float* wdw,
+                    const float* b2, const void* w3, const float* s3, const float* b3, int B, int H, int W, int Cin,
+                    int Mid, int Cout, int stride, int residual, int act, void* stream);
 /* Depthwise 3x3 (stride 1) + bias + hardswish + pointwise projection + BN (+ residual) in one wgmma kernel, for MBConv blocks
  * whose expanded tensor is too wide for the fully fused kernels (EfficientViT stages 3/4): mid [B,H,W,Mid] bf16 is TMA-staged in
  * 64-channel chunks with its halo, the depthwise runs as diagonal m16n8k8 MMAs, its output goes straight into the swizzled A

@@ -92,7 +92,7 @@ def bench_case(ops, name, kind, cin, mid, cout, stride, side, B, seconds, dev, s
         s1 = (torch.rand(mid, generator=g) + 0.5).to(dev)
         b1 = (torch.randn(mid, generator=g) * 0.2).to(dev)
         res = stride == 1
-        run = lambda: ops.mbconv_fused(x, w1, s1, b1, wdw9, b2, w3, s3, b3, stride, res, "hswish", impl="tc")
+        run = lambda: ops.mbconv_fused(x, w1, s1, b1, wdw9, b2, w3, s3, b3, stride, res, "hswish")
         nbytes = 2 * (x.numel() + B * Ho * Wo * cout)
         xn = x.float().permute(0, 3, 1, 2)
         e = F.hardswish(F.conv2d(xn, w1.float()[:, :, None, None]) * s1.view(1, -1, 1, 1) + b1.view(1, -1, 1, 1))

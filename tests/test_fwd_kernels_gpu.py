@@ -1,4 +1,4 @@
-"""The image students' forward kernels (mbconv_fused.cu, mbconv_tc.cu, mbconv_tc_s2.cu, dwproj_tc.cu, dw_tc.cu, dw_tiled.cu, the
+"""The image students' forward kernels (mbconv_tc.cu, mbconv_tc_s2.cu, dwproj_tc.cu, dw_tc.cu, dw_tiled.cu, the
 forward kernels of conv.cu, stem_fused.cu, litemla_tc.cu, litemla.cu, repvit_ops.cu, tinyvit_ops.cu), element by element against
 the fp64 statements of tests/ref_fwd.py, each output element within its own bound.
 
@@ -14,7 +14,7 @@ GAMMA = 2 (ref_train_bwd.GAMMA) holds without change.  Worst err/bound per secti
 limit): fp32 outputs -- LiteMLA KV partials 0.0081 (generic) and 0.0015 (tensor core), channel_mean 0.0044, bilinear 0.0041;
 bf16 outputs -- 0.95 ... 0.996 in every other section (depthwise, MBConv, dwproj, stems, aggreg, LiteMLA, LayerNorm, window
 attention, scale_channels; LiteMLA tc 0.88), where the output's own rounding half-step dominates the bound and is reached.  The
-whole file (330 tests, the route-closure forwards and training steps included) took 24 s there.
+whole file (319 tests, the route-closure forwards and training steps included) took 34 s there.
 """
 import math
 
@@ -96,9 +96,8 @@ def ln_key(C):
 def route_key(name, a):
     """Route key of one recorded es3_* forward call: the instantiation its arguments select (None: not a kernel of this file)."""
     act = {v: k for k, v in ACT.items()}
-    mb = {"es3_mbconv_fused_bf16": "mbconv_fused", "es3_mbconv_tc_bf16": "mbconv_tc", "es3_mbconv_tc_s2_bf16": "mbconv_tc_s2"}
-    if name in mb:
-        return (mb[name], a[13], a[14], a[15], a[16])
+    if name == "es3_mbconv_bf16":
+        return ("mbconv_tc" if a[16] == 1 else "mbconv_tc_s2", a[13], a[14], a[15], a[16])
     if name == "es3_dwproj_tc_bf16":
         return ("dwproj", a[11], a[12])
     if name == "es3_dwconv_tc_bf16":
@@ -213,14 +212,15 @@ def _mb_weights(cuda, cin, mid, cout, g):
     return w1, s1, b1, wdw, b2, w3, s3, b3
 
 
-def _mb_call(lib, fn, x, y, wt, taps, cin, mid, cout, stride, res):
+def _mb_call(lib, x, y, wt, taps, cin, mid, cout, stride, res, act="hswish"):
     w1, s1, b1, _, b2, w3, s3, b3 = wt
     B, H, W = x.shape[:3]
-    return lib.call_rc(fn, x.data_ptr(), y.data_ptr(), w1.data_ptr(), s1.data_ptr(), b1.data_ptr(), taps.data_ptr(), b2.data_ptr(),
-                       w3.data_ptr(), s3.data_ptr(), b3.data_ptr(), B, H, W, cin, mid, cout, stride, int(res), ACT["hswish"], _st())
+    return lib.call_rc("es3_mbconv_bf16", x.data_ptr(), y.data_ptr(), w1.data_ptr(), s1.data_ptr(), b1.data_ptr(), taps.data_ptr(),
+                       b2.data_ptr(), w3.data_ptr(), s3.data_ptr(), b3.data_ptr(), B, H, W, cin, mid, cout, stride, int(res), ACT[act],
+                       _st())
 
 
-def _mb_case(cuda, fn, impl, cin, mid, cout, stride, B, H, W):
+def _mb_case(cuda, cin, mid, cout, stride, B, H, W):
     lib = _lib(cuda)
     g = _gen(cuda, "mb", cin, mid, cout, stride, B, H, W)
     x = _bf(torch.randn(B, H, W, cin, device=cuda, generator=g))
@@ -231,78 +231,79 @@ def _mb_case(cuda, fn, impl, cin, mid, cout, stride, B, H, W):
     buf, inside = _flat_out(B * Ho * Wo * cout, torch.bfloat16, cuda)
 
     def run(o):
-        assert _mb_call(lib, fn, x, o, wt, taps, cin, mid, cout, stride, res) == 0
+        assert _mb_call(lib, x, o, wt, taps, cin, mid, cout, stride, res) == 0
     got = _twice(run, buf)
     y = got[:B * Ho * Wo * cout].view(B, Ho, Wo, cout)
     w1, s1, b1, _, b2, w3, s3, b3 = (t.double() for t in wt)
     ref, bound, _, _ = R.mbconv(x.double(), w1, s1, b1, taps.double(), b2, w3, s3, b3, stride, res)
-    what = f"{fn} ({cin},{mid},{cout},s{stride}) B{B} {H}x{W}"
-    _check(f"3 {fn}", y, ref, bound, what)
+    what = f"es3_mbconv_bf16 ({cin},{mid},{cout},s{stride}) B{B} {H}x{W}"
+    _check(f"3 es3_mbconv_bf16 s{stride}", y, ref, bound, what)
     _assert_untouched(got, inside, what)
     from efficientsam3_b200 import ops
-    _bits_equal(ops.mbconv_fused(x, *wt[:3], wt[3].clone(), *wt[4:], stride, res, "hswish", impl=impl), y, "ops.mbconv_fused vs direct")
+    _bits_equal(ops.mbconv_fused(x, *wt[:3], wt[3].clone(), *wt[4:], stride, res, "hswish"), y, "ops.mbconv_fused vs direct")
     return x, wt, taps, y
 
 
 GEO = {1: [(2, 3, 5), (2, 1, 37), (2, 1, 1), (2, 17, 33), (2, 9, 17), (2, 7, 15), (1, 8, 16), (24, 37, 37)],
        2: [(2, 3, 5), (2, 1, 37), (2, 1, 1), (2, 17, 33), (2, 18, 34), (2, 7, 31), (1, 8, 32), (40, 37, 37)]}
-MB_FUSED = [(16, 64, 32, 2), (32, 128, 32, 1), (32, 128, 64, 2), (64, 256, 64, 1), (64, 256, 128, 2)]
-MB_TC = [(32, 128, 32, 1), (64, 256, 64, 1)]
-MB_S2 = [(16, 64, 32, 2), (32, 128, 64, 2), (64, 256, 128, 2)]
+# Cin 128 (input tile held as two 64-channel slabs): 1 x 1, below one tile, one tile (stride 1: 8 x 16 output, stride 2: 8 x 32
+# input) and one pixel past it, the ragged 63 x 63 that 1008-px inputs give, and the EV-M shape of bench.py (64 x 64 at batch 32)
+GEO_CIN128 = {1: [(2, 1, 1), (2, 3, 5), (2, 1, 37), (1, 8, 16), (2, 7, 15), (2, 9, 17), (2, 63, 63), (32, 64, 64)],
+              2: [(2, 1, 1), (2, 3, 5), (2, 1, 37), (1, 8, 32), (2, 7, 31), (2, 10, 34), (2, 63, 63), (32, 64, 64)]}
+MB_TC = [(32, 128, 32, 1), (64, 256, 64, 1), (128, 512, 128, 1)]
+MB_S2 = [(16, 64, 32, 2), (32, 128, 64, 2), (64, 256, 128, 2), (128, 512, 256, 2)]
 
 
 def _mb_rows(blocks):
-    return [blk + geo for blk in blocks for geo in GEO[blk[3]]]
-
-
-@pytest.mark.parametrize("cin,mid,cout,stride,B,H,W", _mb_rows(MB_FUSED))
-def test_mbconv_fused_mma(cuda, cin, mid, cout, stride, B, H, W):
-    """All five ES3_MB instantiations of the mma.sync kernel (TH x 16 tiles, TH = 8 | 4): H, W of 1, less than a tile, tile +- 1,
-    odd; a batch of 24 / 40 images."""
-    _mb_case(cuda, "es3_mbconv_fused_bf16", "mma", cin, mid, cout, stride, B, H, W)
+    return [blk + geo for blk in blocks for geo in (GEO_CIN128 if blk[0] == 128 else GEO)[blk[3]]]
 
 
 @pytest.mark.parametrize("cin,mid,cout,stride,B,H,W", _mb_rows(MB_TC))
 def test_mbconv_tc(cuda, cin, mid, cout, stride, B, H, W):
     """The wgmma stride-1 residual kernel, 8 x 16 tiles: one-pixel edge tiles, images below one tile, and batches large enough that
     every persistent CTA runs tiles of several images (the rows of the former tile-geometry test, under per-element bounds)."""
-    _mb_case(cuda, "es3_mbconv_tc_bf16", "tc", cin, mid, cout, stride, B, H, W)
+    _mb_case(cuda, cin, mid, cout, stride, B, H, W)
 
 
 @pytest.mark.parametrize("cin,mid,cout,stride,B,H,W", _mb_rows(MB_S2))
 def test_mbconv_tc_s2(cuda, cin, mid, cout, stride, B, H, W):
     """The wgmma stride-2 kernel, 4 x 16 tiles over 9 x 33 input tiles: the expand rows past S2_PIN of the last 64-row block go to
     the scratch slot; W = 33 / 34 / 37 put real pixels in the last input column of a tile."""
-    _mb_case(cuda, "es3_mbconv_tc_s2_bf16", "tc", cin, mid, cout, stride, B, H, W)
+    _mb_case(cuda, cin, mid, cout, stride, B, H, W)
 
 
-@pytest.mark.parametrize("fn,blk,B", [("es3_mbconv_fused_bf16", (32, 128, 32, 1), 24), ("es3_mbconv_tc_bf16", (64, 256, 64, 1), 24),
-                                      ("es3_mbconv_tc_s2_bf16", (32, 128, 64, 2), 40), ("es3_mbconv_fused_bf16", (64, 256, 128, 2), 40),
-                                      ("es3_mbconv_tc_s2_bf16", (64, 256, 128, 2), 40)])
-def test_mbconv_batch_invariant(cuda, fn, blk, B):
+@pytest.mark.parametrize("blk", MB_TC + MB_S2)
+def test_mbconv_batch_invariant(cuda, blk):
     """Image i of a batch is bit-identical to image i run alone (state leaking between the tiles of a persistent CTA would not be)."""
-    impl = "mma" if fn == "es3_mbconv_fused_bf16" else "tc"
-    x, wt, taps, y = _mb_case(cuda, fn, impl, *blk, B, 37, 37)
+    B = 24 if blk[3] == 1 else 40
+    x, wt, taps, y = _mb_case(cuda, *blk, B, 37, 37)
     lib = _lib(cuda)
     for i in (0, B // 2, B - 1):
         one = torch.full_like(y[i:i + 1], float("nan"))
-        assert _mb_call(lib, fn, x[i:i + 1].contiguous(), one, wt, taps, *blk, blk[3] == 1) == 0
-        _bits_equal(one[0], y[i], f"{fn} image {i} of {B} vs alone")
+        assert _mb_call(lib, x[i:i + 1].contiguous(), one, wt, taps, *blk, blk[3] == 1) == 0
+        _bits_equal(one[0], y[i], f"es3_mbconv_bf16 {blk} image {i} of {B} vs alone")
 
 
-@pytest.mark.parametrize("fn,blk", [("es3_mbconv_fused_bf16", (48, 192, 48, 1)), ("es3_mbconv_fused_bf16", (32, 128, 32, 2)),
-                                    ("es3_mbconv_tc_bf16", (32, 128, 64, 2)), ("es3_mbconv_tc_bf16", (48, 192, 48, 1)),
-                                    ("es3_mbconv_tc_s2_bf16", (32, 128, 32, 1)), ("es3_mbconv_tc_s2_bf16", (64, 256, 64, 2))])
-def test_mbconv_declined_shapes_write_nothing(cuda, fn, blk):
+# Shapes es3_mbconv_bf16 declines: uninstantiated blocks, instantiated blocks at the other stride or residual setting, and every
+# instantiated block with an activation other than hardswish
+MB_DECLINED = [((48, 192, 48, 1), True, "hswish"), ((32, 128, 32, 2), False, "hswish"), ((64, 256, 64, 2), False, "hswish"),
+               ((256, 1024, 256, 1), True, "hswish"), ((128, 256, 128, 1), True, "hswish"), ((128, 512, 128, 2), False, "hswish"),
+               ((128, 512, 256, 1), True, "hswish"), ((32, 128, 32, 1), False, "hswish"), ((128, 512, 128, 1), False, "hswish"),
+               ((128, 512, 256, 2), True, "hswish")]
+MB_DECLINED += [(blk, blk[3] == 1, (None, "relu", "gelu")[i % 3]) for i, blk in enumerate(MB_TC + MB_S2)]
+
+
+@pytest.mark.parametrize("blk,res,act", MB_DECLINED)
+def test_mbconv_declined_shapes_write_nothing(cuda, blk, res, act):
     lib = _lib(cuda)
     cin, mid, cout, stride = blk
-    g = _gen(cuda, "decl", fn, blk)
+    g = _gen(cuda, "decl", blk, res, act)
     x = _bf(torch.randn(1, 9, 9, cin, device=cuda, generator=g))
     wt = _mb_weights(cuda, cin, mid, cout, g)
     buf, inside = _flat_out(81 * cout, torch.bfloat16, cuda)
-    assert _mb_call(lib, fn, x, buf, wt, wt[3], cin, mid, cout, stride, stride == 1) == -1
+    assert _mb_call(lib, x, buf, wt, wt[3], cin, mid, cout, stride, res, act) == -1
     torch.cuda.synchronize()
-    _assert_untouched(buf, torch.zeros_like(inside), f"{fn} declined {blk}")
+    _assert_untouched(buf, torch.zeros_like(inside), f"es3_mbconv_bf16 declined {blk} residual={res} act={act}")
 
 
 DWP = [(mid, cout, res, geo) for mid, cout in ((512, 128), (1024, 256)) for res in (True, False)
@@ -636,7 +637,7 @@ def covered_keys():
     keys = {dw_tc_key(c[0][0], c[0][1], c[1]) for c in DWTC}
     keys |= {("dw_tiled", 3, 2, c[1]) for c in DWT}
     keys |= {("dw", c[0][0], c[0][1], c[1]) for c in DWG}
-    for fn, blocks in (("mbconv_fused", MB_FUSED), ("mbconv_tc", MB_TC), ("mbconv_tc_s2", MB_S2)):
+    for fn, blocks in (("mbconv_tc", MB_TC), ("mbconv_tc_s2", MB_S2)):
         keys |= {(fn,) + blk for blk in blocks}
     keys |= {("dwproj", c[0], c[1]) for c in DWP}
     keys |= {("stem", c[0], c[1]) for c in STEM} | {("dsconv", c[0], c[1]) for c in DSC}
@@ -651,8 +652,15 @@ def covered_keys():
 @pytest.mark.parametrize("name", STUDENTS)
 def test_route_closure(cuda, monkeypatch, name):
     """Every forward-kernel route `name` reaches in the eval forward at 1024^2 (batch 2) and in one native training step (1024^2,
-    embed 64, batch 1) with batch-statistics and with frozen BatchNorm is run by some table row above."""
+    embed 64, batch 1) with batch-statistics and with frozen BatchNorm is run by some table row above.  The eval forward of
+    efficientvit_b1 runs both Cin-128 MBConv blocks (its stage-3 blocks and stage-4 opener), that of efficientvit_b0 the stride-1
+    one (its stage-4 blocks)."""
     calls = eval_forward_calls(cuda, monkeypatch, name)
+    cin128 = {route_key(n, a) for n, a in calls if n == "es3_mbconv_bf16" and a[13] == 128}
+    expected = {"efficientvit_b1": {("mbconv_tc",) + MB_TC[2], ("mbconv_tc_s2",) + MB_S2[3]},
+                "efficientvit_b0": {("mbconv_tc",) + MB_TC[2]}}.get(name)
+    if expected is not None:
+        assert cin128 == expected, f"{name}: Cin-128 MBConv routes {sorted(cin128)}, expected {sorted(expected)}"
     for frozen in (False, True):
         calls += training_step_calls(cuda, monkeypatch, name, frozen)
     reached = {k for k in (route_key(n, a) for n, a in calls) if k is not None}

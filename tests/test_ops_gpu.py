@@ -287,10 +287,9 @@ def test_cpu_tensor_is_an_error():
     (16, 64, 32, 2, False, 64, 64), (32, 128, 32, 1, True, 40, 48), (32, 128, 64, 2, False, 33, 47),
     (64, 256, 64, 1, True, 31, 17), (64, 256, 128, 2, False, 64, 64), (16, 64, 32, 2, False, 63, 65),
     (64, 256, 64, 1, True, 128, 128), (32, 128, 32, 1, True, 8, 16), (64, 256, 128, 2, False, 37, 29), (32, 128, 64, 2, False, 130, 66)])
-@pytest.mark.parametrize("impl", ["mma", "tc"])
-def test_mbconv_fused(cuda, cin, mid, cout, stride, res, H, W, impl):
-    """One-kernel MBConv (mma.sync kernel / wgmma kernel) vs the op-by-op fp32 statement (intermediates rounded to bf16
-    where the unfused native path would materialise them)."""
+def test_mbconv_fused(cuda, cin, mid, cout, stride, res, H, W):
+    """One-kernel MBConv vs the op-by-op fp32 statement (intermediates rounded to bf16 where the unfused native path would
+    materialise them)."""
     from efficientsam3_b200 import ops
     g = torch.Generator().manual_seed(cin + mid + H)
     B = 2
@@ -300,7 +299,7 @@ def test_mbconv_fused(cuda, cin, mid, cout, stride, res, H, W, impl):
     wdw = (torch.randn(mid, 1, 3, 3, generator=g) / 3).to(cuda); b2 = (torch.randn(mid, generator=g) * 0.2).to(cuda)
     w3 = _bf(torch.randn(cout, mid, generator=g) / math.sqrt(mid)).to(cuda)
     s3 = (torch.rand(cout, generator=g) + 0.5).to(cuda); b3 = (torch.randn(cout, generator=g) * 0.2).to(cuda)
-    y = ops.mbconv_fused(x, w1, s1, b1, wdw.reshape(mid, 9).t().contiguous(), b2, w3, s3, b3, stride, res, "hswish", impl=impl)
+    y = ops.mbconv_fused(x, w1, s1, b1, wdw.reshape(mid, 9).t().contiguous(), b2, w3, s3, b3, stride, res, "hswish")
     assert y is not None
     xn = x.float().permute(0, 3, 1, 2)
     e = F.hardswish(F.conv2d(xn, w1.float()[:, :, None, None]) * s1.view(1, -1, 1, 1) + b1.view(1, -1, 1, 1))
@@ -358,7 +357,7 @@ def test_fused_wgmma_kernels_are_bit_reproducible(cuda, kind, cin, mid, cout, st
         x = _bf(torch.randn(B, H, W, cin, generator=g)).to(cuda)
         w1 = _bf(torch.randn(mid, cin, generator=g) / math.sqrt(cin)).to(cuda)
         s1 = (torch.rand(mid, generator=g) + 0.5).to(cuda); b1 = (torch.randn(mid, generator=g) * 0.2).to(cuda)
-        run = lambda: ops.mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, stride == 1, "hswish", impl="tc")
+        run = lambda: ops.mbconv_fused(x, w1, s1, b1, wdw, b2, w3, s3, b3, stride, stride == 1, "hswish")
     first = run()
     assert first is not None
     first = first.clone()

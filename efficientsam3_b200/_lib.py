@@ -27,7 +27,7 @@ SIGNATURES: dict[str, list] = {
     "es3_attention_tc_bf16": [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
     "es3_attention_mma_bf16": [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
     "es3_attention_causal_bf16": [_vp, _vp, _i, _i, _i, _i, _f, _vp],
-    "es3_text_embed": [_vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
+    "es3_text_embed": [_vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp],
     "es3_repmixer_bf16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp],
     # text-student backward and text KD loss (text_bwd.cu)
     "es3_text_attn_bwd": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp],

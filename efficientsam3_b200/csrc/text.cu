@@ -10,7 +10,7 @@ namespace es3 {
 // [0, vocab) still never reads outside the table here (its row is written as zeros).
 __global__ void text_embed_kernel(const long long* __restrict__ ids, const float* __restrict__ table, int vocab,
                                   const float* __restrict__ pos, float* __restrict__ x, float* __restrict__ emb,
-                                  int emb_with_pos, int L, int C4, long long n4) {
+                                  int L, int C4, long long n4) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     const long long tok = i / C4;
     const int c4 = (int)(i - tok * C4);
@@ -23,7 +23,7 @@ __global__ void text_embed_kernel(const long long* __restrict__ ids, const float
       y = make_float4(t.x + p.x, t.y + p.y, t.z + p.z, t.w + p.w);
     }
     reinterpret_cast<float4*>(x)[i] = y;
-    if (emb != nullptr) reinterpret_cast<float4*>(emb)[i] = emb_with_pos ? y : t;
+    if (emb != nullptr) reinterpret_cast<float4*>(emb)[i] = t;
   }
 }
 
@@ -74,13 +74,13 @@ __global__ void __launch_bounds__(RM_THREADS) repmixer_kernel(const float* __res
 
 using namespace es3;
 
-extern "C" int es3_text_embed(const long long* ids, const float* table, int vocab, const float* pos, float* x, float* emb,
-                              int emb_with_pos, int B, int L, int C, void* stream) {
+extern "C" int es3_text_embed(const long long* ids, const float* table, int vocab, const float* pos, float* x, float* emb, int B,
+                              int L, int C, void* stream) {
   ES3_REQUIRE(B >= 1 && L >= 1 && C >= 4 && C % 4 == 0, "es3_text_embed: need B, L >= 1 and C %% 4 == 0 (B=%d L=%d C=%d)", B, L, C);
   ES3_REQUIRE(vocab >= 1, "es3_text_embed: empty table");
   const long long n4 = (long long)B * L * (C / 4);
   const int grid = (int)((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
-  text_embed_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ids, table, vocab, pos, x, emb, emb_with_pos, L, C / 4, n4);
+  text_embed_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ids, table, vocab, pos, x, emb, L, C / 4, n4);
   ES3_LAUNCH_CHECK("text_embed_kernel");
   return 0;
 }

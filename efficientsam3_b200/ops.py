@@ -494,7 +494,7 @@ def text_embed(ids, table, pos=None, emb="none"):
     x = torch.empty((B * L, C), device=table.device, dtype=torch.float32)
     e = torch.empty_like(x) if emb == "plain" else None
     _call("es3_text_embed", "text_embed", _nb(ids, x, e, pos) + B * L * C * 4, 0, ids.data_ptr(), table.data_ptr(), V, _ptr(pos),
-          x.data_ptr(), _ptr(e), 0, B, L, C, _stream())
+          x.data_ptr(), _ptr(e), B, L, C, _stream())
     return x, (x if emb == "pos" else e)
 
 

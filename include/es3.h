@@ -200,12 +200,12 @@ long long es3_attention_fp8_ws_floats(int B, int H, int W, int num_heads, int wi
  * H = 1, W = L, win = 0. */
 int es3_attention_causal_bf16(const void* qkv, void* out, int B, int L, int C, int num_heads, float scale, void* stream);
 /* Token embedding: x[b*L+l] = table[ids[b,l]] (+ pos[l]) as fp32 [B*L, C] (the residual stream); emb (optional) receives
- * the positional-added rows (emb_with_pos = 1, MobileCLIP forward_embedding, mobile_clip.py:815-823) or the plain table
- * rows (0, the VE teacher's inputs_embeds, text_encoder_ve.py:303).  ids int64 (device), table [vocab, C] fp32, pos
+ * the plain table rows (the VE teacher's inputs_embeds, text_encoder_ve.py:303; MobileCLIP's forward_embedding returns x
+ * itself, mobile_clip.py:815-823).  ids int64 (device), table [vocab, C] fp32, pos
  * [L, C] fp32 or NULL; C % 4 == 0.  Callers validate ids against vocab on the host; an id outside the table is never
  * dereferenced (its row reads as zeros). */
-int es3_text_embed(const long long* ids, const float* table, int vocab, const float* pos, float* x, float* emb, int emb_with_pos,
-                   int B, int L, int C, void* stream);
+int es3_text_embed(const long long* ids, const float* table, int vocab, const float* pos, float* x, float* emb, int B, int L,
+                   int C, void* stream);
 /* RepMixerBlock prologue, eval mode (mobile_clip.py:545-702), over x [B*L, C] fp32 tokens (sequence axis = the conv's W):
  * x1 = bm + sum_k wm[k] x[l+k-5] (RepMixer with BN_skip, BN(conv 1x11), identity and layer scale folded into the
  * taps wm [11][C] and bias bm [C], zero padding) in fp32, then u = bf + sum_k wf[k] x1[l+k-5] (ConvFFN.conv: depthwise

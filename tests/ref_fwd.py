@@ -227,14 +227,17 @@ def scale_channels(x, gate):
     return ref, _out(ref, U * ref.abs(), True)
 
 
-def layernorm(x, gamma, beta, eps):
+def layernorm(x, gamma, beta, eps, bf16=True, e_x=None):
     """es3_layernorm_bf16 over rows x [M, C]: mean = fl(sum) / C, q = sum (x - mean)^2, rstd = rsqrtf(q / C + eps) (2 ulp),
-    y = fmaf((x - mean) rstd, gamma, beta), bf16 store."""
+    y = fmaf((x - mean) rstd, gamma, beta), bf16 store; bf16 = False: the fp32 store of es3_layernorm_f32 (which multiplies by
+    fl(1 / C): one more rounding of the mean).  e_x: a per-element error already in the kernel's x (the rounding of its pos add)."""
     C = x.shape[1]
     mu = x.mean(1, keepdim=True)
-    e_mu = GAMMA * C * U * x.abs().mean(1, keepdim=True) + U * mu.abs()
+    e_mu = GAMMA * C * U * x.abs().mean(1, keepdim=True) + (U if bf16 else 2 * U) * mu.abs()
+    if e_x is not None:
+        e_mu = e_mu + e_x.mean(1, keepdim=True)
     d = x - mu
-    e_d = e_mu + U * d.abs()
+    e_d = e_mu + U * d.abs() + (0.0 if e_x is None else e_x)
     q = (d * d).sum(1, keepdim=True)
     e_q = (2 * d.abs() * e_d).sum(1, keepdim=True) + GAMMA * (C + 1) * U * q
     var = q / C + eps
@@ -244,7 +247,7 @@ def layernorm(x, gamma, beta, eps):
     xh = d * rstd
     e_xh = d.abs() * e_rstd + rstd * e_d + U * xh.abs()
     ref = xh * gamma + beta
-    return ref, _out(ref, gamma.abs() * e_xh + U * ref.abs(), True)
+    return ref, _out(ref, gamma.abs() * e_xh + U * ref.abs(), bf16)
 
 
 def win_tokens(B, H, W, ws):
@@ -258,29 +261,77 @@ def win_tokens(B, H, W, ws):
     return torch.where(idx[None] >= 0, idx[None] + off, torch.full_like(idx[None], -1)).reshape(B * nH * nW, ws * ws)
 
 
+EX2_REL = 4 * U                 # ex2.approx.ftz.f32: 2 ulp of the result (CUDA C++ Programming Guide, intrinsic functions: exp2f's
+#                                ex2.approx path; __expf = ex2.approx(x log2 e) is listed at 2 + floor(1.173 |x|) ulp, the |x| part
+#                                being the product's rounding); an ulp is 2^-23 relative, i.e. 2u
+
+
+def softmax_attn(q, k, v, scale, bias=None, causal=False, ex2=False, kv_tile=None):
+    """Flash-style softmax attention over q [..., N, d], k, v [..., Nk, d] (heads in the leading axes): s = scale q k^T (+ bias)
+    (+ -inf above the diagonal when causal), p = exp(s - rowmax) in fp32, P = bf16(p) into PV, l = sum of the fp32 p,
+    y = (P v) / l.  Returns (y, bound on |y32 - y| before the output's own rounding).
+
+    ex2 = False: p = __expf(fl(scale s32) + bias - m) (the window-attention kernels).  ex2 = True: the exponent is ex2.approx of an
+    fp32 argument in log2 units -- fl(fl(s32 c) - m) with c = fl(scale log2 e) (attn_fwd_kernel, mma.sync) or fmaf(s32, c, -m),
+    m = fl(rowmax s32 c) (attn_tc_kernel, wgmma): each of s32 c and m is within scale e_raw + 2u |s| of its exact value, the
+    subtraction or fma rounds once (u |arg|), ex2 adds EX2_REL.
+    kv_tile: the kernel's KV tile (online softmax): the running max, the corr = exp(m_old - m_new) rescale of l and of the P v
+    accumulator, and the bf16 rounding of P against the running max of its tile.  Each rescale adds one rounding (corr's ex2 and
+    its argument, then the product: 8u per tile to l and to P v); a tile after which the running max may still rise has its P
+    rounded against that tile's max, not the row's, so its elements are charged a full bf16 rounding (2^-8 p) rather than band()."""
+    d = q.shape[-1]
+    raw = q @ k.transpose(-1, -2)
+    s = scale * raw
+    e_raw = abs(scale) * GAMMA * d * U * (q.abs() @ k.abs().transpose(-1, -2))
+    if bias is not None:
+        s = s + bias
+    e_s = e_raw + U * s.abs() if not ex2 else e_raw + 2 * U * s.abs()
+    masked = None
+    if causal:
+        N, Nk = s.shape[-2:]
+        masked = torch.ones(N, Nk, dtype=torch.bool, device=s.device).triu(1)
+        s = s.masked_fill(masked, float("-inf"))
+        e_s = e_s.masked_fill(masked, 0.0)
+    mx = s.amax(-1, keepdim=True)
+    arg = s - mx
+    p = torch.exp(arg)
+    if ex2:
+        delta = e_s + e_s.amax(-1, keepdim=True) + U * arg.abs() + EX2_REL
+    else:
+        delta = e_s + 2 * e_s.amax(-1, keepdim=True) + U * arg.abs() + 2 * U * (2 + 1.16 * arg.abs())   # relative error of each p
+    if masked is not None:
+        delta = delta.masked_fill(masked, 0.0)
+    Nk = s.shape[-1]
+    nt = 1 if kv_tile is None else -(-Nk // kv_tile)
+    rescale = 8 * U * (nt - 1)
+    l = p.sum(-1, keepdim=True)
+    rel_l = (p * delta).sum(-1, keepdim=True) / l + GAMMA * Nk * U + rescale
+    P, dev = band(p, p * delta)
+    if nt > 1:
+        err = (delta.amax(-1, keepdim=True) + U * mx.abs()).expand_as(s)
+        tile = torch.arange(Nk, device=s.device) // kv_tile
+        for t in range(nt - 1):
+            cols = tile == t
+            m_t = s[..., :kv_tile * (t + 1)].amax(-1, keepdim=True)
+            later = s[..., kv_tile * (t + 1):].amax(-1, keepdim=True)
+            rises = (later >= m_t - 2 * err[..., :1]) & cols
+            dev = torch.where(rises, torch.maximum(dev, 2.0 ** -8 * p), dev)
+    o = P @ v
+    e_o = dev @ v.abs() + (GAMMA * Nk * U + rescale) * (P @ v.abs())
+    y = o / l
+    e_y = e_o / l + y.abs() * (rel_l + 2 * U) + U * y.abs()
+    return y, e_y
+
+
 def win_attn_bias(qkv, qkv_pad, bias, B, H, W, C, heads, ws, scale):
-    """es3_win_attn_bias_bf16, head dim 32: per window (padded positions take qkv_pad), s = scale q k^T + bias,
-    p = exp(s - rowmax) in fp32 (MUFU), P = bf16(p) into PV, l = sum of the fp32 p, y = (P v) / l, bf16 store.
-    `bias` is what the kernel reads: pass fp16(bias) for ws = 14 (its shared-memory table).
+    """es3_win_attn_bias_bf16, head dim 32: per window (padded positions take qkv_pad), softmax_attn with the per-head bias and
+    __expf, bf16 store.  `bias` is what the kernel reads: pass fp16(bias) for ws = 14 (its shared-memory table).
     Returns (ref, bound) of out [B H W, C]; padded queries are not outputs."""
     tok = win_tokens(B, H, W, ws).to(qkv.device)
     nwin, N = tok.shape
     rows = torch.cat([qkv, qkv_pad[None]], 0)[torch.where(tok >= 0, tok, torch.full_like(tok, qkv.shape[0]))]
     t = rows.reshape(nwin, N, heads, 3, 32).permute(3, 0, 2, 1, 4)              # [3, nwin, heads, N, 32]
-    q, k, v = t[0], t[1], t[2]
-    s = scale * q @ k.transpose(-1, -2) + bias
-    e_s = abs(scale) * GAMMA * 32 * U * (q.abs() @ k.abs().transpose(-1, -2)) + U * s.abs()
-    mx = s.amax(-1, keepdim=True)
-    arg = s - mx
-    p = torch.exp(arg)
-    delta = e_s + 2 * e_s.amax(-1, keepdim=True) + U * arg.abs() + 2 * U * (2 + 1.16 * arg.abs())   # relative error of each p
-    l = p.sum(-1, keepdim=True)
-    rel_l = (p * delta).sum(-1, keepdim=True) / l + GAMMA * N * U
-    P, dev = band(p, p * delta)
-    o = P @ v
-    e_o = dev @ v.abs() + GAMMA * N * U * (P @ v.abs())
-    y = o / l
-    e_y = e_o / l + y.abs() * (rel_l + 2 * U) + U * y.abs()
+    y, e_y = softmax_attn(t[0], t[1], t[2], scale, bias)
     y, e_y = y.permute(0, 2, 1, 3).reshape(nwin * N, C), e_y.permute(0, 2, 1, 3).reshape(nwin * N, C)
     keep = tok.reshape(-1) >= 0
     out = torch.empty(B * H * W, C, dtype=y.dtype, device=y.device)

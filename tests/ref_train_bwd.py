@@ -310,9 +310,9 @@ def litemla_bwd(ms, dy, kv_part, heads2, dim, eps):
 
 
 # ------------------------------------------------------------------------------------------------ TinyViT pieces
-def layernorm_bwd(x, dy, gamma, eps, dg0, db0, dres):
+def layernorm_bwd(x, dy, gamma, eps, dg0, db0, dres, bf16=True):
     """nn.LayerNorm backward over rows of x, dy [M, C]: dx = rstd (g - mean(g) - xh mean(g xh)) (+ dres), g = dy gamma;
-    dgamma += sum dy xh, dbeta += sum dy.  Returns dict name -> (ref, bound); dx is a bf16 store."""
+    dgamma += sum dy xh, dbeta += sum dy.  Returns dict name -> (ref, bound); dx is a bf16 store (bf16 = False: fp32)."""
     M, C = x.shape
     mu = x.mean(1, keepdim=True)
     e_mu = GAMMA * C * U * x.abs().mean(1, keepdim=True) + U * mu.abs()
@@ -344,7 +344,7 @@ def layernorm_bwd(x, dy, gamma, eps, dg0, db0, dres):
     e_dg = (dy.abs() * e_xh).sum(0) + GAMMA * (M + 1) * U * (dg0.abs() + (dy * xh).abs().sum(0))
     db = db0 + dy.sum(0)
     e_db = GAMMA * (M + 1) * U * (db0.abs() + dy.abs().sum(0))
-    return {"dx": (dx, _out(dx, e_dx, True)), "dgamma": (dg, _out(dg, e_dg, False)), "dbeta": (db, _out(db, e_db, False))}
+    return {"dx": (dx, _out(dx, e_dx, bf16)), "dgamma": (dg, _out(dg, e_dg, False)), "dbeta": (db, _out(db, e_db, False))}
 
 
 def win_attn_tokens(B, H, W, ws):
@@ -354,35 +354,63 @@ def win_attn_tokens(B, H, W, ws):
     return t.reshape(B * nH * nW, ws * ws)
 
 
-def win_attn_bias_bwd(qkv, dout, bias, B, H, W, C, heads, ws, scale):
-    """Backward of windowed attention with a per-head bias, head dim 32: s = scale q k^T + bias, P = softmax(s), o = P v.
-    dP = do v^T, D = rowsum(P dP), dS = P (dP - D); dq = scale dS k, dk = scale dS^T q, dv = P^T do.
-    Returns dict: "dqkv" (ref, bound) [B*H*W, 3C] bf16 store, "dS" (ref, bound) [nwin, heads, N, N] fp32."""
-    tok = win_attn_tokens(B, H, W, ws).to(qkv.device)
-    nwin, N = tok.shape
-    t = qkv[tok].reshape(nwin, N, heads, 3, 32).permute(3, 0, 2, 1, 4)        # [3, nwin, heads, N, 32]
-    q, k, v = t[0], t[1], t[2]
-    do = dout[tok].reshape(nwin, N, heads, 32).permute(0, 2, 1, 3)
-    s = scale * q @ k.transpose(-1, -2) + bias
-    e_s = abs(scale) * GAMMA * 32 * U * (q.abs() @ k.abs().transpose(-1, -2)) + U * s.abs()
+def softmax_attn_bwd(q, k, v, do, scale, bias=None, causal=False, o=None, exp_rel=None):
+    """Backward of softmax attention over q, k, v, do [..., N, d]: s = scale q k^T (+ bias) (+ -inf above the diagonal when causal),
+    P = softmax(s), o = P v.  dP = do v^T, D = rowsum(do o), dS = P (dP - D); dq = scale dS k, dk = scale dS^T q, dv = P^T do.
+    o: the forward output the kernel is given (D is then taken over it, as es3_text_attn_bwd's contract states); None: the exact
+    P v (D = rowsum(P dP)).  exp_rel(arg): the relative error of the kernel's exp (default __expf: (2 + 1.16 |arg|) ulp).
+    Returns dict name -> (ref, inner bound) for dq, dk, dv and dS."""
+    d = q.shape[-1]
+    N = k.shape[-2]
+    s = scale * q @ k.transpose(-1, -2)
+    if bias is not None:
+        s = s + bias
+    e_s = abs(scale) * GAMMA * d * U * (q.abs() @ k.abs().transpose(-1, -2)) + U * s.abs()
+    masked = None
+    if causal:
+        masked = torch.ones(s.shape[-2], N, dtype=torch.bool, device=s.device).triu(1)
+        s = s.masked_fill(masked, float("-inf"))
+        e_s = e_s.masked_fill(masked, 0.0)
     P = torch.softmax(s, -1)
     mx = s.amax(-1, keepdim=True)
     arg = s - mx
-    delta = e_s + 2 * e_s.amax(-1, keepdim=True) + U * arg.abs() + 2 * U * (2 + 1.16 * arg.abs())   # relative error of each exp
+    e_exp = 2 * U * (2 + 1.16 * arg.abs()) if exp_rel is None else exp_rel(arg)
+    delta = e_s + 2 * e_s.amax(-1, keepdim=True) + U * arg.abs() + e_exp        # relative error of each exp
+    if masked is not None:
+        delta = delta.masked_fill(masked, 0.0)
     rel_l = (P * delta).sum(-1, keepdim=True) + GAMMA * N * U
     e_P = P * (delta + rel_l + 2 * U)
     dP = do @ v.transpose(-1, -2)
-    e_dP = GAMMA * 32 * U * (do.abs() @ v.abs().transpose(-1, -2))
-    D = (P * dP).sum(-1, keepdim=True)
-    e_D = (e_P * dP.abs() + P * e_dP).sum(-1, keepdim=True) + GAMMA * N * U * (P * dP.abs()).sum(-1, keepdim=True) + U * D.abs()
+    e_dP = GAMMA * d * U * (do.abs() @ v.abs().transpose(-1, -2))
+    if o is None:
+        D = (P * dP).sum(-1, keepdim=True)
+        e_D = (e_P * dP.abs() + P * e_dP).sum(-1, keepdim=True) + GAMMA * N * U * (P * dP.abs()).sum(-1, keepdim=True) + U * D.abs()
+    else:
+        D = (do * o).sum(-1, keepdim=True)
+        e_D = GAMMA * d * U * (do * o).abs().sum(-1, keepdim=True) + U * D.abs()
     dS = P * (dP - D)
     e_dS = e_P * (dP - D).abs() + P * (e_dP + e_D + U * (dP - D).abs()) + U * dS.abs()
+    if masked is not None:
+        dS = dS.masked_fill(masked, 0.0)
+        e_dS = e_dS.masked_fill(masked, 0.0)
     dq = scale * dS @ k
     e_dq = abs(scale) * (e_dS @ k.abs() + GAMMA * N * U * (dS.abs() @ k.abs())) + U * dq.abs()
     dk = scale * dS.transpose(-1, -2) @ q
     e_dk = abs(scale) * (e_dS.transpose(-1, -2) @ q.abs() + GAMMA * N * U * (dS.abs().transpose(-1, -2) @ q.abs())) + U * dk.abs()
     dv = P.transpose(-1, -2) @ do
     e_dv = e_P.transpose(-1, -2) @ do.abs() + GAMMA * N * U * (P.transpose(-1, -2) @ do.abs())
+    return {"dq": (dq, e_dq), "dk": (dk, e_dk), "dv": (dv, e_dv), "dS": (dS, e_dS)}
+
+
+def win_attn_bias_bwd(qkv, dout, bias, B, H, W, C, heads, ws, scale):
+    """Backward of windowed attention with a per-head bias, head dim 32 (softmax_attn_bwd per window, D = rowsum(P dP)).
+    Returns dict: "dqkv" (ref, bound) [B*H*W, 3C] bf16 store, "dS" (ref, bound) [nwin, heads, N, N] fp32."""
+    tok = win_attn_tokens(B, H, W, ws).to(qkv.device)
+    nwin, N = tok.shape
+    t = qkv[tok].reshape(nwin, N, heads, 3, 32).permute(3, 0, 2, 1, 4)        # [3, nwin, heads, N, 32]
+    do = dout[tok].reshape(nwin, N, heads, 32).permute(0, 2, 1, 3)
+    r = softmax_attn_bwd(t[0], t[1], t[2], do, scale, bias)
+    (dq, e_dq), (dk, e_dk), (dv, e_dv), (dS, e_dS) = r["dq"], r["dk"], r["dv"], r["dS"]
 
     def scatter(a, b, c):
         g = torch.stack([a, b, c], 3).permute(0, 2, 1, 3, 4).reshape(nwin * N, heads * 96)   # [nwin, N, heads, 3, 32]

@@ -1,5 +1,6 @@
 """GPU: the native text encoders (MobileCLIP students, SAM3 text teacher) end to end from strings against the reference
-fixtures and the CPU oracle, the three new kernels against torch fp32, batch invariance, the text dump, the raise paths."""
+fixtures and the CPU oracle, batch invariance, the text dump, the raise paths (the kernels element by element:
+tests/test_text_kernels_gpu.py)."""
 import numpy as np
 import pytest
 import torch
@@ -101,58 +102,6 @@ def test_caption_alone_equals_caption_in_batch_of_64(cuda):
     assert torch.equal(alone[:, 0], many[:, 1])
     t = small_teacher(cuda)
     assert torch.equal(t([caps[3]], device=cuda)[:, 0], t(batch, device=cuda)[:, 3])
-
-
-# ------------------------------------------------------------------------------------------------ kernels vs torch fp32
-@pytest.mark.parametrize("L", [1, 16, 32, 77, 128])
-@pytest.mark.parametrize("heads", [8, 12, 16])
-def test_causal_attention_kernel(cuda, L, heads):
-    from efficientsam3_b200 import ops
-    B, C = 3, heads * 64
-    g = torch.Generator(device="cpu").manual_seed(L * 100 + heads)
-    qkv = (torch.randn(B * L, 3 * C, generator=g) * 1.5).to(torch.bfloat16).to(cuda)
-    out = ops.attention_causal(qkv, B, L, C, heads, 64 ** -0.5)
-    q, k, v = qkv.float().view(B, L, 3, heads, 64).permute(2, 0, 3, 1, 4)
-    s = (q @ k.transpose(-1, -2)) * 64 ** -0.5 + torch.full((L, L), float("-inf"), device=cuda).triu(1)
-    ref = (torch.softmax(s, -1) @ v).transpose(1, 2).reshape(B * L, C)
-    assert rel_l2(out.float().cpu(), ref.cpu()) < 1e-2
-    # token 0 of each sequence attends to itself only: its output is its value row
-    np.testing.assert_allclose(out.float().view(B, L, C)[:, 0].cpu().numpy(), v.transpose(1, 2).reshape(B, L, C)[:, 0]
-                               .to(torch.bfloat16).float().cpu().numpy(), rtol=1e-2, atol=1e-2)
-
-
-@pytest.mark.parametrize("L", [1, 5, 11, 32, 77])
-def test_repmixer_kernel(cuda, L):
-    import torch.nn.functional as F
-    from efficientsam3_b200 import ops
-    B, C = 4, 512
-    g = torch.Generator(device="cpu").manual_seed(L)
-    x = torch.randn(B * L, C, generator=g)
-    wm, wf = torch.randn(11, C, generator=g) * 0.3, torch.randn(11, C, generator=g) * 0.3
-    bm, bf = torch.randn(C, generator=g), torch.randn(C, generator=g)
-    x1, u = ops.repmixer(x.to(cuda), B, L, *(t.to(cuda) for t in (wm, bm, wf, bf)))
-
-    def dw(t, w, b):   # depthwise 1x11, zero padding, fp64
-        t = t.double().view(B, L, C).permute(0, 2, 1)
-        return (F.conv1d(t, w.double().t().unsqueeze(1), b.double(), padding=5, groups=C)).permute(0, 2, 1).reshape(B * L, C)
-    r1 = dw(x, wm, bm)
-    r2 = dw(r1, wf, bf)
-    np.testing.assert_allclose(x1.cpu().double().numpy(), r1.numpy(), rtol=1e-5, atol=1e-5)
-    assert rel_l2(u.float().cpu(), r2) < 5e-3
-    with pytest.raises(ValueError, match="1..128"):
-        ops.repmixer(torch.zeros(129, C, device=cuda), 1, 129, *(t.to(cuda) for t in (wm, bm, wf, bf)))
-
-
-def test_text_embed_is_an_exact_gather(cuda):
-    from efficientsam3_b200 import ops
-    g = torch.Generator(device="cpu").manual_seed(3)
-    table, pos = torch.randn(1000, 512, generator=g), torch.randn(20, 512, generator=g)
-    ids = torch.randint(0, 1000, (5, 20), generator=g)
-    x, e = ops.text_embed(ids.to(cuda), table.to(cuda), pos.to(cuda), emb="plain")
-    assert torch.equal(e.cpu(), table[ids].reshape(100, 512))
-    assert torch.equal(x.cpu(), (table[ids] + pos).reshape(100, 512))
-    x2, e2 = ops.text_embed(ids.to(cuda), table.to(cuda), None, emb="pos")
-    assert torch.equal(x2.cpu(), table[ids].reshape(100, 512)) and e2 is x2
 
 
 # ------------------------------------------------------------------------------------------------ dump and raise paths

@@ -1,4 +1,4 @@
-"""GPU: training the MobileCLIP base text students natively -- the text backward kernels against torch fp32 autograd, whole
+"""GPU: training the MobileCLIP base text students natively -- the text KD loss's composition against torch fp32 autograd, whole
 training graphs against the oracle's fp32 autograd (with the bf16-autocast oracle as the precision yardstick), the train-mode
 forward against the eval fixtures, the optimiser interplay (arena, exclusion, accumulation, determinism) and the raise paths."""
 import random
@@ -17,90 +17,7 @@ from test_text_train_cpu import ref_text_loss
 pytestmark = pytest.mark.gpu
 
 
-def _bf(t):
-    return t.to(torch.bfloat16)
-
-
 # ------------------------------------------------------------------------------------------------ kernels vs torch fp32
-def _attn_ref(qkv, dout, B, L, C, heads, causal):
-    x = qkv.float().reshape(B, L, 3, heads, C // heads).permute(2, 0, 3, 1, 4).clone().requires_grad_(True)
-    q, k, v = x[0], x[1], x[2]
-    s = (q * (C // heads) ** -0.5) @ k.transpose(-1, -2)
-    if causal:
-        s = s + OT.causal_mask(L, qkv.device)
-    o = torch.softmax(s, -1) @ v
-    o.backward(dout.float().reshape(B, L, heads, -1).transpose(1, 2))
-    return x.grad.permute(1, 3, 0, 2, 4).reshape(B * L, 3 * C)
-
-
-@pytest.mark.parametrize("causal", [False, True])
-@pytest.mark.parametrize("heads", [8, 12])
-@pytest.mark.parametrize("L", [1, 16, 32, 77, 128])
-def test_attention_bwd_kernel(cuda, L, heads, causal):
-    from efficientsam3_b200 import ops
-    g = torch.Generator().manual_seed(L * 100 + heads + causal)
-    B, C = 3, 64 * heads
-    qkv = _bf(torch.randn(B * L, 3 * C, generator=g)).to(cuda)
-    dout = _bf(torch.randn(B * L, C, generator=g)).to(cuda)
-    scale = 64 ** -0.5
-    o = ops.attention_causal(qkv, B, L, C, heads, scale) if causal else ops.attention(qkv, B, 1, L, C, heads, 0, scale)
-    got = ops.text_attn_bwd(qkv, o, dout, B, L, C, heads, scale, causal)
-    ref = _attn_ref(qkv, dout, B, L, C, heads, causal)
-    for part in range(3):                      # dq | dk | dv, each against its own scale
-        sl = slice(part * C, (part + 1) * C)
-        # at L = 1 the softmax is constant, so dq and dk are exactly 0 in exact arithmetic: measure them on dqkv's scale
-        scale_ref = ref[:, sl].abs().max().item() or ref.abs().max().item()
-        err = (got[:, sl].float() - ref[:, sl]).abs().max().item() / scale_ref
-        assert err <= 1e-2, (part, err)
-    assert torch.equal(got, ops.text_attn_bwd(qkv, o, dout, B, L, C, heads, scale, causal))     # deterministic
-
-
-def test_layernorm_bwd_f32_kernel(cuda):
-    from efficientsam3_b200 import ops
-    g = torch.Generator().manual_seed(3)
-    for M, C in ((2048, 512), (1100, 768), (5, 256)):
-        x = (torch.randn(M, C, generator=g) * 3 + 0.5).to(cuda)
-        dy, dres = torch.randn(M, C, generator=g).to(cuda), torch.randn(M, C, generator=g).to(cuda)
-        w, b = (torch.randn(C, generator=g) + 1).to(cuda), torch.randn(C, generator=g).to(cuda)
-        dg, db = torch.full((C,), 0.25, device=cuda), torch.zeros(C, device=cuda)
-        dx, dxb = ops.layernorm_bwd_f32(x, dy, w, 1e-5, dg, db, dres=dres, want_bf16=True)
-        xr, wr, br = x.clone().requires_grad_(True), w.clone().requires_grad_(True), b.clone().requires_grad_(True)
-        F.layer_norm(xr, (C,), wr, br, 1e-5).backward(dy)
-        assert max_err_over_scale(dx.cpu(), (xr.grad + dres).cpu()) <= 2e-3
-        assert torch.equal(dxb, dx.to(torch.bfloat16))
-        assert max_err_over_scale((dg - 0.25).cpu(), wr.grad.cpu()) <= 2e-3
-        assert max_err_over_scale(db.cpu(), br.grad.cpu()) <= 2e-3
-
-
-def test_embedding_and_positional_grads(cuda):
-    from efficientsam3_b200 import ops
-    g = torch.Generator().manual_seed(5)
-    V, C, B, L = 300, 512, 8, 32
-    ids = torch.randint(0, 40, (B, L), generator=g)
-    ids[:, -20:] = 0                                            # padding: row 0 collects > 160 tokens, i.e. several chunks
-    dx = torch.randn(B * L, C, generator=g).to(cuda)
-    grad = torch.zeros(V, C, device=cuda)
-    plan = ops.embed_grad_plan(ids, cuda)
-    assert plan["nchunk"] > plan["uid"].numel()                 # the padding id is split over several chunks
-    ops.text_embed_grad(dx, plan, grad)
-    table = torch.zeros(V, C, device=cuda, requires_grad=True)
-    F.embedding(ids.to(cuda), table).backward(dx.view(B, L, C))
-    assert max_err_over_scale(grad.cpu(), table.grad.cpu()) <= 2e-3
-    unused = torch.ones(V, dtype=torch.bool)
-    unused[ids.unique()] = False
-    assert torch.count_nonzero(grad[unused.to(cuda)]).item() == 0   # ids that do not occur: exactly zero
-    for N in (32, 77, 16):                                      # N == L, the 77-entry table at 32 tokens, a shorter table
-        pe = torch.randn(1, 1, N, C, generator=g).to(cuda).requires_grad_(True)
-        tab = F.interpolate(pe, size=(L, C), mode="bilinear") if N != L else pe
-        tab.reshape(L, C).unsqueeze(0).expand(B, L, C).backward(dx.view(B, L, C))
-        gp = torch.zeros(1, 1, N, C, device=cuda)
-        ops.text_pos_grad(dx, B, L, gp)
-        assert max_err_over_scale(gp.cpu(), pe.grad.cpu()) <= 2e-3, N
-        if N != L:
-            fwd = ops.text_pos_resize(pe.detach().reshape(N, C).contiguous(), L)
-            assert max_err_over_scale(fwd.cpu(), tab.detach().reshape(L, C).cpu()) <= 1e-6
-
-
 @pytest.mark.parametrize("masked", [False, True])
 def test_text_kd_loss_kernels(cuda, masked):
     from efficientsam3_b200.stage1.losses import TextKDLossFunction, text_kd_loss

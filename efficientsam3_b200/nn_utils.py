@@ -148,12 +148,13 @@ class NativePlanMixin:
 
 class StagedGraphMixin:
     """CUDA-graph replay of an eval forward whose inputs arrive from the host (the text encoders: token ids validated on the
-    host, EOT row indices).  One graph per key (shapes, input kind, device): its inputs are static device buffers, refilled
-    before each replay -- host int64 tensors through a pinned staging buffer (one asynchronous copy), CUDA tensors device to
-    device -- and its outputs are the graph's own buffers, overwritten by the next replay with the same key.
+    host, EOT row indices; the point-prompt predictor: prompt coordinates and labels scaled on the host).  One graph per key
+    (shapes, input kind, device): its inputs are static device buffers, refilled before each replay -- host tensors of any
+    dtype through one pinned staging buffer (one asynchronous copy), CUDA tensors device to device -- and its outputs are the
+    graph's own buffers, overwritten by the next replay with the same key.
 
-    A graph reads the packed weights of every NativePlanMixin below the module by address, so it is captured again when
-    a parameter or buffer moves (params_fingerprint: optimiser steps through torch, load_state_dict, a replaced Parameter, a move
+    A graph reads the packed weights of every NativePlanMixin below the modules it runs (the module itself unless `_graphed`
+    names others) by address, so it is captured again when a parameter or buffer of those modules moves (params_fingerprint: optimiser steps through torch, load_state_dict, a replaced Parameter, a move
     to another device) or a plan was invalidated (FlatAdamW's step and the batch-statistics BatchNorm reset `_plan_key`).  The
     entry keeps the plans it was captured with alive, so a stale graph never reads freed memory.  At most `max_graphs` graphs are
     kept; the oldest capture is evicted first."""
@@ -169,17 +170,19 @@ class StagedGraphMixin:
         self._graph_max = max_graphs
         return self
 
-    def _graphed(self, key, host, dev_in, fn):
-        """fn(*static inputs) -> outputs, replayed from the graph of `key` (its last element is the device).  host: CPU int64
-        tensors, dev_in: CUDA tensors; fn receives device buffers of the same shapes, host ones first."""
+    def _graphed(self, key, host, dev_in, fn, modules=None):
+        """fn(*static inputs) -> outputs, replayed from the graph of `key` (its last element is the device).  host: CPU tensors,
+        dev_in: CUDA tensors; fn receives device buffers of the same shapes and dtypes, host ones first.  modules: the modules
+        whose parameters and plans the graph reads (default: this module)."""
         dev = key[-1]
-        fp = params_fingerprint(self)
+        modules = (self,) if modules is None else tuple(modules)
+        fp = tuple(params_fingerprint(m) for m in modules)
         ent = self._graphs.get(key)
         with torch.cuda.device(dev):
             if ent is None or ent["fp"] != fp or any(getattr(m, "_plan_key", None) is not k for m, k, _ in ent["plans"]):
                 del ent                             # release the stale graph's memory before capturing its successor
                 self._graphs.pop(key, None)
-                ent = self._capture(dev, host, dev_in, fn, fp)
+                ent = self._capture(dev, host, dev_in, fn, fp, modules)
                 while len(self._graphs) >= self._graph_max:
                     self._graphs.pop(next(iter(self._graphs)))
                 self._graphs[key] = ent
@@ -190,28 +193,33 @@ class StagedGraphMixin:
         return ent["out"]
 
     @staticmethod
+    def _host_offsets(host):
+        """Byte offset of each host tensor in the staging buffer (16-byte aligned, so every dtype can be viewed in place)."""
+        offs, o = [], 0
+        for h in host:
+            offs.append(o)
+            o += (h.numel() * h.element_size() + 15) // 16 * 16
+        return offs, o
+
+    @staticmethod
     def _stage(ent, host, dev_in):
         if host:
             ent["copied"].synchronize()             # the previous replay's copy out of the pinned buffer has been read
-            o = 0
-            for h in host:
-                ent["pinned"][o:o + h.numel()].copy_(h.reshape(-1))
-                o += h.numel()
+            for h, o in zip(host, ent["offs"]):
+                b = h.reshape(-1).view(torch.uint8)
+                ent["pinned"][o:o + b.numel()].copy_(b)
             ent["flat"].copy_(ent["pinned"], non_blocking=True)
             ent["copied"].record()
         for s, t in zip(ent["dev_in"], dev_in):
             s.copy_(t)
 
-    def _capture(self, dev, host, dev_in, fn, fp):
+    def _capture(self, dev, host, dev_in, fn, fp, modules):
         from . import ops
-        n = sum(h.numel() for h in host)
-        ent = dict(fp=fp, pinned=torch.empty(n, dtype=torch.int64, pin_memory=True),
-                   flat=torch.empty(n, dtype=torch.int64, device=dev), copied=torch.cuda.Event(),
+        offs, n = self._host_offsets(host)
+        ent = dict(fp=fp, offs=offs, pinned=torch.empty(n, dtype=torch.uint8, pin_memory=True),
+                   flat=torch.empty(n, dtype=torch.uint8, device=dev), copied=torch.cuda.Event(),
                    dev_in=[torch.empty(t.shape, dtype=t.dtype, device=t.device) for t in dev_in])
-        static, o = [], 0
-        for h in host:
-            static.append(ent["flat"][o:o + h.numel()].view(h.shape))
-            o += h.numel()
+        static = [ent["flat"][o:o + h.numel() * h.element_size()].view(h.dtype).view(h.shape) for h, o in zip(host, offs)]
         static += ent["dev_in"]
         self._stage(ent, host, dev_in)
         fn(*static)                                 # un-captured pass: packs weights, builds positional tables, configures kernels
@@ -222,6 +230,6 @@ class StagedGraphMixin:
         with torch.cuda.graph(graph, capture_error_mode="thread_local"):
             out = fn(*static)
         ent.update(graph=graph, out=out, launches=ops.launch_count - n0,
-                   plans=[(m, getattr(m, "_plan_key", None), getattr(m, "_plan_cache", None)) for m in self.modules()
-                          if isinstance(m, NativePlanMixin)])
+                   plans=[(m, getattr(m, "_plan_key", None), getattr(m, "_plan_cache", None)) for top in modules
+                          for m in top.modules() if isinstance(m, NativePlanMixin)])
         return ent

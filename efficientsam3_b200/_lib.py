@@ -56,7 +56,7 @@ SIGNATURES: dict[str, list] = {
     "es3_mask_downscale_tokens": [_vp] * 12 + [_ll, _vp, _vp, _i, _i, _i, _i, _f, _vp],
     "es3_fill_small_components": [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _vp],
     "es3_add_rows": [_vp, _vp, _ll, _i, _i, _vp, _vp, _vp],
-    "es3_nchw_f32_to_tokens": [_vp, _vp, _vp, _vp, _i, _i, _i, _vp],
+    "es3_nchw_f32_to_tokens": [_vp, _vp, _vp, _i, _i, _i, _vp],
     "es3_attn_few_queries": [_vp, _ll, _vp, _vp, _ll, _i, _vp, _ll, _i, _i, _i, _i, _i, _f, _vp],
     "es3_attn_few_keys": [_vp, _ll, _vp, _vp, _ll, _vp, _ll, _i, _i, _i, _i, _i, _f, _vp],
     "es3_ln_rows_gelu": [_vp, _vp, _vp, _f, _vp, _ll, _i, _vp],

@@ -140,4 +140,19 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// Image -> token attention (es3_attn_few_keys and its fp32 twin) stages its keys and values in shared memory FEW_KEYS_TILE tokens
+// at a time: s [2][cap][D] gets rows row0 .. row0 + nt - 1 of k and v [., ldkv] (K at s, V at s + cap D).  Every thread of the
+// block calls it; the barriers keep the previous tile alive until every thread has read it.
+constexpr int FEW_KEYS_TILE = 16;
+__device__ __forceinline__ void few_keys_load_tile(float* s, const float* __restrict__ k, const float* __restrict__ v, long long ldkv,
+                                                   long long row0, int nt, int cap, int D) {
+  __syncthreads();
+  for (int i = threadIdx.x; i < nt * D; i += blockDim.x) {
+    const int t = i / D, c = i % D;
+    s[i] = k[(row0 + t) * ldkv + c];
+    s[cap * D + i] = v[(row0 + t) * ldkv + c];
+  }
+  __syncthreads();
+}
+
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }

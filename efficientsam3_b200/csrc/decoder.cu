@@ -79,9 +79,9 @@ __global__ void add_rows_kernel(const float* __restrict__ x, const float* __rest
   }
 }
 
-// [B,C,HW] fp32 -> [B,HW,C] fp32 (+ optional per-channel vector add, e.g. no_mask_embed), also bf16 copy.
-__global__ void nchw_to_tokens_kernel(const float* __restrict__ in, const float* __restrict__ addc, float* __restrict__ out_f32,
-                                      bf16* __restrict__ out_bf16, int HW, int C) {
+// [B,C,HW] fp32 -> [B,HW,C] fp32 and / or its bf16 copy.
+__global__ void nchw_to_tokens_kernel(const float* __restrict__ in, float* __restrict__ out_f32, bf16* __restrict__ out_bf16, int HW,
+                                      int C) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
@@ -94,7 +94,7 @@ __global__ void nchw_to_tokens_kernel(const float* __restrict__ in, const float*
   for (int i = ty; i < 32; i += 8) {
     const int p = p0 + i, c = c0 + tx;
     if (p < HW && c < C) {
-      const float v = tile[tx][i] + (addc ? addc[c] : 0.f);
+      const float v = tile[tx][i];
       if (out_f32) out_f32[((long long)b * HW + p) * C + c] = v;
       if (out_bf16) out_bf16[((long long)b * HW + p) * C + c] = __float2bfloat16(v);
     }
@@ -152,49 +152,53 @@ __global__ void attn_few_queries_kernel(const float* __restrict__ q, long long l
   }
 }
 
-// Many queries (image tokens), few keys (<= 16 tokens): one thread per (query, head).
-// q [B,Nq,ldq] bf16, k/v [B,Tk,ldkv] fp32, out [B,Nq,ldo] bf16.  cross_attn_image_to_token core.
+// Many queries (image tokens), few keys (the decoder's output and prompt tokens, any number): one thread per (query, head).
+// q [B,Nq,ldq] bf16, k/v [B,Tk,ldkv] fp32, out [B,Nq,ldo] bf16.  cross_attn_image_to_token core.  K/V stream through shared
+// memory in tiles of FEW_KEYS_TILE tokens; the softmax is sequential per thread, so the tiling does not change the arithmetic.
 template <int HD>
 __global__ void attn_few_keys_kernel(const bf16* __restrict__ q, long long ldq, const float* __restrict__ k,
                                      const float* __restrict__ v, long long ldkv, bf16* __restrict__ out, long long ldo,
                                      int Nq, int Tk, int H, float scale) {
-  extern __shared__ float skv[];  // [2][Tk][H*HD]
+  extern __shared__ float skv[];  // [2][cap][H*HD], cap = min(Tk, FEW_KEYS_TILE)
   const int b = blockIdx.y;
-  const int D = H * HD;
-  for (int i = threadIdx.x; i < Tk * D; i += blockDim.x) {
-    const int t = i / D, c = i % D;
-    skv[i] = k[((long long)b * Tk + t) * ldkv + c];
-    skv[Tk * D + i] = v[((long long)b * Tk + t) * ldkv + c];
-  }
-  __syncthreads();
+  const int D = H * HD, cap = min(Tk, FEW_KEYS_TILE);
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= Nq * H) return;
+  const bool active = idx < Nq * H;   // inactive threads still take part in the tile loads and barriers
   const int h = idx % H, n = idx / H;
   float qr[HD];
   const bf16* qp = q + ((long long)b * Nq + n) * ldq + h * HD;
+  if (active) {
 #pragma unroll
-  for (int d = 0; d < HD; d += 8) {
-    float f[8];
-    unpack8(*reinterpret_cast<const uint4*>(qp + d), f);
+    for (int d = 0; d < HD; d += 8) {
+      float f[8];
+      unpack8(*reinterpret_cast<const uint4*>(qp + d), f);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) qr[d + e] = f[e] * scale;
+      for (int e = 0; e < 8; ++e) qr[d + e] = f[e] * scale;
+    }
   }
   float mx = -INFINITY, l = 0.f, o[HD];
 #pragma unroll
   for (int d = 0; d < HD; ++d) o[d] = 0.f;
-  for (int t = 0; t < Tk; ++t) {   // online softmax over the few keys
-    const float* kp = skv + t * D + h * HD;
-    float a = 0.f;
+  for (int t0 = 0; t0 < Tk; t0 += FEW_KEYS_TILE) {
+    const int nt = min(FEW_KEYS_TILE, Tk - t0);
+    few_keys_load_tile(skv, k, v, ldkv, (long long)b * Tk + t0, nt, cap, D);
+    if (active) {
+      for (int t = 0; t < nt; ++t) {   // online softmax over the few keys
+        const float* kp = skv + t * D + h * HD;
+        float a = 0.f;
 #pragma unroll
-    for (int d = 0; d < HD; ++d) a = fmaf(qr[d], kp[d], a);
-    const float mn = fmaxf(mx, a);
-    const float corr = __expf(mx - mn), p = __expf(a - mn);
-    l = l * corr + p;
-    const float* vp = skv + Tk * D + t * D + h * HD;
+        for (int d = 0; d < HD; ++d) a = fmaf(qr[d], kp[d], a);
+        const float mn = fmaxf(mx, a);
+        const float corr = __expf(mx - mn), p = __expf(a - mn);
+        l = l * corr + p;
+        const float* vp = skv + cap * D + t * D + h * HD;
 #pragma unroll
-    for (int d = 0; d < HD; ++d) o[d] = fmaf(p, vp[d], o[d] * corr);
-    mx = mn;
+        for (int d = 0; d < HD; ++d) o[d] = fmaf(p, vp[d], o[d] * corr);
+        mx = mn;
+      }
+    }
   }
+  if (!active) return;
   const float inv = 1.f / l;
   bf16* op = out + ((long long)b * Nq + n) * ldo + h * HD;
 #pragma unroll
@@ -450,10 +454,9 @@ extern "C" int es3_add_rows(const float* x, const float* add, long long M, int C
   return 0;
 }
 
-extern "C" int es3_nchw_f32_to_tokens(const float* in, const float* addc, float* out_f32, void* out_bf16, int B, int HW,
-                                      int C, void* stream) {
+extern "C" int es3_nchw_f32_to_tokens(const float* in, float* out_f32, void* out_bf16, int B, int HW, int C, void* stream) {
   dim3 grid(ceil_div(HW, 32), ceil_div(C, 32), B);
-  nchw_to_tokens_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(in, addc, out_f32, (bf16*)out_bf16, HW, C);
+  nchw_to_tokens_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(in, out_f32, (bf16*)out_bf16, HW, C);
   ES3_LAUNCH_CHECK("nchw_to_tokens_kernel");
   return 0;
 }
@@ -461,15 +464,16 @@ extern "C" int es3_nchw_f32_to_tokens(const float* in, const float* addc, float*
 extern "C" int es3_attn_few_queries(const float* q, long long ldq, const void* k, const void* v, long long ldkv, int kv_f32,
                                     float* out, long long ldo, int B, int H, int head_dim, int Tq, int Tk, float scale,
                                     void* stream) {
-  ES3_REQUIRE(head_dim == 16 || head_dim == 32, "es3_attn_few_queries: head_dim %d not in {16,32}", head_dim);
+  // head_dim 32 is self-attention over the tokens, whose K/V are fp32; token-to-image attention (bf16 or fp32 K/V) has head_dim 16
+  ES3_REQUIRE(head_dim == 16 || (head_dim == 32 && kv_f32), "es3_attn_few_queries: head_dim %d with %s K/V not supported", head_dim,
+              kv_f32 ? "fp32" : "bf16");
   dim3 grid(ceil_div(Tq, 4), H, B);
   cudaStream_t st = (cudaStream_t)stream;
   if (head_dim == 16) {
     if (kv_f32) attn_few_queries_kernel<16, float><<<grid, 128, 0, st>>>(q, ldq, (const float*)k, (const float*)v, ldkv, out, ldo, Tq, Tk, scale);
     else attn_few_queries_kernel<16, bf16><<<grid, 128, 0, st>>>(q, ldq, (const bf16*)k, (const bf16*)v, ldkv, out, ldo, Tq, Tk, scale);
   } else {
-    if (kv_f32) attn_few_queries_kernel<32, float><<<grid, 128, 0, st>>>(q, ldq, (const float*)k, (const float*)v, ldkv, out, ldo, Tq, Tk, scale);
-    else attn_few_queries_kernel<32, bf16><<<grid, 128, 0, st>>>(q, ldq, (const bf16*)k, (const bf16*)v, ldkv, out, ldo, Tq, Tk, scale);
+    attn_few_queries_kernel<32, float><<<grid, 128, 0, st>>>(q, ldq, (const float*)k, (const float*)v, ldkv, out, ldo, Tq, Tk, scale);
   }
   ES3_LAUNCH_CHECK("attn_few_queries_kernel");
   return 0;
@@ -477,8 +481,8 @@ extern "C" int es3_attn_few_queries(const float* q, long long ldq, const void* k
 
 extern "C" int es3_attn_few_keys(const void* q, long long ldq, const float* k, const float* v, long long ldkv, void* out,
                                  long long ldo, int B, int H, int head_dim, int Nq, int Tk, float scale, void* stream) {
-  ES3_REQUIRE(head_dim == 16 && Tk <= 16, "es3_attn_few_keys: head_dim must be 16 and Tk <= 16 (got %d, %d)", head_dim, Tk);
-  const size_t smem = (size_t)2 * Tk * H * head_dim * sizeof(float);
+  ES3_REQUIRE(head_dim == 16 && Tk > 0, "es3_attn_few_keys: head_dim must be 16 and Tk > 0 (got %d, %d)", head_dim, Tk);
+  const size_t smem = (size_t)2 * std::min(Tk, FEW_KEYS_TILE) * H * head_dim * sizeof(float);
   dim3 grid(ceil_div((long long)Nq * H, 256), B);
   attn_few_keys_kernel<16><<<grid, 256, smem, (cudaStream_t)stream>>>((const bf16*)q, ldq, k, v, ldkv, (bf16*)out, ldo, Nq, Tk, H, scale);
   ES3_LAUNCH_CHECK("attn_few_keys_kernel");

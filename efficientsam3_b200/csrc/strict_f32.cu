@@ -227,46 +227,50 @@ __global__ void bilinear_nhwc_f32_to_nchw_kernel(const float* __restrict__ x, fl
 
 
 // image -> token attention with few keys (TwoWayAttentionBlock.cross_attn_image_to_token, sam/transformer.py:168-176), fp32 in / out,
-// libm expf (the bf16-mode kernel in decoder.cu uses ex2.approx).  Thread = (query row, head); keys / values of the image in smem.
+// libm expf (the bf16-mode kernel in decoder.cu uses ex2.approx).  Thread = (query row, head).  Keys / values stream through smem
+// in tiles of FEW_KEYS_TILE tokens, once per pass of the two-pass softmax (max, then the sum of the exponentials) and once more for
+// P V; each pass recomputes the scores with the same fmaf chain, so every pass sees the same fp32 score.
 template <int HD>
 __global__ void attn_few_keys_f32_kernel(const float* __restrict__ q, long long ldq, const float* __restrict__ k,
                                          const float* __restrict__ v, long long ldkv, float* __restrict__ out, long long ldo, int Nq,
                                          int Tk, int H, float scale) {
-  extern __shared__ float skv[];  // [2][Tk][H*HD]
+  extern __shared__ float skv[];  // [2][cap][H*HD], cap = min(Tk, FEW_KEYS_TILE)
   const int b = blockIdx.y;
-  const int D = H * HD;
-  for (int i = threadIdx.x; i < Tk * D; i += blockDim.x) {
-    const int t = i / D, c = i % D;
-    skv[i] = k[((long long)b * Tk + t) * ldkv + c];
-    skv[Tk * D + i] = v[((long long)b * Tk + t) * ldkv + c];
-  }
-  __syncthreads();
+  const int D = H * HD, cap = min(Tk, FEW_KEYS_TILE), ntile = (Tk + FEW_KEYS_TILE - 1) / FEW_KEYS_TILE;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= Nq * H) return;
+  const bool active = idx < Nq * H;   // inactive threads still take part in the tile loads and barriers
   const int h = idx % H, n = idx / H;
   const float* qp = q + ((long long)b * Nq + n) * ldq + h * HD;
-  float qr[HD], s[16];
+  float qr[HD], o[HD];
 #pragma unroll
-  for (int d = 0; d < HD; ++d) qr[d] = qp[d];
-  float mx = -INFINITY;
-  for (int t = 0; t < Tk; ++t) {
-    const float* kp = skv + t * D + h * HD;
-    float a = 0.f;
+  for (int d = 0; d < HD; ++d) { qr[d] = active ? qp[d] : 0.f; o[d] = 0.f; }
+  float mx = -INFINITY, l = 0.f, inv = 0.f;
+  for (int pass = 0; pass < 3; ++pass) {   // 0: row max; 1: l = sum of exp; 2: o = sum of (exp / l) v
+    if (pass == 2) inv = 1.f / l;
+    for (int tile = 0; tile < ntile; ++tile) {
+      const int t0 = tile * FEW_KEYS_TILE, nt = min(FEW_KEYS_TILE, Tk - t0);
+      if (pass == 0 || ntile > 1) few_keys_load_tile(skv, k, v, ldkv, (long long)b * Tk + t0, nt, cap, D);
+      if (!active) continue;
+      for (int t = 0; t < nt; ++t) {
+        const float* kp = skv + t * D + h * HD;
+        float a = 0.f;
 #pragma unroll
-    for (int d = 0; d < HD; ++d) a = fmaf(qr[d], kp[d], a);
-    s[t] = a * scale;
-    mx = fmaxf(mx, s[t]);
+        for (int d = 0; d < HD; ++d) a = fmaf(qr[d], kp[d], a);
+        const float s = __fmul_rn(a, scale);   // rounded before the max and the subtraction: no contraction into an fma
+        if (pass == 0) { mx = fmaxf(mx, s); continue; }
+        const float p = expf(s - mx);
+        if (pass == 1) { l += p; continue; }
+        const float w = p * inv;
+        const float* vp = skv + cap * D + t * D + h * HD;
+#pragma unroll
+        for (int d = 0; d < HD; ++d) o[d] = fmaf(w, vp[d], o[d]);
+      }
+    }
   }
-  float l = 0.f;
-  for (int t = 0; t < Tk; ++t) { s[t] = expf(s[t] - mx); l += s[t]; }
-  const float inv = 1.f / l;
+  if (!active) return;
   float* op = out + ((long long)b * Nq + n) * ldo + h * HD;
 #pragma unroll
-  for (int d = 0; d < HD; ++d) {
-    float o = 0.f;
-    for (int t = 0; t < Tk; ++t) o = fmaf(s[t] * inv, skv[Tk * D + t * D + h * HD + d], o);
-    op[d] = o;
-  }
+  for (int d = 0; d < HD; ++d) op[d] = o[d];
 }
 
 // y = gelu_erf(LayerNorm(x) * w + b) over rows of C <= 128 channels, fp32 out (MaskDecoder.output_upscaling, mask_decoder.py:59-70).
@@ -515,8 +519,8 @@ extern "C" int es3_bilinear_nhwc_f32_to_nchw(const float* x, float* y, int B, in
 
 extern "C" int es3_attn_few_keys_f32(const float* q, long long ldq, const float* k, const float* v, long long ldkv, float* out,
                                      long long ldo, int B, int H, int head_dim, int Nq, int Tk, float scale, void* stream) {
-  ES3_REQUIRE(head_dim == 16 && Tk <= 16, "es3_attn_few_keys_f32: head_dim must be 16 and Tk <= 16 (got %d, %d)", head_dim, Tk);
-  const int smem = 2 * Tk * H * head_dim * (int)sizeof(float);
+  ES3_REQUIRE(head_dim == 16 && Tk > 0, "es3_attn_few_keys_f32: head_dim must be 16 and Tk > 0 (got %d, %d)", head_dim, Tk);
+  const int smem = 2 * std::min(Tk, FEW_KEYS_TILE) * H * head_dim * (int)sizeof(float);
   dim3 grid(ceil_div((long long)Nq * H, 256), B);
   attn_few_keys_f32_kernel<16><<<grid, 256, smem, (cudaStream_t)stream>>>(q, ldq, k, v, ldkv, out, ldo, Nq, Tk, H, scale);
   ES3_LAUNCH_CHECK("attn_few_keys_f32_kernel");

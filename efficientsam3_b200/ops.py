@@ -1204,15 +1204,15 @@ def add_rows(x, add=None, out_bf16=False, out_f32=True):
     return yb, yf
 
 
-def nchw_to_tokens(x, addc=None, out_bf16=True, out_f32=True):
-    """x [B,C,H,W] fp32 (+ per-channel addc) -> token-major ([B*HW,C] fp32 | None, bf16 | None)."""
+def nchw_to_tokens(x, out_bf16=True, out_f32=True):
+    """x [B,C,H,W] fp32 -> token-major ([B*HW,C] fp32 | None, bf16 | None)."""
     _chk(x, torch.float32, "x")
     _ensure_init(x)
     x = x.contiguous()
     B, C, H, W = x.shape
     yf = torch.empty((B * H * W, C), device=x.device, dtype=torch.float32) if out_f32 else None
     yb = torch.empty((B * H * W, C), device=x.device, dtype=torch.bfloat16) if out_bf16 else None
-    _call("es3_nchw_f32_to_tokens", "nchw_to_tokens", _nb(x, yf, yb), 0, x.data_ptr(), _ptr(addc), _ptr(yf), _ptr(yb), B,
+    _call("es3_nchw_f32_to_tokens", "nchw_to_tokens", _nb(x, yf, yb), 0, x.data_ptr(), _ptr(yf), _ptr(yb), B,
           H * W, C, _stream())
     return yf, yb
 

@@ -307,14 +307,15 @@ int es3_fill_small_components(const float* in, float* out, int* labels_ws, int* 
                               float max_hole_area, float max_sprinkle_area, void* stream);
 /* y[m] = x[m] + add[m % R] over C channels; bf16 and/or fp32 output (queries + pe, keys + key_pe). */
 int es3_add_rows(const float* x, const float* add, long long M, int C, int R, void* y_bf16, float* y_f32, void* stream);
-/* [B,C,HW] fp32 (+ per-channel vector, e.g. no_mask_embed) -> token-major [B,HW,C] fp32 and/or bf16. */
-int es3_nchw_f32_to_tokens(const float* in, const float* addc, float* out_f32, void* out_bf16, int B, int HW, int C,
-                           void* stream);
+/* [B,C,HW] fp32 -> token-major [B,HW,C] fp32 and/or bf16. */
+int es3_nchw_f32_to_tokens(const float* in, float* out_f32, void* out_bf16, int B, int HW, int C, void* stream);
 /* Softmax attention, few queries (prompt tokens) x many keys; q fp32, k/v bf16 (kv_f32 = 0) or fp32; out fp32.
- * Replaces Attention core for self_attn / cross_attn_token_to_image (transformer.py:185-264). head_dim 16|32. */
+ * Replaces Attention core for self_attn / cross_attn_token_to_image (transformer.py:185-264). head_dim 16 (k/v bf16 or fp32)
+ * or 32 (k/v fp32). */
 int es3_attn_few_queries(const float* q, long long ldq, const void* k, const void* v, long long ldkv, int kv_f32, float* out,
                          long long ldo, int B, int H, int head_dim, int Tq, int Tk, float scale, void* stream);
-/* Softmax attention, many queries (image tokens, bf16) x <= 16 keys (fp32); out bf16 (cross_attn_image_to_token). */
+/* Softmax attention, many queries (image tokens, bf16) x any number of keys (fp32); out bf16
+ * (cross_attn_image_to_token). */
 int es3_attn_few_keys(const void* q, long long ldq, const float* k, const float* v, long long ldkv, void* out, long long ldo,
                       int B, int H, int head_dim, int Nq, int Tk, float scale, void* stream);
 /* y = gelu(LayerNorm_C(x) * w + b) on rows of C <= 128 channels -> bf16 (LayerNorm2d + GELU, mask_decoder.py:59-70). */

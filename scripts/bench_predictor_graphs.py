@@ -6,8 +6,8 @@ restatement of the SAM heads (oracle/sam_heads.py) on the same GPU and the same 
 
 Models: the point segmenter over the SAM3 ViT trunk and over the EV-M student encoder (build_efficientsam3_point_segmenter
 ("efficientvit", "b1")), both at 1008^2 with their default initialisation (the timing does not depend on the weights).  One
-set_image on a seeded 1500 x 2250 uint8 image, then predict with 1, 3 and 8 points, a box, a box plus a point and a point plus
-a mask_input, each with multimask_output True and False; the predictor's defaults otherwise (hole filling up to 256 px, binary
+set_image on a seeded 1500 x 2250 uint8 image, then predict with 1, 3, 8 and 12 points (6 output tokens, 12 points and the
+padding point: 19 image-to-token keys, more than one 16-key tile), a box, a box plus a point and a point plus a mask_input, each with multimask_output True and False; the predictor's defaults otherwise (hole filling up to 256 px, binary
 masks at the original size).  The oracle arm runs without hole filling: its fill_holes labels components with scipy on the CPU.
 Per arm and call: the median and p10-p90 of the device time (CUDA events around the call) and of the host time until predict
 returns (it returns host arrays, so both include the copy out).  The arms run in turn, `--rounds` times, so that a drift of the
@@ -57,9 +57,12 @@ def cases(low_prev):
     pts = rng.uniform([0, 0], [2250, 1500], size=(8, 2))
     lab = rng.integers(0, 2, size=8)
     box = np.array([300.0, 200.0, 1800.0, 1300.0])
+    pts12 = np.concatenate([pts, rng.uniform([0, 0], [2250, 1500], size=(4, 2))])     # drawn after: the first 8 stay as they were
+    lab12 = np.concatenate([lab, rng.integers(0, 2, size=4)])
     return {"1 point": dict(point_coords=pts[:1], point_labels=lab[:1]),
             "3 points": dict(point_coords=pts[:3], point_labels=lab[:3]),
             "8 points": dict(point_coords=pts, point_labels=lab),
+            "12 points": dict(point_coords=pts12, point_labels=lab12),
             "box": dict(box=box),
             "box + point": dict(box=box, point_coords=pts[:1], point_labels=lab[:1]),
             "point + mask_input": dict(point_coords=pts[:1], point_labels=lab[:1], mask_input=low_prev)}

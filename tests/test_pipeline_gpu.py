@@ -145,6 +145,12 @@ def test_interactive_predictor_api_vs_oracle(cuda):
     compare(out_b, oracle_for(0, pc[:1], pl[:1], box, None, False, hw), "box + point")
     out_m = pred.predict(point_coords=pc[:1], point_labels=pl[:1], mask_input=out_b[2], multimask_output=True, return_logits=True)
     compare(out_m, oracle_for(0, pc[:1], pl[:1], None, out_b[2], True, hw), "point + mask")
+    # --- long prompts (repeated clicks): 6 output tokens + the points + the padding point pass 16 image-to-token keys
+    many = np.stack([rng.uniform(0, 420, 20), rng.uniform(0, 300, 20)], 1)
+    many_lab = rng.integers(0, 2, 20)
+    for n, bx in ((10, None), (12, None), (20, None), (8, box)):
+        out_n = pred.predict(point_coords=many[:n], point_labels=many_lab[:n], box=bx, multimask_output=bx is None, return_logits=True)
+        compare(out_n, oracle_for(0, many[:n], many_lab[:n], bx, None, bx is None, hw), f"{'box + ' if bx is not None else ''}{n} points")
     bm = pred.predict(point_coords=pc, point_labels=pl, multimask_output=True)[0]
     # like the reference (`masks.squeeze(0).float()...numpy()`, :290) the thresholded masks come back as float32 0/1
     assert bm.dtype == np.float32 and set(np.unique(bm)) <= {0.0, 1.0} and np.array_equal(bm > 0.5, out[0] > 0)

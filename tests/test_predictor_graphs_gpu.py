@@ -64,10 +64,15 @@ def _prompt_cases(low_prev):
     pts = np.array([[210.0, 150.0], [30.0, 40.0], [400.0, 10.0], [5.0, 290.0], [100.0, 100.0]])
     lab = np.array([1, 0, 1, 1, 0])
     box = np.array([40.0, 30.0, 380.0, 260.0])
+    rng = np.random.default_rng(12)
+    many = np.stack([rng.uniform(0, 420, 12), rng.uniform(0, 300, 12)], 1)
+    many_lab = rng.integers(0, 2, 12)
     return {
         "N=1": dict(point_coords=pts[:1], point_labels=lab[:1]),
         "N=2": dict(point_coords=pts[:2], point_labels=lab[:2]),
         "N=5": dict(point_coords=pts, point_labels=lab),
+        "N=12": dict(point_coords=many, point_labels=many_lab),
+        "box+N=8": dict(box=box, point_coords=many[:8], point_labels=many_lab[:8]),
         "box": dict(box=box),
         "box+points": dict(box=box, point_coords=pts[:2], point_labels=lab[:2]),
         "point+mask": dict(point_coords=pts[:1], point_labels=lab[:1], mask_input=low_prev),

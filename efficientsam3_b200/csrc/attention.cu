@@ -266,8 +266,12 @@ extern "C" int es3_attention_bf16(const void* qkv, void* out, int B, int H, int 
 template <bool CAUSAL>
 static int attention_mma(const void* qkv, void* out, int B, int H, int W, int C, int num_heads, int win, float scale,
                          void* stream) {
-  ES3_REQUIRE(C == num_heads * AT_D, "es3_attention_bf16: head_dim must be 64 (C=%d heads=%d)", C, num_heads);
-  ES3_REQUIRE(win == 0 || (H % win == 0 && W % win == 0), "es3_attention_bf16: H,W must be multiples of the window (%d,%d,%d)", H, W, win);
+  const char* name = CAUSAL ? "es3_attention_causal_bf16" : "es3_attention_mma_bf16";
+  ES3_REQUIRE(B > 0 && H > 0 && W > 0 && win >= 0, "%s: bad shape B=%d H=%d W=%d win=%d", name, B, H, W, win);
+  ES3_REQUIRE(C == num_heads * AT_D, "%s: head_dim must be 64 (C=%d heads=%d)", name, C, num_heads);
+  // cp.async loads and the output's uint4 stores move 16 bytes at a time
+  ES3_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)out & 15) == 0, "%s: qkv and out must be 16-byte aligned", name);
+  ES3_REQUIRE(win == 0 || (H % win == 0 && W % win == 0), "%s: H,W must be multiples of the window (%d,%d,%d)", name, H, W, win);
   AttnArgs a;
   a.qkv = (const bf16*)qkv; a.out = (bf16*)out; a.H = H; a.W = W; a.C = C; a.win = win;
   a.nwx = win ? W / win : 1;

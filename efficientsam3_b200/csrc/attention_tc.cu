@@ -204,7 +204,11 @@ using namespace es3;
 // wgmma flash attention; same contract as es3_attention_bf16 (which dispatches here for L >= 128).
 extern "C" int es3_attention_tc_bf16(const void* qkv, void* out, int B, int H, int W, int C, int num_heads, int win,
                                      float scale, void* stream) {
+  ES3_REQUIRE(B > 0 && H > 0 && W > 0 && win >= 0, "es3_attention_tc_bf16: bad shape B=%d H=%d W=%d win=%d", B, H, W, win);
   ES3_REQUIRE(C == num_heads * FA_D, "es3_attention_tc_bf16: head_dim must be 64 (C=%d heads=%d)", C, num_heads);
+  // cp.async moves 16-byte chunks of qkv; the output is stored as bf16 pairs
+  ES3_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)out & 3) == 0,
+              "es3_attention_tc_bf16: qkv must be 16-byte and out 4-byte aligned");
   ES3_REQUIRE(win == 0 || (H % win == 0 && W % win == 0), "es3_attention_tc_bf16: H,W must be multiples of the window");
   FaArgs a;
   a.qkv = (const bf16*)qkv; a.out = (bf16*)out; a.H = H; a.W = W; a.C = C; a.win = win;

@@ -569,6 +569,8 @@ extern "C" int es3_attention_f32(const float* qkv, float* out, const float* bias
   ES3_REQUIRE(head_dim == 32 || head_dim == 64, "es3_attention_f32: head_dim must be 32 or 64 (got %d)", head_dim);
   ES3_REQUIRE(B > 0 && H > 0 && W > 0 && ld % 4 == 0 && q_off % 4 == 0 && k_off % 4 == 0 && v_off % 4 == 0 && head_stride % 4 == 0,
               "es3_attention_f32: bad layout");
+  // keys and values are read as float4 from qkv rows and from pad_row
+  ES3_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)pad_row & 15) == 0, "es3_attention_f32: qkv and pad_row must be 16-byte aligned");
   ES3_REQUIRE(win >= 0 && (win == 0 || (H % win == 0 && W % win == 0) || pad_row != nullptr),
               "es3_attention_f32: windows overhang the %dx%d grid and no pad_row was given", H, W);
   const int nwx = win ? ceil_div(W, win) : 1, nwin = win ? ceil_div(H, win) * nwx : 1;

@@ -150,7 +150,7 @@ extern "C" int es3_layernorm_f32_e4m3(const float* x, const float* gamma, const 
 }
 
 extern "C" int es3_im2col_patch(const float* x, void* cols, int B, int S, int P, int Kp, void* stream) {
-  ES3_REQUIRE(S % P == 0 && Kp >= 3 * P * P && Kp % 8 == 0, "es3_im2col_patch: bad S=%d P=%d Kp=%d", S, P, Kp);
+  ES3_REQUIRE(B > 0 && S % P == 0 && Kp >= 3 * P * P && Kp % 8 == 0, "es3_im2col_patch: bad B=%d S=%d P=%d Kp=%d", B, S, P, Kp);
   const int hp = S / P;
   const long long total = (long long)B * hp * hp * Kp;
   im2col_patch_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, (bf16*)cols, S, P, hp, hp, Kp, total);
@@ -159,6 +159,7 @@ extern "C" int es3_im2col_patch(const float* x, void* cols, int B, int S, int P,
 }
 
 extern "C" int es3_tokens_f32_to_nchw(const float* in, float* out, int B, int HW, int C, void* stream) {
+  ES3_REQUIRE(B > 0 && HW > 0 && C > 0, "es3_tokens_f32_to_nchw: bad shape B=%d HW=%d C=%d", B, HW, C);
   dim3 grid(ceil_div(HW, 32), ceil_div(C, 32), B);
   tokens_to_nchw_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(in, out, HW, C);
   ES3_LAUNCH_CHECK("tokens_to_nchw_kernel");

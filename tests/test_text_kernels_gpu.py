@@ -198,19 +198,25 @@ def test_attention_declined_shapes_write_nothing(cuda):
 
 # ----------------------------------------------------------------------------------------------------------- (2) LayerNorm
 LN_C = [128, 256, 384, 512, 640, 768, 896, 1024, 1280, 1536, 2048]          # every es3_layernorm_f32 instantiation
-LNF = [(C, M, pos, shift, out) for (C, M, pos, shift, out) in
+LNF = [(C, M, pos, shift, out, (3, 5, 4)) for (C, M, pos, shift, out) in
        _pairwise(dict(C=LN_C, M=[1, 7, 77 * 3, 1000], pos=[False, True], shift=[0.0, 30.0], out=["f32", "bf16", "both"]), seed=12)]
+LNF += [(1024, 2 * 5184, True, 0.0, "f32", (24, 72, 72))]                     # the ViT teacher's ln_pre: 24 x 24 table over 72 x 72
 
 
-@pytest.mark.parametrize("C,M,pos,shift,out", LNF)
-def test_layernorm_f32(cuda, C, M, pos, shift, out):
-    """All eleven lane-vector counts; the tiled positional add (ps = 3 over a 5 x 4 grid); mean-shifted rows; fp32 and / or bf16
-    stores (bf16 = bf16 of the same fp32 value bit for bit); ops.layernorm is bit-identical."""
+def _lnf_id(c):
+    return "-".join(map(str, c[:5])) + ("" if c[5] == (3, 5, 4) else "-ps{}-{}x{}".format(*c[5]))
+
+
+@pytest.mark.parametrize("C,M,pos,shift,out,geom", LNF, ids=[_lnf_id(c) for c in LNF])
+def test_layernorm_f32(cuda, C, M, pos, shift, out, geom):
+    """All eleven lane-vector counts; the tiled positional add (ps = 3 over a 5 x 4 grid, and the teacher's ln_pre: ps = 24 over
+    72 x 72 tokens of two images); mean-shifted rows; fp32 and / or bf16 stores (bf16 = bf16 of the same fp32 value bit for bit);
+    ops.layernorm is bit-identical."""
     lib = _lib(cuda)
-    g = _gen(cuda, "lnf", C, M, pos, shift, out)
+    g = _gen(cuda, "lnf", C, M, pos, shift, out) if geom == (3, 5, 4) else _gen(cuda, "lnf", C, M, pos, shift, out, geom)
     x = torch.randn(M, C, device=cuda, generator=g) + shift
     gm, bt = torch.randn(C, device=cuda, generator=g), torch.randn(C, device=cuda, generator=g)
-    ps, H, W = 3, 5, 4
+    ps, H, W = geom
     pt = torch.randn(ps * ps, C, device=cuda, generator=g) if pos else None
     yf, fins = _flat_out(M * C, torch.float32, cuda)
     yb, bins = _flat_out(M * C, torch.bfloat16, cuda)

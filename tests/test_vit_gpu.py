@@ -1,6 +1,8 @@
-"""GPU parity of the ViT-trunk kernels and of the native teacher encoder (module API -> C ABI).
+"""GPU parity of the native teacher encoder (module API -> C ABI) and of the QKV GEMM's RoPE epilogue.  The trunk's own kernels
+(attention, patch im2col, LayerNorm, the token layout change) are held element by element to fp64 bounds in
+tests/test_vit_kernels_gpu.py and tests/test_text_kernels_gpu.py.
 
-Tolerances (stated): kernels with bf16 outputs 1e-2 of the tensor scale; fp32-output kernels 2e-3;
+Tolerances (stated): the RoPE epilogue 2e-3 of the tensor scale;
 end-to-end trunk embedding (bf16 GEMM operands, fp32 residual stream, fp32 softmax/LN statistics):
 relative L2 <= 2e-2, cosine >= 0.9995 against the fp32 reference / oracle.
 """
@@ -23,64 +25,6 @@ def _bf(t):
 def _close(got, ref, tol, what=""):
     err = max_err_over_scale(got.float().cpu(), ref.float().cpu())
     assert err <= tol, f"{what}: max err / scale = {err:.3e} > {tol}"
-
-
-@pytest.mark.parametrize("M,C,pos", [(1000, 1024, False), (2 * 64, 256, True), (5184, 1024, True), (77, 128, False)])
-def test_layernorm(cuda, M, C, pos):
-    from efficientsam3_b200 import ops
-    g = torch.Generator().manual_seed(M)
-    x = (torch.randn(M, C, generator=g) * 3 + 1).to(cuda)
-    gam, bet = (torch.rand(C, generator=g) + 0.5).to(cuda), torch.randn(C, generator=g).to(cuda)
-    if pos:
-        H = W = int(math.isqrt(M // 2)) if M == 128 else 72
-        ps = 4 if M == 128 else 24
-        Bn = M // (H * W)
-        tab = torch.randn(ps * ps, C, generator=g).to(cuda)
-        full = tab.view(ps, ps, C).repeat(H // ps + 1, W // ps + 1, 1)[:H, :W].reshape(1, H * W, C).expand(Bn, -1, -1).reshape(M, C)
-        yb, yf = ops.layernorm(x, gam, bet, 1e-5, pos=tab, pos_size=ps, H=H, W=W, out_bf16=True, out_f32=True)
-        ref = F.layer_norm(x + full, (C,), gam, bet, 1e-5)
-    else:
-        yb, yf = ops.layernorm(x, gam, bet, 1e-5, out_bf16=True, out_f32=True)
-        ref = F.layer_norm(x, (C,), gam, bet, 1e-5)
-    _close(yf, ref, 1e-5, "layernorm f32")
-    _close(yb, ref, 1e-2, "layernorm bf16")
-
-
-def test_patch_embed(cuda):
-    from efficientsam3_b200 import ops
-    g = torch.Generator().manual_seed(0)
-    x = torch.randn(2, 3, 112, 112, generator=g).to(cuda)
-    w = (torch.randn(256, 3, 14, 14, generator=g) / 24).to(cuda)
-    kp = (588 + 7) // 8 * 8
-    cols = ops.im2col_patch(x, 14, kp)
-    wp = torch.zeros(256, kp, device=cuda, dtype=torch.bfloat16)
-    wp[:, :588] = w.reshape(256, -1).to(torch.bfloat16)
-    out = ops.gemm(cols, wp, out_dtype=torch.float32)
-    ref = F.conv2d(_bf(x).float(), _bf(w).float(), stride=14).permute(0, 2, 3, 1).reshape(-1, 256)
-    _close(out, ref, 2e-3, "patch embed")
-
-
-@pytest.mark.parametrize("impl", [None, "mma", "tc"])
-@pytest.mark.parametrize("B,H,W,heads,win", [(2, 8, 8, 4, 4), (1, 24, 24, 2, 8), (2, 24, 24, 2, 0), (1, 72, 72, 2, 24),
-                                             (1, 72, 72, 1, 0), (3, 6, 10, 2, 2), (1, 36, 20, 2, 0), (2, 16, 16, 1, 0)])
-def test_attention(cuda, B, H, W, heads, win, impl):
-    from efficientsam3_b200 import ops
-    C = heads * 64
-    g = torch.Generator().manual_seed(H * 7 + win)
-    qkv = _bf(torch.randn(B * H * W, 3 * C, generator=g)).to(cuda)
-    out = ops.attention(qkv, B, H, W, C, heads, win, 0.125, impl=impl)
-    t = qkv.float().view(B, H, W, 3, heads, 64)
-    if win:
-        t = t.view(B, H // win, win, W // win, win, 3, heads, 64).permute(0, 1, 3, 2, 4, 5, 6, 7).reshape(-1, win * win, 3, heads, 64)
-    else:
-        t = t.reshape(B, H * W, 3, heads, 64)
-    q, k, v = t.permute(2, 0, 3, 1, 4).unbind(0)
-    o = F.scaled_dot_product_attention(q, k, v)             # [B', heads, L, 64]
-    o = o.permute(0, 2, 1, 3).reshape(-1, win * win if win else H * W, C)
-    if win:
-        o = o.view(B, H // win, W // win, win, win, C).permute(0, 1, 3, 2, 4, 5)
-    ref = o.reshape(B * H * W, C)
-    _close(out, ref, 1e-2, "attention")
 
 
 @pytest.mark.parametrize("H,W,win", [(8, 8, 4), (24, 24, 0)])
@@ -108,13 +52,6 @@ def test_qkv_rope_epilogue(cuda, H, W, win):
     ref = lin.clone()
     ref[:, :, :, :2] = torch.view_as_real(qk)
     _close(out, ref.reshape(B * H * W, 3 * C), 2e-3, "rope epilogue")
-
-
-def test_tokens_to_nchw(cuda):
-    from efficientsam3_b200 import ops
-    x = torch.randn(2 * 35, 96, device=cuda)
-    y = ops.tokens_f32_to_nchw(x, 2, 5, 7)
-    assert torch.equal(y, x.view(2, 5, 7, 96).permute(0, 3, 1, 2).contiguous())
 
 
 def _check(got, ref, what, l2=2e-2, cs=0.9995):

@@ -141,6 +141,8 @@ SIGNATURES: dict[str, list] = {
     "es3_layernorm_f32_e4m3": [_vp, _vp, _vp, _f, _vp, _vp, _ll, _i, _vp],
     # opt-in FP8 attention of the ViT teacher (attention_fp8.cu)
     "es3_attention_fp8": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
+    # stage-1 image preparation from decoded uint8 (preprocess.cu)
+    "es3_prepare_images_u8": [_vp, _ll, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp],
 }
 
 # workspace-size helpers: name -> argtypes, restype long long
@@ -161,6 +163,7 @@ SIZE_HELPERS: dict[str, list] = {
     "es3_stem_wgrad_ws_floats": [_i, _i, _i, _i],
     "es3_litemla_bwd_ws_floats": [_i, _i, _i],
     "es3_litemla_bwd_generic_ws_floats": [_i, _i, _i, _i],
+    "es3_prepare_images_ws_floats": [_vp, _i, _i],
 }
 
 _lib = None

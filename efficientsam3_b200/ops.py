@@ -5,6 +5,7 @@ dtype / contiguity and raises (no CPU fallback -- a CPU tensor is an error, SURV
 """
 from __future__ import annotations
 
+import ctypes
 import math
 
 import torch
@@ -49,7 +50,8 @@ class strict_precision:
 
 # ------------------------------------------------------------------------------------ accounting
 # kernels launched per C-ABI call (memsets excluded) -- bench.py reports the sum as `gpu_launches`.
-KERNELS_PER_CALL = {"es3_colsum_f32": 2, "es3_layernorm_bwd": 2, "es3_litemla_attn_generic": 2, "es3_fill_small_components": 4, "es3_grad_norm": 2, "es3_adamw_flat": 2, "es3_litemla_attn_tc": 2, "es3_kd_loss_fwd": 2, "es3_channel_mean": 2, "es3_attention_fp8": 2}
+KERNELS_PER_CALL = {"es3_colsum_f32": 2, "es3_layernorm_bwd": 2, "es3_litemla_attn_generic": 2, "es3_fill_small_components": 4, "es3_grad_norm": 2, "es3_adamw_flat": 2, "es3_litemla_attn_tc": 2, "es3_kd_loss_fwd": 2, "es3_channel_mean": 2, "es3_attention_fp8": 2,
+                    "es3_prepare_images_u8": 2}
 launch_count = 0
 
 
@@ -1993,3 +1995,57 @@ def scale_channels_f32(x, gate):
     _call("es3_scale_channels_f32", "scale_channels_f32", 2 * _nb(x), x.numel(), x.data_ptr(), gate.data_ptr(), y.data_ptr(), B, H * W, C,
           _stream())
     return y
+
+
+# ------------------------------------------------------------------------------------ stage-1 image preparation
+PREPARE_MAX_IMAGES = 96   # images per es3_prepare_images_u8 call: its per-image descriptors travel as a kernel parameter
+
+
+def image_table_ws_floats(table, nbytes, S):
+    """Checks a packed-image table on the host -- `table` int64 [B,3] CPU rows (byte offset, h, w) into a uint8 buffer of `nbytes`
+    bytes, output size S -- and returns es3_prepare_images_ws_floats of the whole table.  Raises Es3Error on anything the kernels
+    cannot prepare (an empty batch, S < 1, a side < 1, an image outside the buffer, a side that resizes to 0); launches nothing."""
+    if table.device.type != "cpu" or table.dtype != torch.int64 or table.dim() != 2 or table.shape[1] != 3 or table.shape[0] < 1:
+        raise _lib.Es3Error(f"prepare_images: expected a non-empty int64 [B,3] CPU table, got {table.dtype} {tuple(table.shape)}")
+    if int(S) < 1:
+        raise _lib.Es3Error(f"prepare_images: output size {S} < 1")
+    off, h, w = table.unbind(1)
+    if bool((h < 1).any()) or bool((w < 1).any()):
+        raise _lib.Es3Error(f"prepare_images: image sizes must be >= 1, got {table[:, 1:].tolist()}")
+    if bool((off < 0).any()) or bool((off + h * w * 3 > nbytes).any()):
+        raise _lib.Es3Error(f"prepare_images: an image lies outside the {nbytes}-byte buffer: {table.tolist()}")
+    t = table.contiguous()
+    n = _lib.size("es3_prepare_images_ws_floats", t.data_ptr(), t.shape[0], int(S))
+    if n < 0:
+        raise _lib.Es3Error(f"prepare_images: an image of {t[:, 1:].tolist()} resizes to a side of 0 at S = {S}")
+    return n
+
+
+def prepare_images_u8(src, table, S, mean, std, out=None):
+    """ResizeLongestSide (antialiased bilinear, torch's taps) + (x - mean) / std + zero padding of a ragged uint8 batch:
+    src flat uint8 CUDA (HWC RGB images back to back), table int64 [B,3] CPU (byte offset, h, w) -> out [B,3,S,S] fp32."""
+    table = table.contiguous()
+    image_table_ws_floats(table, src.numel(), S)
+    if len(mean) != 3 or len(std) != 3:
+        raise _lib.Es3Error(f"prepare_images: mean / std need 3 channels, got {len(mean)} / {len(std)}")
+    _chk(src, torch.uint8, "src")
+    if src.dim() != 1 or not src.is_contiguous():
+        raise _lib.Es3Error("prepare_images: src must be a contiguous 1-D uint8 buffer")
+    B = table.shape[0]
+    if out is None:
+        out = torch.empty((B, 3, S, S), device=src.device, dtype=torch.float32)
+    _chk(out, torch.float32, "out")
+    if tuple(out.shape) != (B, 3, S, S) or not out.is_contiguous() or out.device != src.device:
+        raise _lib.Es3Error(f"prepare_images: out must be a contiguous [{B},3,{S},{S}] fp32 tensor on {src.device}")
+    _ensure_init(src)
+    mean_c, std_c = (ctypes.c_float * 3)(*map(float, mean)), (ctypes.c_float * 3)(*map(float, std))
+    chunks = [table[b:b + PREPARE_MAX_IMAGES] for b in range(0, B, PREPARE_MAX_IMAGES)]
+    ws = _f32ws(max(_lib.size("es3_prepare_images_ws_floats", c.data_ptr(), c.shape[0], S) for c in chunks), src.device)
+    for i, c in enumerate(chunks):
+        nb = c.shape[0]
+        nin = int((c[:, 1] * c[:, 2]).sum()) * 3
+        nws = _lib.size("es3_prepare_images_ws_floats", c.data_ptr(), nb, S)
+        _call("es3_prepare_images_u8", "prepare_images_u8", nin + 8 * nws + 12 * nb * S * S, 0,   # bandwidth-bound: bytes only
+              src.data_ptr(), src.numel(), c.data_ptr(), nb, int(S), mean_c, std_c, ws.data_ptr(),
+              out[i * PREPARE_MAX_IMAGES].data_ptr(), _stream())
+    return out

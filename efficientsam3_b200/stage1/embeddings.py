@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from .. import ops
+from .preprocess import MEAN, STD, is_uint8_batch, prepare_images
 
 SEED_BYTES = 4
 
@@ -220,10 +221,13 @@ class EmbeddingDumper:
 
 
 @torch.no_grad()
-def save_embeddings_one_epoch(model, data_loader, path: str, rank: int = 0, max_batch: int | None = None):
+def save_embeddings_one_epoch(model, data_loader, path: str, rank: int = 0, max_batch: int | None = None, img_size: int | None = None,
+                              mean=MEAN, std=STD):
     """Native counterpart of save_embeddings_one_epoch (save_embedding_image_stage1.py:69-126).
     `data_loader` yields ((samples, _), (keys, seeds)) with `samples` a list/tensor of [3,S,S] fp32 images, exactly what the
-    reference's write-mode DatasetWrapper + pseudo_collate produce.  Returns the number of records written."""
+    reference's write-mode DatasetWrapper + pseudo_collate produce, or decoded HWC uint8 images (a list or
+    stage1.preprocess.PackedImages), prepared on the device at `img_size` (default: model.img_size) with `mean` / `std`.
+    Returns the number of records written."""
     model.eval()
     dev = next(model.parameters()).device
     dumper = None
@@ -231,8 +235,11 @@ def save_embeddings_one_epoch(model, data_loader, path: str, rank: int = 0, max_
     with EmbeddingStoreWriter(path, rank) as writer:
         try:
             for (samples, _), (keys, seeds) in data_loader:
-                x = samples if torch.is_tensor(samples) else torch.stack(list(samples), dim=0)
-                x = x.to(dev, non_blocking=True)
+                if is_uint8_batch(samples):
+                    x, _ = prepare_images(samples, img_size or model.img_size, mean, std, device=dev)
+                else:
+                    x = samples if torch.is_tensor(samples) else torch.stack(list(samples), dim=0)
+                    x = x.to(dev, non_blocking=True)
                 out = model(x)
                 if dumper is None:
                     cap = (max_batch or getattr(data_loader, "batch_size", None) or x.shape[0]) * out[0].numel()

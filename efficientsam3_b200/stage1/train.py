@@ -9,6 +9,7 @@ import torch
 
 from .losses import kd_train_step
 from .optim import cosine_lr
+from .preprocess import MEAN, STD, is_uint8_batch, prepare_images
 
 
 def set_bn_state(config, model):
@@ -47,7 +48,9 @@ def lr_for_update(idx, epoch, num_steps, accum, lr_at):
 
 
 def train_one_epoch(config, model, data_loader, optimizer, epoch, lr_at=None, on_step=None):
-    """One epoch of stage-1 distillation.  `optimizer`: stage1.optim.FlatAdamW over `model`.  `lr_at(update_index) -> lr`
+    """One epoch of stage-1 distillation.  `samples` are the reference's [3,S,S] fp32 images with annos["img_size_before_pad"], or
+    decoded HWC uint8 images (a list or stage1.preprocess.PackedImages) that are prepared on the device with DATA.IMG_SIZE /
+    DATA.MEAN / DATA.STD, their sizes before padding coming from the preparation.  `optimizer`: stage1.optim.FlatAdamW over `model`.  `lr_at(update_index) -> lr`
     replaces `lr_scheduler.step_update` (default: the reference's cosine schedule built from config.TRAIN).  `on_step(idx, loss)`
     is called after every iteration with the detached device loss (call `.item()` there only when you log: it syncs).
     Returns the list of per-iteration losses (device scalars)."""
@@ -63,11 +66,16 @@ def train_one_epoch(config, model, data_loader, optimizer, epoch, lr_at=None, on
     dev = next(model.parameters()).device
     losses = []
     for idx, ((samples, annos), (saved_embeddings, seeds)) in enumerate(data_loader):
-        samples = torch.stack(list(samples), dim=0).to(dev, non_blocking=True)
+        if is_uint8_batch(samples):
+            samples, sizes_before_pad = prepare_images(samples, config.DATA.IMG_SIZE, getattr(config.DATA, "MEAN", MEAN),
+                                                       getattr(config.DATA, "STD", STD), device=dev)
+        else:
+            samples = torch.stack(list(samples), dim=0).to(dev, non_blocking=True)
+            sizes_before_pad = annos["img_size_before_pad"]
         saved = torch.from_numpy(np.stack(saved_embeddings, axis=0)).float()
         saved = saved.view(samples.size(0), *embed_shape).to(dev, non_blocking=True)
         update = (idx + 1) % accum == 0
-        loss = kd_train_step(model, optimizer, samples, saved, annos["img_size_before_pad"], cosine_weight=cosine_w,
+        loss = kd_train_step(model, optimizer, samples, saved, sizes_before_pad, cosine_weight=cosine_w,
                              clip_grad=config.TRAIN.CLIP_GRAD,
                              lr=lr_for_update(idx, epoch, num_steps, accum, lr_at) if update else None,
                              accumulation_steps=accum, update=update)

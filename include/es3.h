@@ -346,6 +346,18 @@ int es3_win_attn_bias_bf16(const void* qkv, const void* qkv_pad, const float* bi
 /* LayerNorm over bf16 rows, C % 8 == 0 (TinyViT token stream: Attention.norm / Mlp.norm, tiny_vit.py:206,240). */
 int es3_layernorm_bf16(const void* x, const float* gamma, const float* beta, float eps, void* y, long long M, int C, void* stream);
 
+/* ------------------------------------------------------------------------------------------ stage-1 input */
+/* SA1BDataset's image preparation (stage1/data/sa1b_dataset.py:163-170, 216-227) on the device, for a ragged batch of decoded images:
+ * ResizeLongestSide.apply_image_torch (transforms.py:48-54, 79-85: F.interpolate bilinear, align_corners=False, antialias=True, torch's
+ * tap windows and fp32 weights), then (x - mean[c]) / std[c], then zero padding to S x S.  src: uint8 HWC RGB images back to back,
+ * src_bytes long; table: HOST int64 [B][3] = (byte offset, h, w); mean / std: HOST float[3].  out [B,3,S,S] fp32 NCHW, image b resized to
+ * (h', w') = get_preprocess_shape(h, w, S) and +0 in rows >= h' and columns >= w'.  Two launches (horizontal pass into ws, then vertical
+ * pass + normalisation + padding); B <= 96 per call.  ws: es3_prepare_images_ws_floats(table, B, S) floats, which is -1 when B < 1,
+ * S < 1, or an image has h or w < 1 or resizes to a side < 1. */
+long long es3_prepare_images_ws_floats(const long long* table, int B, int S);
+int es3_prepare_images_u8(const unsigned char* src, long long src_bytes, const long long* table, int B, int S, const float* mean,
+                          const float* std, float* ws, float* out, void* stream);
+
 /* ------------------------------------------------------------------------------------------ stage-1 loss */
 /* Masked MSE + masked cosine KD loss, forward (stage1/train_image_encoder_stage1.py:205-210, 271-307).
  * preds / teacher [B,C,E,E] fp32 NCHW; sizes_hw int32 [B][2] (h, w before padding); ws: B*ceil(E*E/256)*3 floats;

@@ -12,7 +12,7 @@ from pathlib import Path
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = _HERE / "libes3.so"
 
-_vp, _ll, _i, _f = C.c_void_p, C.c_longlong, C.c_int, C.c_float
+_vp, _ll, _i, _f, _d = C.c_void_p, C.c_longlong, C.c_int, C.c_float, C.c_double
 
 # name -> argtypes  (restype is always int unless noted)
 SIGNATURES: dict[str, list] = {
@@ -143,6 +143,10 @@ SIGNATURES: dict[str, list] = {
     "es3_attention_fp8": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp],
     # stage-1 image preparation from decoded uint8 (preprocess.cu)
     "es3_prepare_images_u8": [_vp, _ll, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp],
+    # automatic mask generation post-processing (amg.cu)
+    "es3_amg_mask_stats": [_vp, _vp] + [_i] * 10 + [_d] * 4 + [_i] + [_vp] * 7 + [_i, _vp],
+    "es3_box_nms": [_vp, _vp, _i, _d, _vp, _vp, _vp, _vp],
+    "es3_amg_rle": [_vp] + [_i] * 9 + [_f, _vp, _vp, _i, _vp, _vp, _vp, _vp],
 }
 
 # workspace-size helpers: name -> argtypes, restype long long
@@ -164,6 +168,9 @@ SIZE_HELPERS: dict[str, list] = {
     "es3_litemla_bwd_ws_floats": [_i, _i, _i],
     "es3_litemla_bwd_generic_ws_floats": [_i, _i, _i, _i],
     "es3_prepare_images_ws_floats": [_vp, _i, _i],
+    "es3_amg_mask_stats_ws_floats": [_i],
+    "es3_box_nms_ws_floats": [_i],
+    "es3_amg_rle_ws_floats": [_i, _i],
 }
 
 _lib = None

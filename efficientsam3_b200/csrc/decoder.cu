@@ -3,7 +3,7 @@
 // The dense contractions over the 5184 image tokens run on gemm_tc.cu; everything here is either tiny
 // (8 prompt/output tokens per image: latency-bound) or a streaming pass over the image tokens / masks.
 // Token-side math is fp32 end to end (it feeds the mask logits through the hypernetwork).
-#include "common.cuh"
+#include "bilinear.cuh"
 
 namespace es3 {
 
@@ -271,15 +271,10 @@ __global__ void bilinear_nchw_kernel(const float* __restrict__ in, float* __rest
   const int ox = (int)(idx % Wo);
   const int oy = (int)((idx / Wo) % Ho);
   const long long pl = idx / ((long long)Wo * Ho);
-  float fy = (oy + 0.5f) * sy - 0.5f, fx = (ox + 0.5f) * sx - 0.5f;
-  if (fy < 0.f) fy = 0.f;
-  if (fx < 0.f) fx = 0.f;
-  const int y0 = min((int)fy, Hi - 1), x0 = min((int)fx, Wi - 1);
-  const int y1 = min(y0 + 1, Hi - 1), x1 = min(x0 + 1, Wi - 1);
-  const float ly = fy - y0, lx = fx - x0, hy = 1.f - ly, hx = 1.f - lx;
+  const BilinearTap ty = bilinear_tap(oy, sy, Hi), tx = bilinear_tap(ox, sx, Wi);
   const float* p = in + pl * Hi * Wi;
-  const float v = hy * (hx * __ldg(p + y0 * Wi + x0) + lx * __ldg(p + y0 * Wi + x1)) +
-                  ly * (hx * __ldg(p + y1 * Wi + x0) + lx * __ldg(p + y1 * Wi + x1));
+  const float v = bilinear_mix(ty, tx, __ldg(p + ty.i0 * Wi + tx.i0), __ldg(p + ty.i0 * Wi + tx.i1), __ldg(p + ty.i1 * Wi + tx.i0),
+                               __ldg(p + ty.i1 * Wi + tx.i1));
   if (out) out[idx] = v;
   if (bin) bin[idx] = v > thr ? 1 : 0;
 }

@@ -1282,6 +1282,90 @@ def bilinear_nchw(x, Ho, Wo, binarize_thr=None, want_float=True):
     return out, binm
 
 
+# ------------------------------------------------------------------------------------ automatic mask generation (amg.cu)
+KERNELS_PER_CALL.update({"es3_amg_mask_stats": 4, "es3_box_nms": 3, "es3_amg_rle": 3})
+
+
+class AmgArena:
+    """The masks of one crop that passed es3_amg_mask_stats' filters, in the order they were appended: low-res logits
+    `low` [cap,Hi,Wi] fp32, `box` [cap,4] int32 (XYXY, inclusive, crop frame), `iou` and `stab` [cap] fp32, `point` [cap] int32
+    (index into the crop's point grid) and the device-side `count` [1] int32, which may run past cap (nothing is stored there)."""
+
+    def __init__(self, cap, Hi, Wi, device):
+        self.cap, self.Hi, self.Wi = int(cap), int(Hi), int(Wi)
+        self.low = torch.empty((self.cap, Hi, Wi), device=device, dtype=torch.float32)
+        self.box = torch.empty((self.cap, 4), device=device, dtype=torch.int32)
+        self.iou = torch.empty(self.cap, device=device, dtype=torch.float32)
+        self.stab = torch.empty(self.cap, device=device, dtype=torch.float32)
+        self.point = torch.empty(self.cap, device=device, dtype=torch.int32)
+        self.count = torch.zeros(1, device=device, dtype=torch.int32)
+
+    def reset(self):
+        self.count.zero_()
+        return self
+
+
+def _crop_args(crop_box, orig_hw):
+    x0, y0, x1, y1 = (int(v) for v in crop_box)
+    return x0, y0, x1, y1, int(orig_hw[1]), int(orig_hw[0])
+
+
+def amg_mask_stats(low, iou, crop_box, orig_hw, arena, mask_threshold=0.0, stability_score_offset=1.0, pred_iou_thresh=0.0,
+                   stability_score_thresh=0.0, point_base=0):
+    """One decoded batch low [P,K,Hi,Wi] fp32 / iou [P,K] fp32 of the crop `crop_box` (XYXY) of an image of size orig_hw (h, w):
+    the masks that pass the IoU, stability and crop-edge filters are appended to `arena` (see es3_amg_mask_stats)."""
+    _chk(low, torch.float32, "low"); _chk(iou, torch.float32, "iou")
+    _ensure_init(low)
+    assert low.dim() == 4 and iou.shape == low.shape[:2], (tuple(low.shape), tuple(iou.shape))
+    P, K, Hi, Wi = low.shape
+    assert (Hi, Wi) == (arena.Hi, arena.Wi), ((Hi, Wi), (arena.Hi, arena.Wi))
+    low, iou = low.contiguous(), iou.contiguous()
+    M = P * K
+    ws = torch.empty(_lib.size("es3_amg_mask_stats_ws_floats", M), device=low.device, dtype=torch.int32)
+    x0, y0, x1, y1, W, H = _crop_args(crop_box, orig_hw)
+    _call("es3_amg_mask_stats", "amg_mask_stats", _nb(low), 8 * M * (y1 - y0) * (x1 - x0), low.data_ptr(), iou.data_ptr(), M, K,
+          Hi, Wi, x0, y0, x1, y1, W, H, float(mask_threshold), float(stability_score_offset), float(pred_iou_thresh),
+          float(stability_score_thresh), int(point_base), ws.data_ptr(), arena.low.data_ptr(), arena.box.data_ptr(),
+          arena.iou.data_ptr(), arena.stab.data_ptr(), arena.point.data_ptr(), arena.count.data_ptr(), arena.cap, _stream())
+    return arena
+
+
+def box_nms(boxes, scores, iou_threshold):
+    """torchvision.ops.batched_nms (one category) on integer XYXY boxes [N,4] int32 with scores [N] fp32, equal scores in index
+    order -> (keep [N] int32, count [1] int32) on the device: keep[:count] are the kept indices, best first."""
+    _chk(boxes, torch.int32, "boxes"); _chk(scores, torch.float32, "scores")
+    _ensure_init(boxes)
+    boxes, scores = boxes.contiguous(), scores.contiguous()
+    N = scores.shape[0]
+    assert boxes.shape == (N, 4), tuple(boxes.shape)
+    keep = torch.empty(N, device=boxes.device, dtype=torch.int32)
+    count = torch.empty(1, device=boxes.device, dtype=torch.int32)
+    ws = torch.empty(max(1, _lib.size("es3_box_nms_ws_floats", N)), device=boxes.device, dtype=torch.float32)
+    _call("es3_box_nms", "box_nms", _nb(boxes, scores, keep), 0, boxes.data_ptr(), scores.data_ptr(), N, float(iou_threshold),
+          keep.data_ptr(), count.data_ptr(), ws.data_ptr(), _stream())
+    return keep, count
+
+
+def amg_rle(low, crop_box, orig_hw, mask_threshold=0.0, cap=None, binary=False):
+    """Masks low [K,Hi,Wi] fp32 of the crop `crop_box` in the orig_hw (h, w) frame -> (pos [K,cap] int32, n_trans [K] int32,
+    area [K] int32, uint8 [K,h,w] | None) on the device (see es3_amg_rle).  cap defaults to 4 transitions per column + 64."""
+    _chk(low, torch.float32, "low")
+    _ensure_init(low)
+    low = low.contiguous()
+    K, Hi, Wi = low.shape
+    x0, y0, x1, y1, W, H = _crop_args(crop_box, orig_hw)
+    cap = 4 * W + 64 if cap is None else int(cap)
+    dev = low.device
+    pos = torch.empty((K, cap), device=dev, dtype=torch.int32)
+    n_trans = torch.empty(K, device=dev, dtype=torch.int32)
+    area = torch.empty(K, device=dev, dtype=torch.int32)
+    binm = torch.empty((K, H, W), device=dev, dtype=torch.uint8) if binary else None
+    ws = torch.empty(_lib.size("es3_amg_rle_ws_floats", K, W), device=dev, dtype=torch.int32)
+    _call("es3_amg_rle", "amg_rle", _nb(low, binm), 16 * K * H * W, low.data_ptr(), K, Hi, Wi, x0, y0, x1, y1, W, H,
+          float(mask_threshold), ws.data_ptr(), pos.data_ptr(), cap, n_trans.data_ptr(), area.data_ptr(), _ptr(binm), _stream())
+    return pos, n_trans, area, binm
+
+
 def maxpool2x2(x):
     _chk(x, torch.bfloat16, "x")
     _ensure_init(x)

@@ -327,6 +327,39 @@ int es3_hyper_masks(const float* up, const float* hyper, const float* obj_logits
 int es3_bilinear_nchw_f32(const float* in, float* out, void* bin, float thr, long long planes, int Hi, int Wi, int Ho,
                           int Wo, void* stream);
 
+/* ------------------------------------------------------------------------------------------ automatic mask generation */
+/* Post-processing of SamAutomaticMaskGenerator (amg.cu).  Mask pixels are the bilinear (align_corners=False) samples of the
+ * low-res logits at the crop's size, evaluated exactly as es3_bilinear_nchw_f32 evaluates them; nothing is materialised at
+ * that size.
+ *
+ * es3_amg_mask_stats: one batch of M = P*K decoded masks low [M,Hi,Wi] fp32 with predicted IoU iou [M], crop box XYXY in an
+ * orig_w x orig_h image.  Filters in the reference's order: iou > pred_iou_thresh (when > 0), stability =
+ * #(v > thr + offset) / #(v > thr - offset) >= stability_thresh (when > 0; 0/0 = NaN fails), then the box of (v > thr) (XYXY,
+ * inclusive, crop frame; [0,0,0,0] when empty) must not lie within 20 px of a crop edge that is not an image edge.  Thresholds
+ * are doubles rounded to fp32 as torch compares them.  Survivors are appended in mask order to the arena at *arena_count:
+ * logits arena_low [cap,Hi,Wi], arena_box [cap,4] int32, arena_iou, arena_stab [cap], arena_point [cap] = point_base + m / K.
+ * *arena_count is advanced by the number of survivors even past arena_cap (nothing is written past it).  ws:
+ * es3_amg_mask_stats_ws_floats(M) ints.  Four kernels. */
+long long es3_amg_mask_stats_ws_floats(int M);
+int es3_amg_mask_stats(const float* low, const float* iou, int M, int K, int Hi, int Wi, int crop_x0, int crop_y0, int crop_x1,
+                       int crop_y1, int orig_w, int orig_h, double mask_threshold, double offset, double pred_iou_thresh,
+                       double stability_thresh, int point_base, int* ws, float* arena_low, int* arena_box, float* arena_iou,
+                       float* arena_stab, int* arena_point, int* arena_count, int arena_cap, void* stream);
+/* torchvision.ops.batched_nms with one category on N <= 65536 integer-valued XYXY boxes [N,4] int32: IoU in fp32 as
+ * inter / (area_i + area_j - inter), suppression when IoU > iou_threshold.  Scores are ranked descending with NaN first; equal
+ * scores keep the lower index first (a stable sort).  keep [N] receives the kept indices in that order, *count their number.
+ * ws: es3_box_nms_ws_floats(N) floats, 8-byte aligned.  Three kernels. */
+long long es3_box_nms_ws_floats(int N);
+int es3_box_nms(const int* boxes, const float* scores, int N, double iou_threshold, int* keep, int* count, void* ws, void* stream);
+/* Column-major (SAM's) run-length encoding of K masks low [K,Hi,Wi] of one crop in the orig_w x orig_h frame: a pixel
+ * outside the crop is 0, one inside is (bilinear sample > mask_threshold).  pos [K,cap]: the positions p (x * orig_h + y) where
+ * the value changes from p - 1 (the value before p = 0 is 0), so the run lengths are the differences of [0, pos..., H*W];
+ * n_trans [K] their number (a mask with n_trans > cap writes no positions), area [K] the number of ones.  bin (optional):
+ * uint8 [K,orig_h,orig_w] row-major.  ws: es3_amg_rle_ws_floats(K, orig_w) ints.  Three kernels. */
+long long es3_amg_rle_ws_floats(int K, int W);
+int es3_amg_rle(const float* low, int K, int Hi, int Wi, int crop_x0, int crop_y0, int crop_x1, int crop_y1, int orig_w,
+                int orig_h, float mask_threshold, int* ws, int* pos, int cap, int* n_trans, int* area, void* bin, void* stream);
+
 /* ------------------------------------------------------------------------------------------ RepViT / TinyViT */
 /* Dense 3x3, stride 2, pad 1 with a narrow input (second patch-embed conv: repvit.py:222-223, tiny_vit.py:75-81) on
  * mma.sync.  x [B,H,W,Cin] bf16; w [9][Cout][Cin] bf16 (tap, out channel, in channel); folded-BN scale/bias;

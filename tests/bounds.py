@@ -1,5 +1,7 @@
-"""Shared harness of the element-by-element GPU tests (tests/test_gemm_epilogue_gpu.py, tests/test_train_bwd_gpu.py): covering
-designs, per-element bound checks with a worst err/bound report, NaN-sentinel output buffers and NaN-padded strided operands."""
+"""Shared harness of the element-by-element GPU tests (the gemm_epilogue, train_bwd, fwd_kernels, text_kernels, sam_kernels,
+vit_kernels and amg files): covering designs, per-element bound checks with a worst err/bound report, NaN-sentinel output buffers,
+NaN-padded strided operands, and the calling primitives -- the library, stream and pointers, repeat runs that must be bit-identical,
+and declined shapes that must write nothing."""
 import itertools
 import random
 import zlib
@@ -122,3 +124,65 @@ def _padded(t, strided):
     big = torch.full((t.shape[0], t.shape[1] + 16), float("nan"), dtype=t.dtype, device=t.device)
     big[:, 8:8 + t.shape[1]] = t
     return big[:, 8:8 + t.shape[1]]
+
+
+def _st():
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _p(t):
+    return 0 if t is None else t.data_ptr()
+
+
+def _lib(cuda):
+    from efficientsam3_b200 import _lib
+    _lib.init(cuda.index or 0)
+    return _lib
+
+
+def _bits_equal(a, b, what):
+    a, b = a.contiguous(), b.contiguous()
+    if a.dtype in _INT:
+        a, b = a.view(_INT[a.dtype]), b.view(_INT[b.dtype])
+    assert torch.equal(a, b), what
+
+
+def _twice(run, buf):
+    """run(buffer) on two copies of the prefilled buffer; both must be bit-identical.  Returns the first."""
+    a, b = buf.clone(), buf.clone()
+    run(a)
+    run(b)
+    _bits_equal(a, b, "two runs differ")
+    return a
+
+
+def _prefilled(n, cuda, g):
+    """A flat fp32 buffer of n + TAIL cells: n random values (an accumulating output's prior contents), then NaN sentinels."""
+    buf, inside = _flat_out(n, torch.float32, cuda)
+    buf[:n] = torch.randn(n, device=cuda, generator=g)
+    return buf, inside
+
+
+def _declined(lib, name, args, bufs, what):
+    """A shape `name` declines: the call raises and every buffer keeps its bits."""
+    from efficientsam3_b200._lib import Es3Error
+    before = [b.clone() for b in bufs]
+    with pytest.raises(Es3Error):
+        lib.call(name, *args)
+    torch.cuda.synchronize()
+    for b, b0 in zip(bufs, before):
+        _bits_equal(b, b0, f"{what}: a declined call wrote")
+
+
+def _qkv(cuda, B, L, heads, kind, g):
+    """bf16 qkv rows [B L, 3 C] (head_dim 64): normal, peaked (scores spread by ~100), flat (q = 0) or tied (keys of period 5)."""
+    C = 64 * heads
+    x = torch.randn(B * L, 3 * C, device=cuda, generator=g) * 1.5
+    if kind == "peaked":                                   # scores spread by ~100: near one-hot rows
+        x[:, :2 * C] *= 5
+    elif kind == "flat":                                   # q = 0: every score 0, p = 1
+        x[:, :C] = 0
+    elif kind == "tied":                                   # keys repeat with period 5: tied maxima in every row, across KV tiles
+        k = x[:, C:2 * C].view(B, L, C)
+        x[:, C:2 * C] = k[:, torch.arange(L, device=cuda) % 5].reshape(B * L, C)
+    return _bf(x)

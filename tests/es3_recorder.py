@@ -1,6 +1,8 @@
-"""Records the es3_* calls a piece of native work makes (the route-closure tests of tests/test_train_bwd_gpu.py,
-tests/test_fwd_kernels_gpu.py and tests/test_text_kernels_gpu.py): every _lib.call, and every _lib.call_rc that ran (rc == 0; a
-declined shape returns -1)."""
+"""Records the es3_* calls a piece of native work makes (tests/test_route_closure_gpu.py): every _lib.call, and every _lib.call_rc
+that ran (rc == 0; a declined shape returns -1); and builds the model paths recorded there -- the image students' eval forward and
+training step, the text students' training steps and the SAM3 text teacher, the interactive predictor and the SAM heads' module
+API, the SAM3 image teacher, ViT backbones and the point segmenter's set_image."""
+import numpy as np
 import torch
 
 STUDENTS = ["efficientvit_b0", "efficientvit_b1", "efficientvit_b2", "repvit_m0_9", "repvit_m1_1", "repvit_m2_3", "tiny_vit_5m",
@@ -126,3 +128,128 @@ def text_teacher_calls(cuda, monkeypatch):
         with torch.no_grad():
             t(caps, device=cuda)
     return record_calls(monkeypatch, run)
+
+
+def point_segmenter(kind, cuda):
+    """Sam3PointPromptSegmenter with deterministic weights: the ViT override with one windowed block ("vit") or EV-B1 at 448 px."""
+    from efficientsam3_b200.model.sam1_task import Sam3PointPromptSegmenter
+    from efficientsam3_b200.model_builder import build_efficientsam3_point_segmenter
+    from oracle.weights import fill_state_dict
+    if kind == "vit":
+        seg = Sam3PointPromptSegmenter(vit_overrides=dict(depth=1, global_att_blocks=()))
+    else:
+        seg = build_efficientsam3_point_segmenter("efficientvit", "b1", image_size=448)
+    seg.load_state_dict({k: v for k, v in fill_state_dict(seg.state_dict(), 43).items() if not v.is_complex()}, strict=False)
+    return seg.to(cuda)
+
+
+def predictor_calls(seg, monkeypatch):
+    """The es3_* calls of SAM3InteractiveImagePredictor over `seg` (points, box, box + points, point + mask, mask only, 12 points;
+    multimask and return_logits on and off) and of seg.predict_batch (object-gated, 11 points), after set_image."""
+    from efficientsam3_b200.model.sam1_task import SAM3InteractiveImagePredictor
+    pred = SAM3InteractiveImagePredictor(seg, max_hole_area=64.0, max_sprinkle_area=16.0)
+    rng = np.random.default_rng(3)
+    img = rng.integers(0, 256, size=(300, 420, 3), dtype=np.uint8)
+    pred.set_image(img)
+    pts = np.stack([rng.uniform(0, 420, 12), rng.uniform(0, 300, 12)], 1)
+    lab = rng.integers(0, 2, 12)
+    box = np.array([40.0, 30.0, 380.0, 260.0])
+    low = pred.predict(point_coords=pts[:1], point_labels=lab[:1], multimask_output=False)[2]
+    prompts = [dict(point_coords=pts[:3], point_labels=lab[:3]), dict(box=box), dict(box=box, point_coords=pts[:2], point_labels=lab[:2]),
+               dict(point_coords=pts[:1], point_labels=lab[:1], mask_input=low), dict(mask_input=low),
+               dict(point_coords=pts, point_labels=lab)]
+
+    def run():
+        for kw in prompts:
+            for mm in (True, False):
+                for logits in (True, False):
+                    pred.predict(multimask_output=mm, return_logits=logits, **kw)
+        S = seg.image_size
+        dev = next(seg.parameters()).device
+        seg.set_image_batch(torch.randn(2, 3, S, S, generator=torch.Generator().manual_seed(1)).to(dev))
+        c = torch.rand(2, 11, 2, generator=torch.Generator().manual_seed(2)) * S
+        lb = torch.ones(2, 11, dtype=torch.int32)
+        for mm in (True, False):
+            for logits in (True, False):
+                seg.predict_batch(c.to(dev), lb.to(dev), multimask_output=mm, return_logits=logits)
+    return record_calls(monkeypatch, run)
+
+
+def sam_heads(E, S, sd_pe, sd_md, dev):
+    """PromptEncoder and MaskDecoder (two-way transformer, high-res features, object scores) with state dicts sd_pe / sd_md, eval."""
+    from efficientsam3_b200.sam import MaskDecoder, PromptEncoder, TwoWayTransformer
+    pe = PromptEncoder(embed_dim=256, image_embedding_size=(E, E), input_image_size=(S, S), mask_in_chans=16)
+    md = MaskDecoder(num_multimask_outputs=3, transformer=TwoWayTransformer(depth=2, embedding_dim=256, mlp_dim=2048, num_heads=8),
+                     transformer_dim=256, iou_head_depth=3, iou_head_hidden_dim=256, use_high_res_features=True,
+                     iou_prediction_use_sigmoid=True, pred_obj_scores=True, pred_obj_scores_mlp=True,
+                     use_multimask_token_for_obj_ptr=True)
+    pe.load_state_dict(sd_pe)
+    md.load_state_dict(sd_md)
+    return pe.to(dev).eval(), md.to(dev).eval()
+
+
+def module_api_calls(cuda, monkeypatch):
+    """The es3_* calls of the SAM heads' module API (sam_heads on the sam_heads_16 fixture's keys): points, boxes and a mask prompt,
+    multimask on and off."""
+    from helpers import load_golden, sd_from_keys
+    g = load_golden("sam_heads_16")
+    E, S, B = 16, 224, 2
+    pe, md = sam_heads(E, S, sd_from_keys(g["keys_pe"], 5), sd_from_keys(g["keys_md"], 6), cuda)
+    gen = torch.Generator().manual_seed(4)
+    feat = torch.randn(B, 256, E, E, generator=gen).to(cuda)
+    hr = [torch.randn(B, 32, 4 * E, 4 * E, generator=gen).to(cuda), torch.randn(B, 64, 2 * E, 2 * E, generator=gen).to(cuda)]
+    coords = (torch.rand(B, 3, 2, generator=gen) * S).to(cuda)
+    labels = torch.ones(B, 3, dtype=torch.int32, device=cuda)
+    boxes = torch.tensor([[10.0, 20.0, 100.0, 200.0]] * B, device=cuda)
+    masks = torch.randn(B, 1, 4 * E, 4 * E, generator=gen).to(cuda)
+
+    def run():
+        for kw in (dict(points=(coords, labels), boxes=None, masks=None), dict(points=None, boxes=boxes, masks=masks),
+                   dict(points=(coords, labels), boxes=boxes, masks=None)):
+            sp, de = pe(**kw)
+            for mm in (True, False):
+                md(image_embeddings=feat, image_pe=pe.get_dense_pe(), sparse_prompt_embeddings=sp, dense_prompt_embeddings=de,
+                   multimask_output=mm, repeat_image=False, high_res_features=hr)
+    return record_calls(monkeypatch, run)
+
+
+def teacher_calls(cuda, monkeypatch, strict):
+    """The es3_* calls of SAM3ImageTeacherEncoder at 1008 px (one windowed and one global block, B = 2), in the strict mode or not."""
+    from efficientsam3_b200 import ops
+    from efficientsam3_b200.stage1.model import SAM3ImageTeacherEncoder
+    t = SAM3ImageTeacherEncoder(embed_size=72, vit_overrides=dict(depth=2, global_att_blocks=(1,))).to(cuda)
+    x = torch.randn(2, 3, 1008, 1008, device=cuda, generator=torch.Generator(device=cuda).manual_seed(0))
+
+    def run():
+        with torch.no_grad():
+            if strict:
+                with ops.strict_precision():
+                    t(x)
+            else:
+                t(x)
+    return record_calls(monkeypatch, run)
+
+
+def backbone_calls(cuda, monkeypatch, which):
+    """The es3_* calls of create_sam3_vit_backbone's eval forward (B = 2) with tests/test_vit_gpu.py's 336 configuration or the
+    vit_small_112 fixture's."""
+    from efficientsam3_b200.model.vitdet import create_sam3_vit_backbone
+    from helpers import load_golden
+    cfg = (dict(img_size=336, pretrain_img_size=112, patch_size=14, embed_dim=256, depth=4, num_heads=4, mlp_ratio=4.625,
+                window_size=8, global_att_blocks=(1, 3)) if which == "336" else eval(str(load_golden("vit_small_112")["cfg"])))
+    m = create_sam3_vit_backbone(**cfg).to(cuda).eval()
+    x = torch.randn(2, 3, cfg["img_size"], cfg["img_size"], device=cuda, generator=torch.Generator(device=cuda).manual_seed(1))
+
+    def run():
+        with torch.no_grad():
+            m(x)
+    return record_calls(monkeypatch, run)
+
+
+def segmenter_set_image_calls(cuda, monkeypatch):
+    """The es3_* calls of the interactive predictor's set_image over Sam3PointPromptSegmenter (one windowed block), 600 x 800."""
+    from efficientsam3_b200.model.sam1_task import SAM3InteractiveImagePredictor, Sam3PointPromptSegmenter
+    seg = Sam3PointPromptSegmenter(vit_overrides=dict(depth=1, global_att_blocks=())).to(cuda).eval()
+    pred = SAM3InteractiveImagePredictor(seg)
+    img = np.random.default_rng(4).integers(0, 256, (600, 800, 3), dtype=np.uint8)
+    return record_calls(monkeypatch, lambda: pred.set_image(img))

@@ -21,21 +21,11 @@ import pytest
 import torch
 
 import ref_sam as R
-from bounds import TAIL, _INT, _assert_untouched, _flat_out, _gen
+from bounds import TAIL, _INT, _assert_untouched, _flat_out, _gen, _lib, _st
 from oracle import amg as OA
 from test_amg_cpu import assert_records_equal, case_kwargs, load_cases
 
 gpu = pytest.mark.gpu
-
-
-def _st():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _lib(cuda):
-    from efficientsam3_b200 import _lib
-    _lib.init(cuda.index or 0)
-    return _lib
 
 
 def _bits(t):

@@ -13,22 +13,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from es3_recorder import sam_heads as _build
 from helpers import cosine, load_golden, max_err_over_scale, rel_l2, sd_from_keys
 
 pytestmark = pytest.mark.gpu
-
-
-def _build(E, S, sd_pe, sd_md, dev):
-    import torch.nn as nn
-    from efficientsam3_b200.sam import MaskDecoder, PromptEncoder, TwoWayTransformer
-    pe = PromptEncoder(embed_dim=256, image_embedding_size=(E, E), input_image_size=(S, S), mask_in_chans=16)
-    md = MaskDecoder(num_multimask_outputs=3, transformer=TwoWayTransformer(depth=2, embedding_dim=256, mlp_dim=2048, num_heads=8),
-                     transformer_dim=256, iou_head_depth=3, iou_head_hidden_dim=256, use_high_res_features=True,
-                     iou_prediction_use_sigmoid=True, pred_obj_scores=True, pred_obj_scores_mlp=True,
-                     use_multimask_token_for_obj_ptr=True)
-    pe.load_state_dict(sd_pe)
-    md.load_state_dict(sd_md)
-    return pe.to(dev).eval(), md.to(dev).eval()
 
 
 def _inputs(B, E, S, seed):

@@ -7,14 +7,15 @@ bound, every cell outside it (a flat TAIL, the channels past C of an ldo > C row
 sentinel bits.  Workspaces (the LiteMLA KV partials, channel_mean's partials) are NaN-filled.  Strided operands are channel
 slices of NaN-padded buffers.  Where an ops wrapper adds routing it is called too and must be bit-identical to the direct call.
 Every persistent or tiled kernel runs twice and must be bit-identical, image i of a batch must be bit-identical to image i run
-alone, and a shape an entry point declines (returns -1) writes nothing.  A route-closure test records the forward kernels all
-nine students reach and asserts that some table row runs each of them.
+alone, and a shape an entry point declines (returns -1) writes nothing.  covered_keys() names the route keys (tests/routes.py)
+the tables run, for the route closure of tests/test_route_closure_gpu.py.
 
 GAMMA = 2 (ref_train_bwd.GAMMA) holds without change.  Worst err/bound per section in one run on an H100 80GB HBM3 (700 W power
 limit): fp32 outputs -- LiteMLA KV partials 0.0081 (generic) and 0.0015 (tensor core), channel_mean 0.0044, bilinear 0.0041;
 bf16 outputs -- 0.95 ... 0.996 in every other section (depthwise, MBConv, dwproj, stems, aggreg, LiteMLA, LayerNorm, window
 attention, scale_channels; LiteMLA tc 0.88), where the output's own rounding half-step dominates the bound and is reached.  The
-whole file (319 tests, the route-closure forwards and training steps included) took 34 s there.
+whole file (319 tests, the route-closure forwards and training steps included, since moved to tests/test_route_closure_gpu.py) took
+34 s there.
 """
 import math
 
@@ -23,27 +24,14 @@ import torch
 import torch.nn.functional as F
 
 import ref_fwd as R
-from bounds import TAIL, _INT, _assert_untouched, _bf, _check, _flat_out, _gen, _pairwise, report_worst
-from es3_recorder import STUDENTS, eval_forward_calls, training_step_calls
+from bounds import (TAIL, _assert_untouched, _bf, _bits_equal, _check, _flat_out, _gen, _lib, _p, _pairwise, _st, _twice,
+                    report_worst)
+from routes import dw_tc_key, ln_key
 
 pytestmark = pytest.mark.gpu
 _report_worst = report_worst("fwd kernels")
 ACT = {None: 0, "relu": 1, "hswish": 2, "gelu": 3}
 ACTS = [None, "relu", "hswish", "gelu"]
-
-
-def _st():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _p(t):
-    return 0 if t is None else t.data_ptr()
-
-
-def _lib(cuda):
-    from efficientsam3_b200 import _lib
-    _lib.init(cuda.index or 0)
-    return _lib
 
 
 def _out4(B, H, W, C, ld, dtype, cuda):
@@ -64,65 +52,10 @@ def _slice(x, extra):
     return big[..., 8:8 + x.shape[-1]]
 
 
-def _twice(run, buf):
-    """run(buffer) on two copies of the prefilled buffer; both must be bit-identical.  Returns the first."""
-    a, b = buf.clone(), buf.clone()
-    run(a)
-    run(b)
-    assert torch.equal(a.view(_INT[a.dtype]), b.view(_INT[b.dtype])), "two runs differ"
-    return a
-
-
-def _bits_equal(a, b, what):
-    assert torch.equal(a.contiguous().view(_INT[a.dtype]), b.contiguous().view(_INT[b.dtype])), what
-
-
 def _taps(lib, w):
     out = torch.full_like(w, float("nan"))
     lib.call("es3_round_taps_sum_bf16", w.data_ptr(), out.data_ptr(), w.shape[0], w.shape[1], _st())
     return out
-
-
-# ----------------------------------------------------------------------------------------------------------- route keys
-def dw_tc_key(ks, C, act):
-    return ("dw_tc", ks, 64 if ks == 3 and C % 64 == 0 else 32, act)
-
-
-def ln_key(C):
-    nv = C // 8
-    return ("layernorm", 8 if nv <= 8 else (16 if nv <= 16 else 32))
-
-
-def route_key(name, a):
-    """Route key of one recorded es3_* forward call: the instantiation its arguments select (None: not a kernel of this file)."""
-    act = {v: k for k, v in ACT.items()}
-    if name == "es3_mbconv_bf16":
-        return ("mbconv_tc" if a[16] == 1 else "mbconv_tc_s2", a[13], a[14], a[15], a[16])
-    if name == "es3_dwproj_tc_bf16":
-        return ("dwproj", a[11], a[12])
-    if name == "es3_dwconv_tc_bf16":
-        return dw_tc_key(a[10], a[9], act.get(a[11], a[11]))
-    if name == "es3_dwconv_tiled_bf16":
-        return ("dw_tiled", a[10], a[11], act.get(a[12], a[12]))
-    if name == "es3_dwconv_bf16":
-        return ("dw", a[10], a[11], act.get(a[12], a[12]))
-    if name == "es3_stem_conv3x3_s2":
-        return ("stem", a[7], act.get(a[8], a[8]))
-    if name == "es3_dsconv_res_bf16":
-        return ("dsconv", a[9], act.get(a[10], a[10]))
-    if name == "es3_litemla_attn_generic":
-        return ("litemla_generic", a[8])
-    if name == "es3_conv3x3_s2_narrow_bf16":
-        return ("narrow", a[8], a[9], act.get(a[10], a[10]))
-    if name == "es3_win_attn_bias_bf16":
-        return ("win_attn", a[9])
-    if name == "es3_layernorm_bf16":
-        return ln_key(a[6])
-    simple = {"es3_stem_fused_c16": "stem_fused", "es3_litemla_aggreg_dwpw": "aggreg", "es3_litemla_attn_tc": "litemla_tc",
-              "es3_channel_mean": "channel_mean", "es3_scale_channels": "scale_channels", "es3_round_taps_sum_bf16": "round_taps",
-              "es3_bilinear_nhwc_to_nchw": "bilinear", "es3_maxpool2x2_bf16": "maxpool", "es3_nhwc_to_nchw_f32": "nhwc_to_nchw",
-              "es3_nchw_f32_to_nhwc": "nchw_to_nhwc"}
-    return (simple[name],) if name in simple else None
 
 
 # ----------------------------------------------------------------------------------------------------------- (1) round_taps
@@ -633,37 +566,17 @@ def test_maxpool_and_layouts_bit_exact(cuda, B, H, W, C):
 
 # ----------------------------------------------------------------------------------------------------------- route closure
 def covered_keys():
-    """Every route key some table row above runs, computed from the tables with the key functions route_key uses."""
+    """Every route key (tests/routes.py) some table row above runs."""
     keys = {dw_tc_key(c[0][0], c[0][1], c[1]) for c in DWTC}
-    keys |= {("dw_tiled", 3, 2, c[1]) for c in DWT}
-    keys |= {("dw", c[0][0], c[0][1], c[1]) for c in DWG}
-    for fn, blocks in (("mbconv_tc", MB_TC), ("mbconv_tc_s2", MB_S2)):
-        keys |= {(fn,) + blk for blk in blocks}
-    keys |= {("dwproj", c[0], c[1]) for c in DWP}
-    keys |= {("stem", c[0], c[1]) for c in STEM} | {("dsconv", c[0], c[1]) for c in DSC}
-    keys |= {("narrow", c[0], c[1], c[2]) for c in NARROW}
-    keys |= {("litemla_generic", 16), ("litemla_generic", 32)}
-    keys |= {("win_attn", c[4]) for c in WIN} | {ln_key(c[0]) for c in LN}
-    keys |= {(k,) for k in ("stem_fused", "aggreg", "litemla_tc", "channel_mean", "scale_channels", "round_taps", "bilinear", "maxpool",
-                            "nhwc_to_nchw", "nchw_to_nhwc")}
+    keys |= {("es3_dwconv_tiled_bf16", 3, 2, c[1]) for c in DWT}
+    keys |= {("es3_dwconv_bf16", c[0][0], c[0][1], c[1]) for c in DWG}
+    keys |= {("es3_mbconv_bf16",) + blk for blk in MB_TC + MB_S2}
+    keys |= {("es3_dwproj_tc_bf16", c[0], c[1]) for c in DWP}
+    keys |= {("es3_stem_conv3x3_s2", c[0], c[1]) for c in STEM} | {("es3_dsconv_res_bf16", c[0], c[1]) for c in DSC}
+    keys |= {("es3_conv3x3_s2_narrow_bf16", c[0], c[1], c[2]) for c in NARROW}
+    keys |= {("es3_litemla_attn_generic", 16), ("es3_litemla_attn_generic", 32)}
+    keys |= {("es3_win_attn_bias_bf16", c[4]) for c in WIN} | {ln_key(c[0]) for c in LN}
+    keys |= {(k,) for k in ("es3_stem_fused_c16", "es3_litemla_aggreg_dwpw", "es3_litemla_attn_tc", "es3_channel_mean",
+                            "es3_scale_channels", "es3_round_taps_sum_bf16", "es3_bilinear_nhwc_to_nchw", "es3_maxpool2x2_bf16",
+                            "es3_nhwc_to_nchw_f32", "es3_nchw_f32_to_nhwc")}
     return keys
-
-
-@pytest.mark.parametrize("name", STUDENTS)
-def test_route_closure(cuda, monkeypatch, name):
-    """Every forward-kernel route `name` reaches in the eval forward at 1024^2 (batch 2) and in one native training step (1024^2,
-    embed 64, batch 1) with batch-statistics and with frozen BatchNorm is run by some table row above.  The eval forward of
-    efficientvit_b1 runs both Cin-128 MBConv blocks (its stage-3 blocks and stage-4 opener), that of efficientvit_b0 the stride-1
-    one (its stage-4 blocks)."""
-    calls = eval_forward_calls(cuda, monkeypatch, name)
-    cin128 = {route_key(n, a) for n, a in calls if n == "es3_mbconv_bf16" and a[13] == 128}
-    expected = {"efficientvit_b1": {("mbconv_tc",) + MB_TC[2], ("mbconv_tc_s2",) + MB_S2[3]},
-                "efficientvit_b0": {("mbconv_tc",) + MB_TC[2]}}.get(name)
-    if expected is not None:
-        assert cin128 == expected, f"{name}: Cin-128 MBConv routes {sorted(cin128)}, expected {sorted(expected)}"
-    for frozen in (False, True):
-        calls += training_step_calls(cuda, monkeypatch, name, frozen)
-    reached = {k for k in (route_key(n, a) for n, a in calls) if k is not None}
-    missing = reached - covered_keys()
-    print(f"\n{name}: {len(reached)} forward route keys reached: {sorted(reached, key=repr)}", end="")
-    assert not missing, f"{name} reaches forward routes no table row runs: {sorted(missing, key=repr)}"

@@ -29,21 +29,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from bounds import (L_ACT, U, _INT, _act64, _assert_untouched, _bf, _check, _eps_act, _flat_out, _gen, _matrix_out, _padded,
-                    _pairwise, report_worst, WORST)
+from bounds import (L_ACT, U, _INT, _act64, _assert_untouched, _bf, _check, _eps_act, _flat_out, _gen, _matrix_out, _p, _padded,
+                    _pairwise, _st, report_worst, WORST)
 
 pytestmark = pytest.mark.gpu
 
 GAMMA = 2.0                    # gamma_K = GAMMA * K * u
 _report_worst = report_worst("gemm epilogue")
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _ptr(t):
-    return 0 if t is None else t.data_ptr()
 
 
 def _expect(acc, absprod, K, act=None, scale=None, bias=None, res=None, after=False, out_bf16=False):
@@ -254,7 +246,7 @@ def _conv3x3(cuda, x, w, epi, bn=0, seed=0):
     buf, inside = _flat_out(B * H * W * N, dt, cuda)
     _lib.init(cuda.index or 0)
     rc = _lib.call_rc("es3_conv3x3_bf16", x.data_ptr(), w9.data_ptr(), buf.data_ptr(), int(dt == torch.float32), B, H, W, C, N,
-                      _ptr(scale), _ptr(bias), ops.ACT[act], _ptr(res), bn, _stream())
+                      _p(scale), _p(bias), ops.ACT[act], _p(res), bn, _st())
     assert rc == 0
     xn, wd = x.double().permute(0, 3, 1, 2), w.double()
     acc = F.conv2d(xn, wd, padding=1).permute(0, 2, 3, 1)
@@ -330,7 +322,7 @@ def _convt2x2(cuda, B, H, W, Cin, Cout, mode, res, out, seed=0):
     buf, inside = _flat_out(n, dt, cuda)
     _lib.init(cuda.index or 0)
     rc = _lib.call_rc("es3_convt2x2_bf16", x.data_ptr(), wt.data_ptr(), buf.data_ptr(), int(dt == torch.float32), B, H, W, Cin,
-                      Cout, bias4.data_ptr(), ops.ACT[act], _ptr(r), int(res == "f32"), int(after), _stream())
+                      Cout, bias4.data_ptr(), ops.ACT[act], _p(r), int(res == "f32"), int(after), _st())
     assert rc == 0
     xn = x.double().permute(0, 3, 1, 2)
     acc = F.conv_transpose2d(xn, w.double(), stride=2).permute(0, 2, 3, 1)

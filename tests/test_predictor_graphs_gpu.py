@@ -6,19 +6,9 @@ import numpy as np
 import pytest
 import torch
 
+from es3_recorder import point_segmenter as _seg
+
 pytestmark = pytest.mark.gpu
-
-
-def _seg(kind, cuda):
-    from efficientsam3_b200.model.sam1_task import Sam3PointPromptSegmenter
-    from efficientsam3_b200.model_builder import build_efficientsam3_point_segmenter
-    from oracle.weights import fill_state_dict
-    if kind == "vit":
-        seg = Sam3PointPromptSegmenter(vit_overrides=dict(depth=1, global_att_blocks=()))
-    else:
-        seg = build_efficientsam3_point_segmenter("efficientvit", "b1", image_size=448)
-    seg.load_state_dict({k: v for k, v in fill_state_dict(seg.state_dict(), 43).items() if not v.is_complex()}, strict=False)
-    return seg.to(cuda)
 
 
 @pytest.fixture(scope="module", params=["vit", "student"])

@@ -1,0 +1,99 @@
+"""Route closure: the es3_* calls real model paths make (tests/es3_recorder.py records them) select only kernel instantiations
+that some fp64 table row runs.  Each test hands its recorded calls to routes.assert_closed, which keys every call, requires a key
+function for every entry point reached and looks the key up in the tables of the files tests/routes.py lists for its entry point;
+the extra assertions pin routes a model is expected to reach."""
+import pytest
+
+from es3_recorder import (STUDENTS, TEXT_ROUTES, backbone_calls, eval_forward_calls, module_api_calls, point_segmenter,
+                          predictor_calls, segmenter_set_image_calls, teacher_calls, text_step_calls, text_teacher_calls,
+                          training_step_calls)
+from routes import KEYS, assert_closed
+
+pytestmark = pytest.mark.gpu
+
+
+# ----------------------------------------------------------------------------------------------------------- image students
+@pytest.mark.parametrize("step", ["eval", "train", "train frozen BN"])
+@pytest.mark.parametrize("name", STUDENTS)
+def test_route_closure_student(cuda, monkeypatch, name, step):
+    """The eval forward of `name` at 1024^2 (batch 2), or one native training step (1024^2, embed 64, batch 1) with batch-statistics
+    or frozen BatchNorm: each is recorded once and checked against the forward, backward and every other covering table.  The eval
+    forward of efficientvit_b1 runs both Cin-128 MBConv blocks (its stage-3 blocks and stage-4 opener), that of efficientvit_b0 the
+    stride-1 one (its stage-4 blocks)."""
+    if step != "eval":
+        assert_closed(training_step_calls(cuda, monkeypatch, name, step == "train frozen BN"), f"{name} {step}")
+        return
+    calls = eval_forward_calls(cuda, monkeypatch, name)
+    cin128 = {KEYS[n](a) for n, a in calls if n == "es3_mbconv_bf16" and a[13] == 128}
+    expected = {"efficientvit_b1": {("es3_mbconv_bf16", 128, 512, 128, 1), ("es3_mbconv_bf16", 128, 512, 256, 2)},
+                "efficientvit_b0": {("es3_mbconv_bf16", 128, 512, 128, 1)}}.get(name)
+    if expected is not None:
+        assert cin128 == expected, f"{name}: Cin-128 MBConv routes {sorted(cin128)}, expected {sorted(expected)}"
+    assert_closed(calls, f"{name} {step}")
+
+
+# ----------------------------------------------------------------------------------------------------------- text encoders
+@pytest.mark.parametrize("route", TEXT_ROUTES, ids=[r[0] for r in TEXT_ROUTES])
+def test_route_closure_text(cuda, monkeypatch, route):
+    """The native text training steps of es3_recorder.TEXT_ROUTES: S0 with frozen BN, S1, B, S3 at contexts 32, 77 and 128, the
+    77-entry table at 32 and at 128, masked and plain loss with consistency, and a batch of 512 x 77 tokens (LayerNorm backward over
+    more than 592 x 64 rows)."""
+    reached = assert_closed(text_step_calls(cuda, monkeypatch, *route[1:]), route[0])
+    if route[1] == "MobileCLIP-S0":
+        assert {("es3_repmixer_bf16",), ("es3_repmixer_tm_bwd",)} <= reached
+    if route[0] == "B ctx 128":
+        assert ("es3_attention_causal_bf16", 2) in reached
+    if route[0] == "S3 batch 512":
+        assert any(k[0] == "es3_layernorm_bwd_f32" and k[3] for k in reached)
+
+
+def test_route_closure_sam3_teacher(cuda, monkeypatch):
+    """The SAM3 text teacher's eval forward (width 1024, 16 heads, causal)."""
+    assert ("es3_attention_causal_bf16", 1) in assert_closed(text_teacher_calls(cuda, monkeypatch), "SAM3 text teacher")
+
+
+# ----------------------------------------------------------------------------------------------------------- SAM heads
+@pytest.mark.parametrize("kind", ["vit", "student"])
+def test_route_closure_predictor(cuda, monkeypatch, kind):
+    """SAM3InteractiveImagePredictor and Sam3PointPromptSegmenter.predict_batch (object-gated) on the ViT override and the EV-B1
+    student: points, box, box + points, point + mask, mask only, 12 points; multimask and return_logits on and off."""
+    reached = assert_closed(predictor_calls(point_segmenter(kind, cuda), monkeypatch), f"predictor {kind}")
+    assert ("es3_attn_few_keys", True) in reached                        # 12 points + 6 output tokens + the pad point: two tiles
+    assert ("es3_hyper_masks", True, 3, 1) in reached and ("es3_bilinear_nchw_f32", False, True) in reached
+
+
+def test_route_closure_strict(cuda, monkeypatch):
+    from efficientsam3_b200 import ops
+    seg = point_segmenter("student", cuda)
+    with ops.strict_precision():
+        reached = assert_closed(predictor_calls(seg, monkeypatch), "predictor strict")
+    assert ("es3_attn_few_keys_f32", True) in reached and any(k[0] == "es3_ln_rows_gelu_f32" for k in reached)
+
+
+def test_route_closure_module_api(cuda, monkeypatch):
+    """PromptEncoder / MaskDecoder / TwoWayTransformer as test_decoder_gpu builds them: points, boxes and a mask prompt."""
+    assert_closed(module_api_calls(cuda, monkeypatch), "module API")
+
+
+# ----------------------------------------------------------------------------------------------------------- SAM3 ViT trunk
+def test_route_closure_teacher(cuda, monkeypatch):
+    """SAM3ImageTeacherEncoder at 1008 px, one windowed and one global block, B = 2: both reach attn_tc_kernel<96>."""
+    reached = assert_closed(teacher_calls(cuda, monkeypatch, False), "teacher 1008")
+    assert {("es3_attention_bf16", "tc", 96, True), ("es3_attention_bf16", "tc", 96, False)} <= reached
+
+
+def test_route_closure_teacher_strict(cuda, monkeypatch):
+    reached = assert_closed(teacher_calls(cuda, monkeypatch, True), "teacher 1008 strict")
+    assert ("es3_attention_f32", 64, False, False, True) in reached and ("es3_attention_f32", 64, False, False, False) in reached
+
+
+@pytest.mark.parametrize("which", ["336", "vit_small_112"])
+def test_route_closure_backbone(cuda, monkeypatch, which):
+    """create_sam3_vit_backbone with tests/test_vit_gpu.py's 336 configuration and the vit_small_112 fixture's."""
+    assert_closed(backbone_calls(cuda, monkeypatch, which), f"ViT backbone {which}")
+
+
+def test_route_closure_segmenter(cuda, monkeypatch):
+    """Sam3PointPromptSegmenter (one windowed block) through the interactive predictor's set_image."""
+    reached = assert_closed(segmenter_set_image_calls(cuda, monkeypatch), "segmenter set_image")
+    assert ("es3_attention_bf16", "tc", 96, True) in reached

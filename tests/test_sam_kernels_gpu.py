@@ -5,94 +5,26 @@ Outputs are NaN-prefilled and called through _lib.call: every cell inside the ou
 every cell past it (a flat TAIL) keeps its sentinel bits.  Every kernel runs twice and must be bit-identical; the last prompt or image
 of a batch is bit-identical to the same one run alone; a shape an entry point declines writes nothing; the ops wrappers are
 bit-identical to the direct calls.  The copies (es3_nchw_f32_to_tokens, es3_add_rows' stores, the gated masks, the same-size resize)
-are bit-exact.  A route-closure test records the SAM-head kernels the interactive predictor and the point segmenter reach (ViT and
-EV-M student, every prompt kind, >= 10 points, both output modes, the object-gated batch path, the module API, strict mode) and
-asserts that some table row runs each of them.
+are bit-exact.  covered_keys() names the route keys (tests/routes.py) the tables run, for the route closure of
+tests/test_route_closure_gpu.py (the interactive predictor and the point segmenter on the ViT and an EV-B1 student, every prompt
+kind, >= 10 points, both output modes, the object-gated batch path, the module API, strict mode).
 
 GAMMA = 2 (ref_train_bwd.GAMMA) holds without change.  Worst err/bound per section in one run on an H100 80GB HBM3 (700 W power
 limit): bf16 outputs, where the output's own rounding half-step dominates the bound -- attn_few_keys 0.987, ln_rows_gelu 0.991,
 mask_downscale's bf16 store 0.977; fp32 outputs -- dense_pe 0.412, point_embed 0.376, add_rows 0.25, attn_few_keys_f32 0.059,
 attn_few_queries 0.014 (head_dim 16) and 0.048 (head_dim 32), ln_rows_gelu_f32 0.071, bilinear 0.432, hyper_masks 0.062,
-mask_downscale 0.0052.  The whole file (137 tests, the route-closure predictor runs included) took 15 s there.
+mask_downscale 0.0052.  The whole file (137 tests, the route-closure predictor runs included, since moved to tests/test_route_closure_gpu.py) took 15 s
+there.
 """
-import numpy as np
 import pytest
 import torch
 
 import ref_sam as R
-from bounds import TAIL, _INT, _assert_untouched, _bf, _check, _flat_out, _gen, _pairwise, report_worst
+from bounds import (TAIL, _assert_untouched, _bf, _bits_equal, _check, _declined, _flat_out, _gen, _lib, _p, _pairwise, _st, _twice,
+                    report_worst)
 
 pytestmark = pytest.mark.gpu
 _report_worst = report_worst("SAM-head kernels")
-
-
-def _st():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _p(t):
-    return 0 if t is None else t.data_ptr()
-
-
-def _lib(cuda):
-    from efficientsam3_b200 import _lib
-    _lib.init(cuda.index or 0)
-    return _lib
-
-
-def _twice(run, buf):
-    """run(buffer) on two copies of the prefilled buffer; both must be bit-identical.  Returns the first."""
-    a, b = buf.clone(), buf.clone()
-    run(a)
-    run(b)
-    assert torch.equal(a.view(_INT[a.dtype]), b.view(_INT[b.dtype])), "two runs differ"
-    return a
-
-
-def _bits_equal(a, b, what):
-    a, b = a.contiguous(), b.contiguous()
-    if a.dtype in _INT:
-        a, b = a.view(_INT[a.dtype]), b.view(_INT[b.dtype])
-    assert torch.equal(a, b), what
-
-
-def _declined(lib, name, args, bufs, what):
-    """A shape `name` declines: the call raises and every buffer keeps its bits."""
-    from efficientsam3_b200._lib import Es3Error
-    before = [b.clone() for b in bufs]
-    with pytest.raises(Es3Error):
-        lib.call(name, *args)
-    torch.cuda.synchronize()
-    for b, b0 in zip(bufs, before):
-        _bits_equal(b, b0, f"{what}: a declined call wrote")
-
-
-# ----------------------------------------------------------------------------------------------------------- route keys
-def route_key(name, a):
-    """Route key of one recorded es3_* call: what selects code (head_dim x K/V dtype, outputs present, base / pad / gate).  None: not a
-    kernel of this file."""
-    nz = lambda x: x not in (None, 0)
-    if name == "es3_dense_pe":
-        return ("dense_pe",)
-    if name == "es3_point_embed":
-        return ("point_embed", nz(a[8]))
-    if name == "es3_add_rows":
-        return ("add_rows", nz(a[1]), nz(a[5]), nz(a[6]))
-    if name == "es3_nchw_f32_to_tokens":
-        return ("nchw_to_tokens", nz(a[1]), nz(a[2]))
-    if name == "es3_attn_few_queries":
-        return ("attn_few_queries", a[10], bool(a[5]))
-    if name in ("es3_attn_few_keys", "es3_attn_few_keys_f32"):
-        return ("attn_few_keys", name.endswith("f32"), a[11] > 16)
-    if name in ("es3_ln_rows_gelu", "es3_ln_rows_gelu_f32"):
-        return ("ln_rows_gelu", name.endswith("f32"), a[6])
-    if name == "es3_hyper_masks":
-        return ("hyper_masks", nz(a[2]), a[9], a[10])
-    if name == "es3_bilinear_nchw_f32":
-        return ("bilinear", nz(a[1]), nz(a[2]))
-    if name == "es3_mask_downscale_tokens":
-        return ("mask_downscale", nz(a[11]), nz(a[13]), nz(a[14]))
-    return None
 
 
 # ----------------------------------------------------------------------------------------------------------- (1) positional encodings
@@ -546,101 +478,14 @@ def test_mask_downscale(cuda, hw, B, base, out, kind):
 
 # ----------------------------------------------------------------------------------------------------------- route closure
 def covered_keys():
-    """Every route key some table row above runs, computed from the tables with the key functions route_key uses."""
-    keys = {("dense_pe",)} | {("point_embed", pad) for _, _, pad, _ in POINTS}
-    keys |= {("add_rows", add != "none", out != "f32", out != "bf16") for add, out in ADD}
-    keys |= {("nchw_to_tokens", out != "bf16", out != "f32") for *_, out in NCHW}
-    keys |= {("attn_few_queries", hk[0], hk[1]) for _, _, hk, _, _ in FQ}
-    keys |= {("attn_few_keys", s, tk > 16) for tk, _, _, _, s in FK}
-    keys |= {("ln_rows_gelu", s, C) for C, _, _, s in LNG}
-    keys |= {("hyper_masks", gate, K, off) for (K, off), _, _, gate in HM}
-    keys |= {("bilinear", mode != "bin", mode != "float") for *_, mode in BIL}
-    keys |= {("mask_downscale", base, out != "bf16", out != "f32") for _, _, base, out, _ in MD}
+    """Every route key (tests/routes.py) some table row above runs."""
+    keys = {("es3_dense_pe",)} | {("es3_point_embed", pad) for _, _, pad, _ in POINTS}
+    keys |= {("es3_add_rows", add != "none", out != "f32", out != "bf16") for add, out in ADD}
+    keys |= {("es3_nchw_f32_to_tokens", out != "bf16", out != "f32") for *_, out in NCHW}
+    keys |= {("es3_attn_few_queries", hk[0], hk[1]) for _, _, hk, _, _ in FQ}
+    keys |= {("es3_attn_few_keys_f32" if s else "es3_attn_few_keys", tk > 16) for tk, _, _, _, s in FK}
+    keys |= {("es3_ln_rows_gelu_f32" if s else "es3_ln_rows_gelu", C) for C, _, _, s in LNG}
+    keys |= {("es3_hyper_masks", gate, K, off) for (K, off), _, _, gate in HM}
+    keys |= {("es3_bilinear_nchw_f32", mode != "bin", mode != "float") for *_, mode in BIL}
+    keys |= {("es3_mask_downscale_tokens", base, out != "bf16", out != "f32") for _, _, base, out, _ in MD}
     return keys
-
-
-def _seg(kind, cuda):
-    from test_predictor_graphs_gpu import _seg as build
-    return build(kind, cuda)
-
-
-def _predictor_calls(seg, monkeypatch):
-    from es3_recorder import record_calls
-    from efficientsam3_b200.model.sam1_task import SAM3InteractiveImagePredictor
-    pred = SAM3InteractiveImagePredictor(seg, max_hole_area=64.0, max_sprinkle_area=16.0)
-    rng = np.random.default_rng(3)
-    img = rng.integers(0, 256, size=(300, 420, 3), dtype=np.uint8)
-    pred.set_image(img)
-    pts = np.stack([rng.uniform(0, 420, 12), rng.uniform(0, 300, 12)], 1)
-    lab = rng.integers(0, 2, 12)
-    box = np.array([40.0, 30.0, 380.0, 260.0])
-    low = pred.predict(point_coords=pts[:1], point_labels=lab[:1], multimask_output=False)[2]
-    prompts = [dict(point_coords=pts[:3], point_labels=lab[:3]), dict(box=box), dict(box=box, point_coords=pts[:2], point_labels=lab[:2]),
-               dict(point_coords=pts[:1], point_labels=lab[:1], mask_input=low), dict(mask_input=low),
-               dict(point_coords=pts, point_labels=lab)]
-
-    def run():
-        for kw in prompts:
-            for mm in (True, False):
-                for logits in (True, False):
-                    pred.predict(multimask_output=mm, return_logits=logits, **kw)
-        S = seg.image_size
-        dev = next(seg.parameters()).device
-        seg.set_image_batch(torch.randn(2, 3, S, S, generator=torch.Generator().manual_seed(1)).to(dev))
-        c = torch.rand(2, 11, 2, generator=torch.Generator().manual_seed(2)) * S
-        lb = torch.ones(2, 11, dtype=torch.int32)
-        for mm in (True, False):
-            for logits in (True, False):
-                seg.predict_batch(c.to(dev), lb.to(dev), multimask_output=mm, return_logits=logits)
-    return record_calls(monkeypatch, run)
-
-
-def _closure(calls, who):
-    reached = {k for k in (route_key(n, a) for n, a in calls) if k is not None}
-    missing = reached - covered_keys()
-    print(f"\n{who}: {len(reached)} SAM-head route keys reached: {sorted(reached, key=repr)}", end="")
-    assert not missing, f"{who} reaches SAM-head routes no table row runs: {sorted(missing, key=repr)}"
-    return reached
-
-
-@pytest.mark.parametrize("kind", ["vit", "student"])
-def test_route_closure_predictor(cuda, monkeypatch, kind):
-    """SAM3InteractiveImagePredictor and Sam3PointPromptSegmenter.predict_batch (object-gated) on the ViT override and the EV-B1
-    student: points, box, box + points, point + mask, mask only, 12 points; multimask and return_logits on and off."""
-    reached = _closure(_predictor_calls(_seg(kind, cuda), monkeypatch), f"predictor {kind}")
-    assert ("attn_few_keys", False, True) in reached                   # 12 points + 6 output tokens + the pad point: two tiles
-    assert ("hyper_masks", True, 3, 1) in reached and ("bilinear", False, True) in reached
-
-
-def test_route_closure_strict(cuda, monkeypatch):
-    from efficientsam3_b200 import ops
-    seg = _seg("student", cuda)
-    with ops.strict_precision():
-        reached = _closure(_predictor_calls(seg, monkeypatch), "predictor strict")
-    assert ("attn_few_keys", True, True) in reached and any(k[0] == "ln_rows_gelu" and k[1] for k in reached)
-
-
-def test_route_closure_module_api(cuda, monkeypatch):
-    """PromptEncoder / MaskDecoder / TwoWayTransformer as test_decoder_gpu builds them: points, boxes and a mask prompt."""
-    from es3_recorder import record_calls
-    from helpers import load_golden, sd_from_keys
-    from test_decoder_gpu import _build
-    g = load_golden("sam_heads_16")
-    E, S, B = 16, 224, 2
-    pe, md = _build(E, S, sd_from_keys(g["keys_pe"], 5), sd_from_keys(g["keys_md"], 6), cuda)
-    gen = torch.Generator().manual_seed(4)
-    feat = torch.randn(B, 256, E, E, generator=gen).to(cuda)
-    hr = [torch.randn(B, 32, 4 * E, 4 * E, generator=gen).to(cuda), torch.randn(B, 64, 2 * E, 2 * E, generator=gen).to(cuda)]
-    coords = (torch.rand(B, 3, 2, generator=gen) * S).to(cuda)
-    labels = torch.ones(B, 3, dtype=torch.int32, device=cuda)
-    boxes = torch.tensor([[10.0, 20.0, 100.0, 200.0]] * B, device=cuda)
-    masks = torch.randn(B, 1, 4 * E, 4 * E, generator=gen).to(cuda)
-
-    def run():
-        for kw in (dict(points=(coords, labels), boxes=None, masks=None), dict(points=None, boxes=boxes, masks=masks),
-                   dict(points=(coords, labels), boxes=boxes, masks=None)):
-            sp, de = pe(**kw)
-            for mm in (True, False):
-                md(image_embeddings=feat, image_pe=pe.get_dense_pe(), sparse_prompt_embeddings=sp, dense_prompt_embeddings=de,
-                   multimask_output=mm, repeat_image=False, high_res_features=hr)
-    _closure(record_calls(monkeypatch, run), "module API")

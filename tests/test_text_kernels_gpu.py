@@ -6,9 +6,8 @@ Outputs and workspaces are NaN-prefilled and called through _lib.call: every cel
 within its bound, every cell past it (a flat TAIL) keeps its sentinel bits.  Accumulating outputs (dgamma, dbeta, the embedding
 and positional gradients, consistency's dp and loss) are prefilled with random values and checked as +=.  Every fixed-order
 reduction runs twice and must be bit-identical; a sequence run alone must be bit-identical to the same sequence inside a batch; a
-shape an entry point declines writes nothing; the ops wrappers are bit-identical to the direct calls.  A route-closure test records
-the text kernels the native text students' training steps and the SAM3 text teacher's eval forward reach and asserts that some table
-row runs each of them.
+shape an entry point declines writes nothing; the ops wrappers are bit-identical to the direct calls.  covered_keys() names the
+route keys (tests/routes.py) the tables run, for the route closure of tests/test_route_closure_gpu.py.
 
 GAMMA = 2 (ref_train_bwd.GAMMA) holds without change.  Worst err/bound per section in one run on an H100 80GB HBM3 (700 W power
 limit): bf16 outputs -- attention 0.995 (mma.sync) and 0.934 (wgmma), attention backward 0.994, LayerNorm 0.995, RepMixer u 0.994,
@@ -16,113 +15,23 @@ RepMixer backward dy 0.996, where the output's own rounding half-step dominates 
 0.065 (dgamma), 0.125 (dbeta), RepMixer x1 0.169, embedding gradient 0.186, positional gradient 0.099, positional resize 0.991
 (its bound is its own two roundings), RepMixer backward 0.681 (tm dx), 0.197 (ffn e), <= 0.085 (the accumulated gradients), KD
 partials 0.038, out3 0.017, dp 0.143, consistency 0.2 at most.  The whole file (226 tests, the route-closure training steps
-included) took 29 s there.
+included, since moved to tests/test_route_closure_gpu.py) took 29 s there.
 """
+import zlib
+
 import pytest
 import torch
 
 import ref_text as R
-from es3_recorder import TEXT_ROUTES, text_step_calls, text_teacher_calls
-from bounds import TAIL, _INT, _assert_untouched, _bf, _check, _flat_out, _gen, _pairwise, report_worst
+from bounds import (TAIL, _assert_untouched, _bf, _bits_equal, _check, _declined, _flat_out, _gen, _lib, _p, _pairwise,
+                    _prefilled, _qkv, _st, _twice, report_worst)
+from routes import attn_key, causal_attn_key
 
 pytestmark = pytest.mark.gpu
 _report_worst = report_worst("text kernels")
 
 
-def _st():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _p(t):
-    return 0 if t is None else t.data_ptr()
-
-
-def _lib(cuda):
-    from efficientsam3_b200 import _lib
-    _lib.init(cuda.index or 0)
-    return _lib
-
-
-def _twice(run, buf):
-    """run(buffer) on two copies of the prefilled buffer; both must be bit-identical.  Returns the first."""
-    a, b = buf.clone(), buf.clone()
-    run(a)
-    run(b)
-    assert torch.equal(a.view(_INT[a.dtype]), b.view(_INT[b.dtype])), "two runs differ"
-    return a
-
-
-def _bits_equal(a, b, what):
-    assert torch.equal(a.contiguous().view(_INT[a.dtype]), b.contiguous().view(_INT[b.dtype])), what
-
-
-def _prefilled(n, cuda, g):
-    """A flat fp32 buffer of n + TAIL cells: n random values (an accumulating output's prior contents), then NaN sentinels."""
-    buf, inside = _flat_out(n, torch.float32, cuda)
-    buf[:n] = torch.randn(n, device=cuda, generator=g)
-    return buf, inside
-
-
-def _declined(lib, name, args, bufs, what):
-    """A shape `name` declines: the call raises and every buffer keeps its bits."""
-    from efficientsam3_b200._lib import Es3Error
-    before = [b.clone() for b in bufs]
-    with pytest.raises(Es3Error):
-        lib.call(name, *args)
-    torch.cuda.synchronize()
-    for b, b0 in zip(bufs, before):
-        _bits_equal(b, b0, f"{what}: a declined call wrote")
-
-
-# ----------------------------------------------------------------------------------------------------------- route keys
-def attn_key(L, causal):
-    if causal:
-        return ("attention_mma", 2 if L >= 128 else 1, True)
-    return ("attention_tc", None, False) if L >= 128 else ("attention_mma", 1, False)
-
-
-def route_key(name, a):
-    """Route key of one recorded es3_* call (None: not a kernel of this file)."""
-    if name == "es3_attention_causal_bf16":
-        return attn_key(a[3], True)
-    if name == "es3_attention_bf16":
-        L = a[7] * a[7] if a[7] else a[3] * a[4]
-        return attn_key(L, False) if a[7] == 0 else None
-    if name == "es3_text_attn_bwd":
-        return ("text_attn_bwd", bool(a[8]))
-    if name == "es3_layernorm_f32":
-        return ("layernorm_f32", a[11] // 128)
-    if name == "es3_layernorm_bwd_f32":
-        return ("layernorm_bwd_f32", a[3] not in (None, 0), a[6] not in (None, 0), a[7] > 37888)
-    if name == "es3_text_pos_resize":
-        return ("pos_resize",)
-    if name == "es3_text_pos_grad":
-        return ("pos_grad", a[2] == a[3])
-    if name in ("es3_text_kd_loss_fwd", "es3_text_kd_loss_bwd"):
-        key = ("kd_loss_fwd" if name.endswith("fwd") else "kd_loss_bwd", a[2] not in (None, 0))
-        return key + ((a[9] not in (None, 0), a[10] not in (None, 0)) if name.endswith("bwd") else ())
-    if name == "es3_text_consistency_bwd":
-        return ("consistency_bwd", a[6] not in (None, 0), a[7] not in (None, 0))
-    simple = {"es3_text_embed": "text_embed", "es3_repmixer_bf16": "repmixer", "es3_text_embed_grad": "embed_grad",
-              "es3_text_consistency_fwd": "consistency_fwd", "es3_cast_f32_to_bf16": "cast_bf16", "es3_cast_f32_to_f16": "cast_f16",
-              "es3_repmixer_ls_bwd": "repmixer_ls_bwd", "es3_repmixer_ffn_bwd": "repmixer_ffn_bwd", "es3_repmixer_tm_bwd": "repmixer_tm_bwd"}
-    return (simple[name],) if name in simple else None
-
-
 # ----------------------------------------------------------------------------------------------------------- (1) attention
-def _qkv(cuda, B, L, heads, kind, g):
-    C = 64 * heads
-    x = torch.randn(B * L, 3 * C, device=cuda, generator=g) * 1.5
-    if kind == "peaked":                                   # scores spread by ~100: near one-hot rows
-        x[:, :2 * C] *= 5
-    elif kind == "flat":                                   # q = 0: every score 0, p = 1
-        x[:, :C] = 0
-    elif kind == "tied":                                   # keys repeat with period 5: tied maxima in every row, across KV tiles
-        k = x[:, C:2 * C].view(B, L, C)
-        x[:, C:2 * C] = k[:, torch.arange(L, device=cuda) % 5].reshape(B * L, C)
-    return _bf(x)
-
-
 ATTN = _pairwise(dict(L=[1, 2, 15, 16, 17, 31, 32, 33, 63, 64, 65, 77, 127, 128], heads=[1, 8, 12, 16], B=[1, 3, 64],
                       kind=["normal", "peaked", "flat", "tied"], causal=[True, False]), seed=11)
 ATTN_SCALE = 64 ** -0.5
@@ -153,7 +62,7 @@ def test_attention_fwd_bwd(cuda, L, heads, B, kind, causal):
     buf, inside = _flat_out(B * L * C, torch.bfloat16, cuda)
     got = _twice(lambda o: _attn_fwd(lib, qkv, o, B, L, C, heads, causal), buf)
     o = got[:B * L * C].view(B * L, C)
-    kernel = "tc" if attn_key(L, causal)[0] == "attention_tc" else "mma"
+    kernel = "mma" if causal else attn_key("es3_attention_bf16", 1, L, 0)[1]
     ref, bound = R.attention(qkv.double(), B, L, heads, ATTN_SCALE, causal, kernel)
     what = f"attention {kernel} causal={causal} L{L} heads{heads} B{B} {kind}"
     _check(f"1 attention {kernel} causal={causal}", o, ref, bound, what)
@@ -518,7 +427,7 @@ V_TEXT = 49408
 
 def _ids(kind, cuda):
     """[B, L] int64 ids (CPU) with the structure `kind` names."""
-    g = torch.Generator().manual_seed(hash(kind) % 2 ** 31)
+    g = torch.Generator().manual_seed(zlib.crc32(kind.encode()))
     if kind == "chunk_edges":                  # ids with exactly 31, 32, 33, 64, 65 tokens, and some singletons
         ids = torch.cat([torch.full((n,), i + 1) for i, n in enumerate((31, 32, 33, 64, 65))] + [torch.arange(100, 125)])
         ids = ids[torch.randperm(ids.numel(), generator=g)]
@@ -805,55 +714,17 @@ def test_casts_bit_exact(cuda, n):
 
 
 # ----------------------------------------------------------------------------------------------------------- route closure
-# Kernels the text routes reach that other files hold to their bounds: the GEMMs (tests/test_gemm_epilogue_gpu.py); the batch-
-# statistics RepMixerBlock kernels of S0 (tests/test_syncbn_repmixer_gpu.py).  The bias / GELU epilogues, their backward,
-# the column sums and the weight gradients are train_bwd.cu's: each key the text routes reach must be a covered key of
-# tests/test_train_bwd_gpu.py.
-EXCLUDED = {"es3_gemm_bf16", "es3_gemm_bf16_ex", "es3_repmixer_bn_fwd", "es3_repmixer_bn_ffn_bwd", "es3_repmixer_bn_tm_bwd"}
-TRAIN_BWD = {"es3_wgrad_pw", "es3_wgrad_tc", "es3_colsum_f32", "es3_affine_act", "es3_bn_act_bwd_reduce", "es3_bn_act_bwd_apply"}
-
-
-def _closure(calls, who):
-    import test_train_bwd_gpu as TB
-    reached = {k for k in (route_key(n, a) for n, a in calls) if k is not None}
-    missing = reached - covered_keys()
-    bwd = {TB.route_key(n, a) for n, a in calls if n in TRAIN_BWD}
-    unknown = {n for n, a in calls if route_key(n, a) is None} - EXCLUDED - TRAIN_BWD - {"es3_init"}   # es3_init: device check
-    print(f"\n{who}: {len(reached)} text route keys reached: {sorted(reached, key=repr)}", end="")
-    assert not missing, f"{who} reaches text routes no table row runs: {sorted(missing, key=repr)}"
-    assert not bwd - TB.covered_keys(), f"{who} reaches train_bwd.cu routes no table row runs: {sorted(bwd - TB.covered_keys(), key=repr)}"
-    assert not unknown, f"{who} reaches kernels neither this file nor another's table accounts for: {sorted(unknown)}"
-    return reached
-
-
 def covered_keys():
-    """Every route key some table row above runs, computed from the tables with the key functions route_key uses."""
-    keys = {attn_key(c[0], c[4]) for c in ATTN} | {("text_attn_bwd", c[4]) for c in ATTN}
-    keys |= {("layernorm_f32", c[0] // 128) for c in LNF}
-    keys |= {("layernorm_bwd_f32", c[2], c[3], c[1] > 37888) for c in LNB}
-    keys |= {("repmixer",) for _ in REPMIXER} | {(k,) for _ in RMB for k in ("repmixer_ls_bwd", "repmixer_ffn_bwd", "repmixer_tm_bwd")}
-    keys |= {("pos_resize",) for N, L, _ in POS if N != L} | {("pos_grad", N == L) for N, L, _ in POS}
-    keys |= {("embed_grad",) for _ in EMBED_GRAD}
-    keys |= {("kd_loss_fwd", c[2]) for c in KD} | {("kd_loss_bwd", c[2], c[3], c[4]) for c in KD}
-    keys |= {("consistency_fwd",) for _ in CON} | {("consistency_bwd", c[3], c[4]) for c in CON}
-    keys |= {("text_embed",) for _ in EMB} | {k for _ in CASTS for k in (("cast_bf16",), ("cast_f16",))}
+    """Every route key (tests/routes.py) some table row above runs."""
+    keys = {causal_attn_key(c[0]) if c[4] else attn_key("es3_attention_bf16", 1, c[0], 0) for c in ATTN}
+    keys |= {("es3_text_attn_bwd", c[4]) for c in ATTN}
+    keys |= {("es3_layernorm_f32", c[0] // 128) for c in LNF}
+    keys |= {("es3_layernorm_bwd_f32", c[2], c[3], c[1] > 37888) for c in LNB}
+    keys |= {("es3_repmixer_bf16",) for _ in REPMIXER}
+    keys |= {(k,) for _ in RMB for k in ("es3_repmixer_ls_bwd", "es3_repmixer_ffn_bwd", "es3_repmixer_tm_bwd")}
+    keys |= {("es3_text_pos_resize",) for N, L, _ in POS if N != L} | {("es3_text_pos_grad", N == L) for N, L, _ in POS}
+    keys |= {("es3_text_embed_grad",) for _ in EMBED_GRAD}
+    keys |= {("es3_text_kd_loss_fwd", c[2]) for c in KD} | {("es3_text_kd_loss_bwd", c[2], c[3], c[4]) for c in KD}
+    keys |= {("es3_text_consistency_fwd",) for _ in CON} | {("es3_text_consistency_bwd", c[3], c[4]) for c in CON}
+    keys |= {("es3_text_embed",) for _ in EMB} | {k for _ in CASTS for k in (("es3_cast_f32_to_bf16",), ("es3_cast_f32_to_f16",))}
     return keys
-
-
-@pytest.mark.parametrize("route", TEXT_ROUTES, ids=[r[0] for r in TEXT_ROUTES])
-def test_route_closure(cuda, monkeypatch, route):
-    """Every text-kernel route the native training steps of es3_recorder.TEXT_ROUTES reach is run by some table row above: S0 with
-    frozen BN, S1, B, S3 at contexts 32, 77 and 128, the 77-entry table at 32 and at 128, masked and plain loss with consistency,
-    and a batch of 512 x 77 tokens (LayerNorm backward over more than 592 x 64 rows)."""
-    reached = _closure(text_step_calls(cuda, monkeypatch, *route[1:]), route[0])
-    if route[1] == "MobileCLIP-S0":
-        assert {("repmixer",), ("repmixer_tm_bwd",)} <= reached
-    if route[0] == "B ctx 128":
-        assert ("attention_mma", 2, True) in reached
-    if route[0] == "S3 batch 512":
-        assert any(k[0] == "layernorm_bwd_f32" and k[3] for k in reached if len(k) == 4)
-
-
-def test_route_closure_sam3_teacher(cuda, monkeypatch):
-    """The SAM3 text teacher's eval forward (width 1024, 16 heads, causal)."""
-    assert ("attention_mma", 1, True) in _closure(text_teacher_calls(cuda, monkeypatch), "SAM3 text teacher")

@@ -29,7 +29,8 @@ GAMMA = 2 was set from one run on an H100 80GB HBM3 (700 W power limit).  Worst 
 (10) layernorm_bwd dgamma 0.089, dbeta 0.003, window dS 0.007, colsum 0.18.  bf16 outputs: 0.95 ... 0.996 in every section
 (dw_bwd_data, affine_act, bn_act_bwd dz, se_apply, litemla_bwd, layernorm_bwd dx, window dqkv), because the half-step of the
 output rounding dominates their bound and is reached; bilinear_bwd 0.66.  The whole file (359 tests, the route-closure training
-steps included) took 22 s there.
+steps included, since moved to tests/test_route_closure_gpu.py) took 22 s there.  covered_keys() names the route keys
+(tests/routes.py) the tables run.
 """
 import math
 
@@ -38,27 +39,13 @@ import torch
 import torch.nn.functional as F
 
 import ref_train_bwd as R
-from es3_recorder import STUDENTS, training_step_calls
-from bounds import (_INT, TAIL, _assert_untouched, _bf, _check, _flat_out, _gen, _pairwise, _sentinel, report_worst)
+from bounds import _INT, TAIL, _assert_untouched, _bf, _check, _flat_out, _gen, _lib, _p, _pairwise, _sentinel, _st, report_worst
+from routes import key_dw_bwd_data, key_wgrad_pw, key_wgrad_tc
 
 pytestmark = pytest.mark.gpu
 _report_worst = report_worst("train bwd")
 ACT_CODE = {None: 0, "relu": 1, "hswish": 2, "gelu": 3}
 BN_MODE = {"none": 0, "eval": 1, "batch": 2}
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _ptr(t):
-    return 0 if t is None else t.data_ptr()
-
-
-def _lib(cuda):
-    from efficientsam3_b200 import _lib
-    _lib.init(cuda.index or 0)
-    return _lib
 
 
 def _nan_ws(lib, name, *args, cuda):
@@ -105,58 +92,6 @@ def _strided_out(rows, cols, ld, dtype, cuda, fill=None):
     return buf, inside, idx
 
 
-# ----------------------------------------------------------------------------------------------------------- route keys
-def wg_pick(c):
-    return 1 if c <= 16 else (2 if c <= 32 else 4)
-
-
-def key_wgrad_pw(N, K, shifted):
-    return ("wgrad_pw", wg_pick(N), wg_pick(K), "shift" if shifted else "plain")
-
-
-def key_wgrad_tc(K):
-    return ("wgrad_tc", 128 if K >= 128 else 64)
-
-
-def key_dw_bwd_data(ks, stride):
-    return ("dw_bwd_data", "s2k3" if (ks, stride) == (3, 2) else "generic", ks, stride)
-
-
-def key_dw_wgrad(impl, ks, stride):
-    return ("dwconv_wgrad", impl, ks, stride)
-
-
-def route_key(name, a):
-    """Route key of one recorded es3_* call: the kernel instantiation its arguments select (None: not a backward kernel)."""
-    act = {v: k for k, v in ACT_CODE.items()}
-    if name == "es3_wgrad_pw":
-        return key_wgrad_pw(a[5], a[6], a[7] > 0)
-    if name == "es3_wgrad_tc":
-        return key_wgrad_tc(a[6])
-    if name == "es3_dwconv_bwd_data":
-        return key_dw_bwd_data(a[7], a[8])
-    if name in ("es3_dwconv_wgrad", "es3_dwconv_wgrad_win"):
-        return key_dw_wgrad("win" if name.endswith("win") else "direct", a[7], a[8])
-    if name == "es3_bn_act_bwd_reduce":
-        return ("bn_act_bwd", act[a[4]], {v: k for k, v in BN_MODE.items()}[a[5]], a[2] != 0)
-    if name == "es3_bn_act_bwd_apply":
-        return ("bn_act_bwd_apply", act[a[4]], a[2] != 0)
-    if name == "es3_affine_act":
-        return ("affine_act", act[a[3]], a[1] != 0, a[4] != 0)
-    if name == "es3_stem_wgrad":
-        return ("stem_wgrad", a[5])
-    if name == "es3_litemla_attn_bwd_generic":
-        return ("litemla_bwd_generic", a[12])
-    if name == "es3_layernorm_bwd":
-        return ("layernorm_bwd", a[3] != 0)
-    if name == "es3_win_attn_bias_bwd":
-        return ("win_attn_bias_bwd", a[11])
-    simple = {"es3_bn_stats": "bn_stats", "es3_add_bf16": "add_bf16", "es3_se_bwd_dgate": "se_dgate", "es3_se_bwd_apply": "se_apply",
-              "es3_bilinear_bwd": "bilinear_bwd", "es3_litemla_attn_bwd": "litemla_bwd", "es3_colsum_f32": "colsum",
-              "es3_transpose_pad_bf16": "transpose_pad", "es3_accumulate_strided": "accumulate_strided"}
-    return (simple[name],) if name in simple else None
-
-
 # ----------------------------------------------------------------------------------------------------------- (1) es3_wgrad_pw
 def _wgrad_pw_run(cuda, dz, x, M, N, K, ldn, ldk, shift, dW_fill_idx, buf):
     lib = _lib(cuda)
@@ -166,7 +101,7 @@ def _wgrad_pw_run(cuda, dz, x, M, N, K, ldn, ldk, shift, dW_fill_idx, buf):
     def run(bufs):
         ws.fill_(float("nan"))
         lib.call("es3_wgrad_pw", dz.data_ptr(), dz.stride(0), x.data_ptr(), x.stride(0), M, N, K, H, W, dy, dx, ws.data_ptr(),
-                 bufs[0].data_ptr(), ldn, ldk, _stream())
+                 bufs[0].data_ptr(), ldn, ldk, _st())
     return _twice(run, buf)[0]
 
 
@@ -217,7 +152,7 @@ def _tap_case(cuda, dz2, xs, N, C, ky, kx, shift, ref_tap, bound_tap, what):
     def run(bufs):
         ws.fill_(float("nan"))
         lib.call("es3_wgrad_pw", dz2.data_ptr(), dz2.stride(0), xs.data_ptr(), xs.stride(0), M, N, C, *shift, ws.data_ptr(),
-                 bufs[0].data_ptr() + 4 * t, 9 * C, 9, _stream())
+                 bufs[0].data_ptr() + 4 * t, 9 * C, 9, _st())
     got = _twice(run, buf)[0]
     _check("1 wgrad_pw taps", got[idx].view(N, C), dW0.double() + ref_tap, bound_tap + 4 * R.U * dW0.double().abs(), what)
     _assert_untouched(got, inside, what)
@@ -297,7 +232,7 @@ def test_wgrad_tc(cuda, monkeypatch, nan_ws, K, N, M, strided, wide):
     def run(bufs):
         ws.fill_(float("nan"))
         assert lib.call_rc("es3_wgrad_tc", dz.data_ptr(), dz.stride(0), x.data_ptr(), x.stride(0), M, N, K, ws.data_ptr(),
-                           bufs[0].data_ptr(), ldn, _stream()) == 0
+                           bufs[0].data_ptr(), ldn, _st()) == 0
     got = _twice(run, buf)[0]
     ref, bound = R.wgrad(dz.double(), x.double(), dW0.double())
     what = f"wgrad_tc M{M} N{N} K{K} strided={strided} ldn={ldn}"
@@ -317,7 +252,7 @@ def test_wgrad_tc_declines_63_rows(cuda, monkeypatch, nan_ws):
     dz, x = _bf(torch.randn(M, N, device=cuda, generator=g)), _bf(torch.randn(M, K, device=cuda, generator=g))
     ws = _nan_ws(lib, "es3_wgrad_tc_ws_floats", M, N, K, cuda=cuda)
     dW = torch.zeros(N, K, device=cuda)
-    assert lib.call_rc("es3_wgrad_tc", dz.data_ptr(), N, x.data_ptr(), K, M, N, K, ws.data_ptr(), dW.data_ptr(), K, _stream()) == -1
+    assert lib.call_rc("es3_wgrad_tc", dz.data_ptr(), N, x.data_ptr(), K, M, N, K, ws.data_ptr(), dW.data_ptr(), K, _st()) == -1
     names = []
     real_call, real_rc = L.call, L.call_rc
     monkeypatch.setattr(L, "call", lambda n, *a: (names.append(n), real_call(n, *a))[1])
@@ -367,7 +302,7 @@ def _dw_bwd_data(cuda, dz, w, H, W, ks, stride, what):
     lib = _lib(cuda)
     B, Ho, Wo, C = dz.shape
     buf, inside = _flat_out(B * H * W * C, torch.bfloat16, cuda)
-    lib.call("es3_dwconv_bwd_data", dz.data_ptr(), w.data_ptr(), buf.data_ptr(), B, H, W, C, ks, stride, _stream())
+    lib.call("es3_dwconv_bwd_data", dz.data_ptr(), w.data_ptr(), buf.data_ptr(), B, H, W, C, ks, stride, _st())
     ref, bound = R.dwconv_bwd_data(dz.double(), w.double(), H, W, ks, stride)
     _check("4 dw_bwd_data", buf[:B * H * W * C].view(B, H, W, C), ref, bound, what)
     _assert_untouched(buf, inside, what)
@@ -443,7 +378,7 @@ def _dw_wgrad(cuda, name, B, H, W, C, ks, stride, sliced, seed=()):
 
     def run(bufs):
         ws.fill_(float("nan"))
-        lib.call(name, dz.data_ptr(), x.data_ptr(), x.stride(2), B, H, W, C, ks, stride, ws.data_ptr(), bufs[0].data_ptr(), _stream())
+        lib.call(name, dz.data_ptr(), x.data_ptr(), x.stride(2), B, H, W, C, ks, stride, ws.data_ptr(), bufs[0].data_ptr(), _st())
     got = _twice(run, buf)[0]
     ref, bound = R.dwconv_wgrad(dz.double(), x.double(), dW0.double(), ks, stride)
     what = f"{name} B{B} {H}x{W} C{C} k{ks}s{stride} sliced={sliced}"
@@ -524,7 +459,7 @@ def test_bn_stats(cuda, M, C):
     ws = _nan_ws(lib, "es3_col_reduce_ws_floats", M, C, cuda=cuda)
     lib.call("es3_bn_stats", z.data_ptr(), M, C, 1e-5, 0.1, gamma.data_ptr(), beta.data_ptr(), ws.data_ptr(),
              *(outs[k][0].data_ptr() for k in ("mean", "invstd", "scale", "shift")), run_bufs["running_mean"][0].data_ptr(),
-             run_bufs["running_var"][0].data_ptr(), nbt.data_ptr(), _stream())
+             run_bufs["running_var"][0].data_ptr(), nbt.data_ptr(), _st())
     assert int(nbt) == 8
     ref = R.bn_stats(z.double(), gamma.double(), beta.double(), 1e-5, 0.1, rm0.double(), rv0.double())
     for k, (r, b) in ref.items():
@@ -560,7 +495,7 @@ def test_affine_act(cuda, act, C, M, has_scale, res, has_shift):
     shift = torch.randn(C, device=cuda, generator=g) if has_shift else None
     r = _bf(torch.randn(M, C, device=cuda, generator=g)) if res else None
     buf, inside = _flat_out(M * C, torch.bfloat16, cuda)
-    lib.call("es3_affine_act", z.data_ptr(), _ptr(scale), _ptr(shift), ACT_CODE[act], _ptr(r), buf.data_ptr(), M, C, _stream())
+    lib.call("es3_affine_act", z.data_ptr(), _p(scale), _p(shift), ACT_CODE[act], _p(r), buf.data_ptr(), M, C, _st())
     d = lambda t: None if t is None else t.double()
     ref, bound = R.affine_act(z.double(), d(scale), d(shift), act, d(r))
     what = f"affine_act {act} M{M} C{C} scale={has_scale} res={res} shift={has_shift}"
@@ -626,14 +561,14 @@ def test_bn_act_bwd(cuda, mode, act, C, M, has_scale):
 
     def run(bufs):
         ws.fill_(float("nan"))
-        lib.call("es3_bn_act_bwd_reduce", da.data_ptr(), z.data_ptr(), _ptr(scale), _ptr(shift), ACT_CODE[act], BN_MODE[mode],
-                 _ptr(mean), _ptr(invstd), M, C, ws.data_ptr(), bufs[0].data_ptr(), bufs[1].data_ptr() if mode != "none" else 0,
-                 bufs[2].data_ptr(), _stream())
+        lib.call("es3_bn_act_bwd_reduce", da.data_ptr(), z.data_ptr(), _p(scale), _p(shift), ACT_CODE[act], BN_MODE[mode],
+                 _p(mean), _p(invstd), M, C, ws.data_ptr(), bufs[0].data_ptr(), bufs[1].data_ptr() if mode != "none" else 0,
+                 bufs[2].data_ptr(), _st())
     coef, dgb, dbb = _twice(run, coef, red[0][0], red[1][0])
     _assert_untouched(coef, cins, "coef")
     dz, dzins = _flat_out(M * C, torch.bfloat16, cuda)
-    lib.call("es3_bn_act_bwd_apply", da.data_ptr(), z.data_ptr(), _ptr(scale), _ptr(shift), ACT_CODE[act], coef.data_ptr(),
-             dz.data_ptr(), M, C, _stream())
+    lib.call("es3_bn_act_bwd_apply", da.data_ptr(), z.data_ptr(), _p(scale), _p(shift), ACT_CODE[act], coef.data_ptr(),
+             dz.data_ptr(), M, C, _st())
     d = lambda t: None if t is None else t.double()
     ref = R.bn_act_bwd(da.double(), z.double(), d(scale), d(shift), act, mode, d(mean), d(invstd), dg0.double(), db0.double())
     what = f"bn_act_bwd {mode} {act} M{M} C{C} scale={has_scale}"
@@ -661,7 +596,7 @@ def test_add_bf16_bit_exact(cuda, M, C, lda, ldb, ldo):
     Bm[:, :C] = _bf(torch.randn(M, C, device=cuda, generator=g))
     a, b = A[:, lda - C:], Bm[:, :C]
     buf, inside, idx = _strided_out(M, C, ldo, torch.bfloat16, cuda)
-    lib.call("es3_add_bf16", a.data_ptr(), lda, b.data_ptr(), ldb, buf.data_ptr(), ldo, M, C, _stream())
+    lib.call("es3_add_bf16", a.data_ptr(), lda, b.data_ptr(), ldb, buf.data_ptr(), ldo, M, C, _st())
     assert torch.equal(buf[idx].view(M, C).view(torch.int16), (a + b).view(torch.int16))
     _assert_untouched(buf, inside, "add_bf16")
 
@@ -678,14 +613,14 @@ def _se_case(cuda, B, HW, C):
 
     def run(bufs):
         ws.fill_(float("nan"))
-        lib.call("es3_se_bwd_dgate", dy.data_ptr(), x.data_ptr(), B, HW, C, ws.data_ptr(), bufs[0].data_ptr(), _stream())
+        lib.call("es3_se_bwd_dgate", dy.data_ptr(), x.data_ptr(), B, HW, C, ws.data_ptr(), bufs[0].data_ptr(), _st())
     got = _twice(run, buf)[0]
     ref, bound = R.se_dgate(dy.double(), x.double(), dg0.double())
     _check("7 se_dgate", got[:B * C].view(B, C), ref, bound, f"se_dgate B{B} HW{HW} C{C}")
     _assert_untouched(got, inside, "se_dgate")
     gate, add = torch.rand(B, C, device=cuda, generator=g), torch.randn(B, C, device=cuda, generator=g) * 0.1
     out, oins = _flat_out(B * HW * C, torch.bfloat16, cuda)
-    lib.call("es3_se_bwd_apply", dy.data_ptr(), gate.data_ptr(), add.data_ptr(), out.data_ptr(), B, HW, C, _stream())
+    lib.call("es3_se_bwd_apply", dy.data_ptr(), gate.data_ptr(), add.data_ptr(), out.data_ptr(), B, HW, C, _st())
     ref, bound = R.se_apply(dy.double(), gate.double(), add.double())
     _check("7 se_apply", out[:B * HW * C].view(B, HW, C), ref, bound, f"se_apply B{B} HW{HW} C{C}")
     _assert_untouched(out, oins, "se_apply")
@@ -722,7 +657,7 @@ def test_stem_wgrad(cuda, B, ci, Cout, H, W):
 
     def run(bufs):
         ws.fill_(float("nan"))
-        lib.call("es3_stem_wgrad", img.data_ptr(), dz.data_ptr(), B, H, W, Cout, ws.data_ptr(), bufs[0].data_ptr(), _stream())
+        lib.call("es3_stem_wgrad", img.data_ptr(), dz.data_ptr(), B, H, W, Cout, ws.data_ptr(), bufs[0].data_ptr(), _st())
     got = _twice(run, buf)[0]
     ref, bound = R.stem_wgrad(img.double(), dz.double(), dW0.double())
     what = f"stem_wgrad B{B} {H}x{W} Cout{Cout}"
@@ -756,7 +691,7 @@ def test_bilinear_bwd(cuda, B, C, Hi, Wi, Ho, Wo):
     lib = _lib(cuda)
     dout = torch.randn(B, C, Ho, Wo, device=cuda, generator=_gen(cuda, "bil", B, C, Hi, Wi, Ho, Wo))
     buf, inside = _flat_out(B * Hi * Wi * C, torch.bfloat16, cuda)
-    lib.call("es3_bilinear_bwd", dout.data_ptr(), buf.data_ptr(), B, Hi, Wi, C, Ho, Wo, _stream())
+    lib.call("es3_bilinear_bwd", dout.data_ptr(), buf.data_ptr(), B, Hi, Wi, C, Ho, Wo, _st())
     ref, bound = R.bilinear_bwd(dout.double(), Hi, Wi)
     what = f"bilinear_bwd B{B} C{C} {Hi}x{Wi} <- {Ho}x{Wo}"
     _check("8 bilinear_bwd", buf[:B * Hi * Wi * C].view(B, Hi, Wi, C), ref, bound, what)
@@ -784,11 +719,11 @@ def _litemla(cuda, B, HW, heads2, dim, generic, pad, seed=()):
     if generic:
         ws = _nan_ws(lib, "es3_litemla_bwd_generic_ws_floats", B, HW, heads2, dim, cuda=cuda)
         args = ("es3_litemla_attn_bwd_generic", msp.data_ptr(), msp.stride(0), dyp.data_ptr(), dyp.stride(0), kv.data_ptr(),
-                nchunk_f, ws.data_ptr(), buf.data_ptr(), ld + pad, B, HW, heads2, dim, 1e-15, _stream())
+                nchunk_f, ws.data_ptr(), buf.data_ptr(), ld + pad, B, HW, heads2, dim, 1e-15, _st())
     else:
         ws = _nan_ws(lib, "es3_litemla_bwd_ws_floats", B, HW, heads2, cuda=cuda)
         args = ("es3_litemla_attn_bwd", msp.data_ptr(), msp.stride(0), dyp.data_ptr(), dyp.stride(0), kv.data_ptr(), nchunk_f,
-                ws.data_ptr(), buf.data_ptr(), ld + pad, B, HW, heads2, 1e-15, _stream())
+                ws.data_ptr(), buf.data_ptr(), ld + pad, B, HW, heads2, 1e-15, _st())
 
     def run(bufs):
         ws.fill_(float("nan"))
@@ -851,8 +786,8 @@ def test_layernorm_bwd(cuda, C, M, dres):
 
     def run(bufs):
         ws.fill_(float("nan"))
-        lib.call("es3_layernorm_bwd", x.data_ptr(), dy.data_ptr(), gamma.data_ptr(), _ptr(r), 1e-5, bufs[0].data_ptr(), M, C,
-                 ws.data_ptr(), bufs[1].data_ptr(), bufs[2].data_ptr(), _stream())
+        lib.call("es3_layernorm_bwd", x.data_ptr(), dy.data_ptr(), gamma.data_ptr(), _p(r), 1e-5, bufs[0].data_ptr(), M, C,
+                 ws.data_ptr(), bufs[1].data_ptr(), bufs[2].data_ptr(), _st())
     dx, dg, db = _twice(run, dx, acc[0][0], acc[1][0])
     ref = R.layernorm_bwd(x.double(), dy.double(), gamma.double(), 1e-5, torch.full((C,), 0.5, dtype=torch.float64, device=cuda),
                           torch.full((C,), -1.0, dtype=torch.float64, device=cuda), None if r is None else r.double())
@@ -886,7 +821,7 @@ def test_win_attn_bias_bwd(cuda, B, H, W, heads, ws, extra):
     dS, dSins, dSidx = _strided_out(nwin, row, ldS, torch.float32, cuda)
     dq, dqins = _flat_out(B * H * W * 3 * C, torch.bfloat16, cuda)
     lib.call("es3_win_attn_bias_bwd", qkv.data_ptr(), dout.data_ptr(), bias.data_ptr(), dq.data_ptr(), dS.data_ptr(), ldS, B, H, W,
-             C, heads, ws, scale, _stream())
+             C, heads, ws, scale, _st())
     ref = R.win_attn_bias_bwd(qkv.double(), dout.double(), bias.double(), B, H, W, C, heads, ws, scale)
     what = f"win_attn_bias_bwd B{B} {H}x{W} heads{heads} ws{ws} ldS+{extra}"
     _check("10 win_attn_bias_bwd dqkv", dq[:B * H * W * 3 * C].view(B * H * W, 3 * C), *ref["dqkv"], what)
@@ -910,7 +845,7 @@ def test_colsum_f32(cuda, M, L, ld):
 
     def run(bufs):
         ws.fill_(float("nan"))
-        lib.call("es3_colsum_f32", src.data_ptr(), ld, M, L, ws.data_ptr(), bufs[0].data_ptr(), _stream())
+        lib.call("es3_colsum_f32", src.data_ptr(), ld, M, L, ws.data_ptr(), bufs[0].data_ptr(), _st())
     got = _twice(run, buf)[0]
     ref, bound = R.colsum(src[:, :L].double(), o0.double())
     _check("10 colsum", got[:L], ref, bound, f"colsum M{M} L{L} ld{ld}")
@@ -919,7 +854,7 @@ def test_colsum_f32(cuda, M, L, ld):
 
 # ----------------------------------------------------------------------------------------------------------- route closure
 def covered_keys():
-    """Every route key some table row above exercises, computed from the tables with the key functions route_key uses."""
+    """Every route key (tests/routes.py) some table row above exercises."""
     keys = set()
     keys |= {key_wgrad_pw(c[0], c[1], False) for c in WGPW_DESIGN}
     keys |= {key_wgrad_pw(N, C, True) for _, _, _, N, C in [(2, 9, 7, 32, 16), (1, 12, 12, 64, 128), (3, 5, 33, 24, 8),
@@ -927,32 +862,14 @@ def covered_keys():
     keys |= {key_wgrad_pw(N, C, True) for _, _, _, N, C in [(2, 10, 14, 24, 8), (1, 32, 32, 48, 16), (1, 512, 512, 24, 8)]}
     keys |= {key_wgrad_tc(c[0]) for c in WGTC_DESIGN}
     keys |= {key_dw_bwd_data(c[4], c[5]) for c in DWBD_CASES}
-    keys |= {key_dw_wgrad("direct", *c[1]) for c in DWD_DESIGN} | {key_dw_wgrad("win", *c[1]) for c in DWW_DESIGN}
-    keys |= {("bn_act_bwd", c[1], c[0], c[4]) for c in BNB_ROWS}
-    keys |= {("bn_act_bwd_apply", c[1], c[4]) for c in BNB_ROWS}
-    keys |= {("affine_act", c[0], c[3], c[4]) for c in AFF_ROWS}
-    keys |= {("stem_wgrad", c[2]) for c in STEM_CASES}
-    keys |= {("litemla_bwd_generic", c[1]) for c in LM_CASES if c[0]}
-    keys |= {("layernorm_bwd", c[2]) for c in LN_DESIGN}
-    keys |= {("win_attn_bias_bwd", c[4]) for c in WIN_CASES}
-    keys |= {(k,) for k in ("bn_stats", "add_bf16", "se_dgate", "se_apply", "bilinear_bwd", "litemla_bwd", "colsum", "transpose_pad",
-                            "accumulate_strided")}
+    keys |= {("es3_dwconv_wgrad",) + c[1] for c in DWD_DESIGN} | {("es3_dwconv_wgrad_win",) + c[1] for c in DWW_DESIGN}
+    keys |= {("es3_bn_act_bwd_reduce", c[1], c[0], c[4]) for c in BNB_ROWS}
+    keys |= {("es3_bn_act_bwd_apply", c[1], c[4]) for c in BNB_ROWS}
+    keys |= {("es3_affine_act", c[0], c[3], c[4]) for c in AFF_ROWS}
+    keys |= {("es3_stem_wgrad", c[2]) for c in STEM_CASES}
+    keys |= {("es3_litemla_attn_bwd_generic", c[1]) for c in LM_CASES if c[0]}
+    keys |= {("es3_layernorm_bwd", c[2]) for c in LN_DESIGN}
+    keys |= {("es3_win_attn_bias_bwd", c[4]) for c in WIN_CASES}
+    keys |= {(k,) for k in ("es3_bn_stats", "es3_add_bf16", "es3_se_bwd_dgate", "es3_se_bwd_apply", "es3_bilinear_bwd",
+                            "es3_litemla_attn_bwd", "es3_colsum_f32", "es3_transpose_pad_bf16", "es3_accumulate_strided")}
     return keys
-
-
-def record_training_step(cuda, monkeypatch, name, frozen_bn, img=1024, embed=64, B=1):
-    """The route keys of one native KD training step (forward, loss, backward) of `name`, from its es3_* calls."""
-    calls = training_step_calls(cuda, monkeypatch, name, frozen_bn, img, embed, B)
-    return {k for k in (route_key(n, a) for n, a in calls) if k is not None}
-
-
-@pytest.mark.parametrize("name", STUDENTS)
-def test_route_closure(cuda, monkeypatch, name):
-    """Every backward-kernel route one native training step of `name` reaches at stage-1's geometry (1024^2, embed 64, batch 1),
-    with batch-statistics and with frozen BatchNorm, is exercised by some table row above."""
-    reached = set()
-    for frozen in (False, True):
-        reached |= record_training_step(cuda, monkeypatch, name, frozen)
-    missing = reached - covered_keys()
-    print(f"\n{name}: {len(reached)} route keys reached: {sorted(reached, key=repr)}", end="")
-    assert not missing, f"{name} reaches backward routes no table row runs: {sorted(missing, key=repr)}"

@@ -7,16 +7,16 @@ Outputs are NaN-prefilled and called through _lib.call: every cell inside the ou
 bound, every cell past it (a flat TAIL, or the columns around a strided output) keeps its sentinel bits; rope_f32 works in place
 and must keep the bits of the v block and of the row padding.  Every case runs twice and must be bit-identical; the last image run
 alone must be bit-identical to the same image inside the batch; es3_attention_bf16 and the ops wrappers are bit-identical to the
-direct entry point they pick; a shape or pointer an entry point declines writes nothing.  A route-closure test records the kernels
-the 1008 px teacher (bf16 and strict), the 336 and vit_small_112 trunks and Sam3PointPromptSegmenter.set_image reach and asserts
-that some table row runs each of them; es3_layernorm_f32 (the teacher's ln_pre, norm1 and norm2) is held by the LNF table of
-tests/test_text_kernels_gpu.py.
+direct entry point they pick; a shape or pointer an entry point declines writes nothing.  covered_keys() names the route keys
+(tests/routes.py) the tables run, for the route closure of tests/test_route_closure_gpu.py (the 1008 px teacher, bf16 and strict,
+the 336 and vit_small_112 trunks and Sam3PointPromptSegmenter.set_image).
 
 GAMMA = 2 (ref_train_bwd.GAMMA) holds without change.  Worst err/bound per section in one run on an H100 80GB HBM3 (700 W power
 limit): bf16 attention -- wgmma BN 96 0.888 (windowed) and 0.612 (global), BN 128 0.931 (global) and 0.945 (windowed), mma.sync MT 1
 0.938 (windowed) and 0.9 (global), MT 2 0.919 (windowed) and 0.618 (global), where the output's own rounding half-step dominates the
 bound; fp32 outputs -- sgemm_f32 0.239, rope_f32 0.249, attention_f32 0.0086 (head_dim 32) and 0.0048 (head_dim 64), ln_rows_f32
-0.022.  The whole file (128 tests, the route-closure forwards included) took 14 s there.
+0.022.  The whole file (128 tests, the route-closure forwards included, since moved to tests/test_route_closure_gpu.py) took 14 s
+there.
 """
 import functools
 
@@ -24,8 +24,9 @@ import pytest
 import torch
 
 import ref_vit as R
-from bounds import _assert_untouched, _check, _flat_out, _gen, _matrix_out, _padded, _pairwise, report_worst
-from test_text_kernels_gpu import _bits_equal, _declined, _lib, _p, _qkv, _st, _twice
+from bounds import (_assert_untouched, _bits_equal, _check, _declined, _flat_out, _gen, _lib, _matrix_out, _p, _padded, _pairwise,
+                    _qkv, _st, _twice, report_worst)
+from routes import attn_key
 
 pytestmark = pytest.mark.gpu
 _report_worst = report_worst("ViT kernels")
@@ -35,30 +36,6 @@ BF = torch.bfloat16
 def _ops():
     from efficientsam3_b200 import ops
     return ops
-
-
-# ----------------------------------------------------------------------------------------------------------- route keys
-def attn_key(name, H, W, win):
-    L = win * win if win else H * W
-    if name == "es3_attention_tc_bf16" or (name == "es3_attention_bf16" and L >= 128):
-        return ("attention_tc", R.bn_tile(L), win > 0)
-    return ("attention_mma", 2 if L >= 128 else 1, win > 0)
-
-
-def route_key(name, a):
-    """Route key of one recorded es3_* call (None: not a kernel of this file)."""
-    if name in ("es3_attention_bf16", "es3_attention_tc_bf16", "es3_attention_mma_bf16"):
-        return attn_key(name, a[3], a[4], a[7])
-    if name == "es3_sgemm_f32":
-        return ("sgemm_f32", a[11], bool(a[14]), a[9] not in (None, 0), a[10] not in (None, 0), a[12] not in (None, 0))
-    if name == "es3_rope_f32":
-        return ("rope_f32", a[7] > 0)
-    if name == "es3_attention_f32":
-        return ("attention_f32", a[9], a[2] not in (None, 0), a[3] not in (None, 0), a[14] > 0)
-    if name == "es3_im2col_f32":
-        return ("im2col_f32", bool(a[9]), a[6], a[7])
-    simple = {"es3_im2col_patch": "im2col_patch", "es3_tokens_f32_to_nchw": "tokens_to_nchw", "es3_ln_rows_f32": "ln_rows_f32"}
-    return (simple[name],) if name in simple else None
 
 
 def _last_image(B, n):
@@ -102,7 +79,7 @@ def _attn_case(cuda, name, kernel, B, H, W, heads, win, kind, scale):
     what = f"{name} B{B} {H}x{W} heads{heads} win{win} {kind} scale {scale}"
     _check(f"1 {key}", o, ref, bound, what)
     _assert_untouched(got, ins, what)
-    if attn_key("es3_attention_bf16", H, W, win) == key:
+    if attn_key("es3_attention_bf16", H, W, win)[1:] == key[1:]:
         d = torch.full((n, C), float("nan"), dtype=BF, device=cuda)
         _attn(lib, "es3_attention_bf16", qkv, d, B, H, W, heads, win, scale)
         _bits_equal(d, o, what + ": es3_attention_bf16 vs the direct call")
@@ -227,7 +204,10 @@ SG = _pairwise(dict(M=[1, 63, 64, 65, 300], N=[1, 17, 64, 100, 1024], K=[1, 15, 
 SG += [(63, 1024, 588, None, False, "none", False),            # the strict teacher's patch embedding (im2col of 14 x 14 x 3)
        (300, 1024, 1024, None, False, "bias", True),           # qkv
        (65, 1024, 4736, None, False, "bias_res", True),        # fc2 + residual
-       (64, 4736, 1024, "gelu", False, "bias", False)]         # fc1
+       (64, 4736, 1024, "gelu", False, "bias", False),         # fc1
+       (257, 16, 27, "hswish", False, "scale_bias", False),    # the strict student encoder: BatchNorm folded into scale and bias
+       (300, 128, 64, None, False, "scale_bias", True),
+       (65, 96, 576, "gelu", False, "scale_bias", False)]
 
 
 @pytest.mark.parametrize("M,N,K,act,after,epi,strided", SG)
@@ -398,12 +378,14 @@ def test_ln_rows_f32(cuda, C, M, shift):
 
 # ----------------------------------------------------------------------------------------------------------- (9) strict im2col
 I2C = [(1, 1008, 1008, 3, 14, 14, 0, True), (2, 112, 112, 3, 14, 14, 0, True), (2, 9, 11, 16, 3, 1, 1, False),
-       (2, 15, 13, 32, 3, 2, 1, False), (1, 20, 18, 24, 3, 2, 1, False)]
+       (2, 15, 13, 32, 3, 2, 1, False), (1, 20, 18, 24, 3, 2, 1, False),
+       (2, 33, 31, 3, 3, 2, 1, True)]                   # the strict student's stem: 3 x 3 stride 2 on the NCHW image
 
 
 @pytest.mark.parametrize("B,H,W,C,ks,stride,pad,nchw", I2C)
 def test_im2col_f32(cuda, B, H, W, C, ks, stride, pad, nchw):
-    """The NCHW patch form (ks 14, stride 14) and the NHWC 3 x 3 forms at stride 1 and 2, bit-exact against F.unfold."""
+    """The NCHW patch form (ks 14, stride 14), the NCHW 3 x 3 stride-2 stem and the NHWC 3 x 3 forms at stride 1 and 2, bit-exact
+    against F.unfold."""
     lib = _lib(cuda)
     shape = (B, C, H, W) if nchw else (B, H, W, C)
     x = torch.randn(*shape, device=cuda, generator=_gen(cuda, "i2c", B, H, W, C, ks, stride))
@@ -423,97 +405,17 @@ def test_im2col_f32(cuda, B, H, W, C, ks, stride, pad, nchw):
 
 
 # ----------------------------------------------------------------------------------------------------------- route closure
-# Kernels the ViT routes reach that other files hold to their bounds: the GEMMs and the RoPE epilogue
-# (tests/test_gemm_epilogue_gpu.py), the casts (tests/test_text_kernels_gpu.py), the neck's convolutions, pooling and layout changes
-# (tests/test_gemm_epilogue_gpu.py, tests/test_fwd_kernels_gpu.py) and the SAM heads' kernels (tests/test_sam_kernels_gpu.py).
-# es3_layernorm_f32 must be a covered key of tests/test_text_kernels_gpu.py.
-EXCLUDED = {"es3_gemm_bf16", "es3_gemm_bf16_ex", "es3_pw_small_bf16", "es3_gemm_simt", "es3_cast_f32_to_bf16", "es3_cast_f32_to_f16",
-            "es3_convt2x2_bf16", "es3_conv3x3_bf16", "es3_maxpool2x2_bf16", "es3_nchw_f32_to_nhwc", "es3_nhwc_to_nchw_f32",
-            "es3_bilinear_nhwc_to_nchw", "es3_bilinear_nchw_f32", "es3_add_rows", "es3_dense_pe", "es3_init"}
-TEXT = {"es3_layernorm_f32"}
-
-
 def covered_keys():
-    """Every route key some table row above runs, computed from the tables with the key functions route_key uses."""
-    keys = {attn_key("es3_attention_tc_bf16", c[1], c[2], c[4]) for c in TC}
-    keys |= {attn_key("es3_attention_mma_bf16", c[1], c[2], c[4]) for c in MMA}
-    keys |= {("im2col_patch",) for _ in PATCH} | {("tokens_to_nchw",) for _ in T2N} | {("ln_rows_f32",) for _ in LNR}
+    """Every route key (tests/routes.py) some table row above runs; es3_attention_bf16 where _attn_case calls it too."""
+    keys = set()
+    for name, rows in (("es3_attention_tc_bf16", TC), ("es3_attention_mma_bf16", MMA)):
+        for c in rows:
+            key, dispatched = attn_key(name, c[1], c[2], c[4]), attn_key("es3_attention_bf16", c[1], c[2], c[4])
+            keys |= {key, dispatched} if dispatched[1:] == key[1:] else {key}
+    keys |= {("es3_im2col_patch",) for _ in PATCH} | {("es3_tokens_f32_to_nchw",) for _ in T2N} | {("es3_ln_rows_f32",) for _ in LNR}
     from efficientsam3_b200.ops import ACT
-    keys |= {("sgemm_f32", ACT[c[3]], c[4], "scale" in c[5], "bias" in c[5], "res" in c[5]) for c in SG}
-    keys |= {("rope_f32", c[0] > 0) for c in ROPE}
-    keys |= {("attention_f32", c[4], c[7], c[8], c[5] > 0) for c in AF32}
-    keys |= {("im2col_f32", c[7], c[4], c[5]) for c in I2C}
+    keys |= {("es3_sgemm_f32", ACT[c[3]], c[4], "scale" in c[5], "bias" in c[5], "res" in c[5]) for c in SG}
+    keys |= {("es3_rope_f32", c[0] > 0) for c in ROPE}
+    keys |= {("es3_attention_f32", c[4], c[7], c[8], c[5] > 0) for c in AF32}
+    keys |= {("es3_im2col_f32", c[7], c[4], c[5]) for c in I2C}
     return keys
-
-
-def _closure(calls, who):
-    import test_text_kernels_gpu as TK
-    reached = {k for k in (route_key(n, a) for n, a in calls) if k is not None}
-    missing = reached - covered_keys()
-    text = {TK.route_key(n, a) for n, a in calls if n in TEXT}
-    unknown = {n for n, a in calls if route_key(n, a) is None} - EXCLUDED - TEXT
-    print(f"\n{who}: {len(reached)} ViT route keys reached: {sorted(reached, key=repr)}", end="")
-    assert not missing, f"{who} reaches ViT routes no table row runs: {sorted(missing, key=repr)}"
-    assert not text - TK.covered_keys(), f"{who} reaches LayerNorm routes no text-kernel row runs: {sorted(text - TK.covered_keys())}"
-    assert not unknown, f"{who} reaches kernels neither this file nor another's table accounts for: {sorted(unknown)}"
-    return reached
-
-
-def _teacher_calls(cuda, monkeypatch, strict):
-    from es3_recorder import record_calls
-    from efficientsam3_b200.stage1.model import SAM3ImageTeacherEncoder
-    t = SAM3ImageTeacherEncoder(embed_size=72, vit_overrides=dict(depth=2, global_att_blocks=(1,))).to(cuda)
-    x = torch.randn(2, 3, 1008, 1008, device=cuda, generator=torch.Generator(device=cuda).manual_seed(0))
-
-    def run():
-        with torch.no_grad():
-            if strict:
-                with _ops().strict_precision():
-                    t(x)
-            else:
-                t(x)
-    return record_calls(monkeypatch, run)
-
-
-def test_route_closure_teacher(cuda, monkeypatch):
-    """SAM3ImageTeacherEncoder at 1008 px, one windowed and one global block, B = 2: both reach attn_tc_kernel<96>."""
-    reached = _closure(_teacher_calls(cuda, monkeypatch, False), "teacher 1008")
-    assert {("attention_tc", 96, True), ("attention_tc", 96, False)} <= reached
-
-
-def test_route_closure_teacher_strict(cuda, monkeypatch):
-    reached = _closure(_teacher_calls(cuda, monkeypatch, True), "teacher 1008 strict")
-    assert ("attention_f32", 64, False, False, True) in reached and ("attention_f32", 64, False, False, False) in reached
-
-
-def _vit_small_cfg():
-    from helpers import load_golden
-    return eval(str(load_golden("vit_small_112")["cfg"]))
-
-
-@pytest.mark.parametrize("which", ["336", "vit_small_112"])
-def test_route_closure_backbone(cuda, monkeypatch, which):
-    """create_sam3_vit_backbone with tests/test_vit_gpu.py's 336 configuration and the vit_small_112 fixture's."""
-    from es3_recorder import record_calls
-    from efficientsam3_b200.model.vitdet import create_sam3_vit_backbone
-    cfg = (dict(img_size=336, pretrain_img_size=112, patch_size=14, embed_dim=256, depth=4, num_heads=4, mlp_ratio=4.625,
-                window_size=8, global_att_blocks=(1, 3)) if which == "336" else _vit_small_cfg())
-    m = create_sam3_vit_backbone(**cfg).to(cuda).eval()
-    x = torch.randn(2, 3, cfg["img_size"], cfg["img_size"], device=cuda, generator=torch.Generator(device=cuda).manual_seed(1))
-
-    def run():
-        with torch.no_grad():
-            m(x)
-    _closure(record_calls(monkeypatch, run), f"ViT backbone {which}")
-
-
-def test_route_closure_segmenter(cuda, monkeypatch):
-    """Sam3PointPromptSegmenter (one windowed block) through the interactive predictor's set_image."""
-    import numpy as np
-    from es3_recorder import record_calls
-    from efficientsam3_b200.model.sam1_task import SAM3InteractiveImagePredictor, Sam3PointPromptSegmenter
-    seg = Sam3PointPromptSegmenter(vit_overrides=dict(depth=1, global_att_blocks=())).to(cuda).eval()
-    pred = SAM3InteractiveImagePredictor(seg)
-    img = np.random.default_rng(4).integers(0, 256, (600, 800, 3), dtype=np.uint8)
-    reached = _closure(record_calls(monkeypatch, lambda: pred.set_image(img)), "segmenter set_image")
-    assert ("attention_tc", 96, True) in reached

@@ -1,6 +1,6 @@
 """Records the es3_* calls a piece of native work makes (tests/test_route_closure_gpu.py): every _lib.call, and every _lib.call_rc
 that ran (rc == 0; a declined shape returns -1); and builds the model paths recorded there -- the image students' eval forward and
-training step, the text students' training steps and the SAM3 text teacher, the interactive predictor and the SAM heads' module
+training step (the eval forward in both precision modes), the text students' training steps and the SAM3 text teacher, the interactive predictor and the SAM heads' module
 API, the SAM3 image teacher, ViT backbones and the point segmenter's set_image."""
 import numpy as np
 import torch
@@ -56,14 +56,19 @@ def training_step_calls(cuda, monkeypatch, name, frozen_bn, img=1024, embed=64, 
     return record_calls(monkeypatch, lambda: KDLossFunction.apply(m(x), teacher, sz, img, 1.0).backward())
 
 
-def eval_forward_calls(cuda, monkeypatch, name, img=1024, embed=64, B=2):
-    """The es3_* calls of one eval forward of `name`."""
+def eval_forward_calls(cuda, monkeypatch, name, img=1024, embed=64, B=2, strict=False):
+    """The es3_* calls of one eval forward of `name`, in the strict precision mode or not."""
+    from efficientsam3_b200 import ops
     m = student(cuda, name, img, embed).eval()
     x = torch.randn(B, 3, img, img, device=cuda, generator=torch.Generator(device=cuda).manual_seed(0))
 
     def run():
         with torch.no_grad():
-            m(x)
+            if strict:
+                with ops.strict_precision():
+                    m(x)
+            else:
+                m(x)
     return record_calls(monkeypatch, run)
 
 

@@ -16,7 +16,7 @@ from collections import defaultdict
 from ref_vit import bn_tile
 
 HOST_ONLY = {"es3_init", "es3_version", "es3_last_error"}       # and the *_ws_floats size queries: no kernel behind them
-_ACT = {0: None, 1: "relu", 2: "hswish", 3: "gelu"}
+_ACT = {0: None, 1: "relu", 2: "hswish", 3: "gelu", 6: "sigmoid"}
 _BN_MODE = {0: "none", 1: "eval", 2: "batch"}
 
 
@@ -126,11 +126,16 @@ _DETAILED = {
     "es3_rope_f32": lambda a: ("es3_rope_f32", a[7] > 0),
     "es3_attention_f32": lambda a: ("es3_attention_f32", a[9], _nz(a[2]), _nz(a[3]), a[14] > 0),
     "es3_im2col_f32": lambda a: ("es3_im2col_f32", bool(a[9]), a[6], a[7]),
+    # the strict mode's student kernels
+    "es3_dwconv_f32": lambda a: ("es3_dwconv_f32", a[11], a[12], _act(a[13]), _nz(a[3]), _nz(a[4])),
+    "es3_litemla_attn_f32": lambda a: ("es3_litemla_attn_f32", a[8], a[6] > 2048),          # HW > 2048: more than one chunk
+    "es3_bias_act_res_f32": lambda a: ("es3_bias_act_res_f32", _act(a[6]), _nz(a[1]), _nz(a[2]), bool(a[7])),
+    "es3_bilinear_nhwc_f32_to_nchw": lambda a: ("es3_bilinear_nhwc_f32_to_nchw", "same" if (a[3], a[4]) == (a[6], a[7]) else "resize"),
 }
 
 _FWD, _BWD, _TEXT, _SAM, _VIT = ("test_fwd_kernels_gpu.py", "test_train_bwd_gpu.py", "test_text_kernels_gpu.py",
                                  "test_sam_kernels_gpu.py", "test_vit_kernels_gpu.py")
-_GEMM, _STRICT = "test_gemm_epilogue_gpu.py", "test_strict_gpu.py"
+_GEMM, _STRICT = "test_gemm_epilogue_gpu.py", "test_strict_kernels_gpu.py"
 _FILES = {
     _FWD: """mbconv_bf16 dwproj_tc_bf16 dwconv_tc_bf16 dwconv_tiled_bf16 dwconv_bf16 stem_conv3x3_s2 dsconv_res_bf16 litemla_attn_generic
              conv3x3_s2_narrow_bf16 win_attn_bias_bf16 layernorm_bf16 stem_fused_c16 litemla_aggreg_dwpw litemla_attn_tc channel_mean
@@ -145,9 +150,9 @@ _FILES = {
              ln_rows_gelu_f32 hyper_masks bilinear_nchw_f32 mask_downscale_tokens""",
     _VIT: """attention_bf16 attention_tc_bf16 attention_mma_bf16 sgemm_f32 rope_f32 attention_f32 im2col_f32 im2col_patch
              tokens_f32_to_nchw ln_rows_f32""",
+    _STRICT: "dwconv_f32 litemla_attn_f32 bias_act_res_f32 bilinear_nhwc_f32_to_nchw scale_channels_f32",
     # files without covered_keys(): they hold the name-only key of the entry points listed for them
     _GEMM: "gemm_bf16 gemm_bf16_ex pw_small_bf16 gemm_simt conv3x3_bf16 convt2x2_bf16",
-    _STRICT: "dwconv_f32 litemla_attn_f32 bias_act_res_f32 bilinear_nhwc_f32_to_nchw scale_channels_f32",
     "test_amg_gpu.py": "amg_mask_stats box_nms amg_rle",
     "test_fp8_gpu.py": "gemm_fp8 quantize_bf16_e4m3 pack_weight_e4m3 layernorm_f32_e4m3",
     "test_fp8_attention_gpu.py": "attention_fp8",

@@ -32,6 +32,29 @@ def test_route_closure_student(cuda, monkeypatch, name, step):
     assert_closed(calls, f"{name} {step}")
 
 
+# The strict route keys the code says these students reach at 1024^2, spelled as the recorded calls spell them: EfficientViT-B1's
+# stage-3 LiteMLA runs at HW 4096 (two chunks) with head dim 16, B2's with head dim 32; RepViT's SqueezeExcite runs fc1 with ReLU and
+# fc2 with the sigmoid gate (bias, no scale, no residual) and gates the map; TinyViT's window attention has the relative bias and
+# pad_row and is windowed.
+STRICT_PINNED = {
+    "efficientvit_b1": {("es3_litemla_attn_f32", 16, True), ("es3_litemla_attn_f32", 16, False)},
+    "efficientvit_b2": {("es3_litemla_attn_f32", 32, True), ("es3_litemla_attn_f32", 32, False)},
+    "repvit_m1_1": {("es3_sgemm_f32", 1, False, False, True, False), ("es3_sgemm_f32", 6, False, False, True, False),
+                    ("es3_scale_channels_f32",)},
+    "tiny_vit_11m": {("es3_attention_f32", 32, True, True, True)},
+}
+
+
+@pytest.mark.parametrize("name", STUDENTS)
+def test_route_closure_student_strict(cuda, monkeypatch, name):
+    """The eval forward of `name` at 1024^2 (batch 2) inside ops.strict_precision(): every strict kernel call keyed and covered by
+    the strict student kernels' tables (tests/test_strict_kernels_gpu.py) or the ViT file's strict tables."""
+    reached = assert_closed(eval_forward_calls(cuda, monkeypatch, name, strict=True), f"{name} strict")
+    assert reached and not [k for k in reached if "bf16" in k[0]], f"{name} strict reaches bf16 kernels"
+    missing = STRICT_PINNED.get(name, set()) - reached
+    assert not missing, f"{name} strict: expected routes not reached: {sorted(missing, key=repr)}"
+
+
 # ----------------------------------------------------------------------------------------------------------- text encoders
 @pytest.mark.parametrize("route", TEXT_ROUTES, ids=[r[0] for r in TEXT_ROUTES])
 def test_route_closure_text(cuda, monkeypatch, route):

@@ -13,8 +13,10 @@ from test_boundary import _declared
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 KERNEL_TEST_FILES = ["test_gemm_epilogue_gpu.py", "test_train_bwd_gpu.py", "test_fwd_kernels_gpu.py", "test_text_kernels_gpu.py",
-                     "test_sam_kernels_gpu.py", "test_vit_kernels_gpu.py"]
+                     "test_sam_kernels_gpu.py", "test_vit_kernels_gpu.py", "test_strict_kernels_gpu.py"]
 MBCONV_B1_STAGE3 = (0,) * 13 + (128, 512, 128, 1, 1, 2, 0)     # es3_mbconv_bf16 arguments: Cin 128, mid 512, Cout 128, stride 1
+# es3_dwconv_f32 arguments of LiteMLA's strict 5 x 5 aggregation (EfficientViT-B1 stage 3 at 1024^2): no scale, no bias, no act
+LITEMLA_AGGREG_F32 = (0, 768, 0, 0, 0, 0, 384, 2, 64, 64, 384, 5, 1, 0, 0)
 
 
 def test_keys_are_the_kernel_entry_points_of_the_header():
@@ -80,3 +82,12 @@ def test_closure_accepts_a_gemm_only_because_covered_lists_it(monkeypatch):
     monkeypatch.setitem(COVERED, "es3_gemm_bf16_ex", ["test_fwd_kernels_gpu.py"])
     with pytest.raises(AssertionError, match="no table row runs"):
         assert_closed([call], "gemm unlisted")
+
+
+def test_closure_rejects_a_strict_dwconv_whose_table_row_is_gone(monkeypatch):
+    call = ("es3_dwconv_f32", LITEMLA_AGGREG_F32)
+    assert assert_closed([call], "strict dwconv") == {("es3_dwconv_f32", 5, 1, None, False, False)}
+    strict = importlib.import_module("test_strict_kernels_gpu")
+    monkeypatch.setattr(strict, "DW", [c for c in strict.DW if (c[4], c[5], c[6], c[7], c[8]) != (5, 1, None, False, False)])
+    with pytest.raises(AssertionError, match="no table row runs"):
+        assert_closed([call], "strict dwconv row removed")

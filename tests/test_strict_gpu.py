@@ -4,14 +4,14 @@
     mask logits  rtol 1e-3   asserted as max|err| <= 1e-3 * max|logit| (measured ~1e-5)
     binary masks bit-exact   (logit > 0) identical on EVERY pixel of the fixtures
 
-and each strict kernel (csrc/strict_f32.cu) against its torch statement in tests/emu_strict.py; the ViT trunk's strict kernels
-(sgemm_f32, im2col_f32, ln_rows_f32, rope_f32, attention_f32) are held element by element to fp64 bounds in
-tests/test_vit_kernels_gpu.py."""
+and the strict compositions conv2d_f32 (im2col + SGEMM), convt2x2_f32 and the SAM heads' fp32 twins against their torch statements in
+tests/emu_strict.py.  The strict kernels themselves are held element by element to fp64 bounds: the ViT trunk's (sgemm_f32,
+im2col_f32, ln_rows_f32, rope_f32, attention_f32) in tests/test_vit_kernels_gpu.py, the students' (dwconv_f32, litemla_attn_f32,
+bilinear_nhwc_f32_to_nchw, bias_act_res_f32, scale_channels_f32) in tests/test_strict_kernels_gpu.py."""
 from types import SimpleNamespace as NS
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import emu_strict as E
 from helpers import load_golden, max_err_over_scale, rel_l2, sd_from_keys
@@ -49,40 +49,6 @@ def test_conv2d_f32(cuda, B, H, W, C, N, ks, stride, nchw):
         _close(got, E.conv2d_f32(x.double(), w.double(), 1, ks // 2, bias=bi.double(), residual=res.double()).float(), 3e-6, "conv2d_f32 + res")
 
 
-@pytest.mark.parametrize("B,H,W,C,ks,stride", [(2, 9, 11, 16, 3, 1), (1, 16, 16, 48, 5, 1), (2, 15, 13, 32, 3, 2), (1, 4, 4, 8, 5, 1)])
-def test_dwconv_f32(cuda, B, H, W, C, ks, stride):
-    from efficientsam3_b200 import ops
-    g = _g(B + H + C + ks)
-    wide = torch.randn(B, H, W, 2 * C + 3, generator=g)
-    x = wide[..., 1:1 + C]                                          # channel slice of a wider map
-    w = torch.randn(ks * ks, C, generator=g) / ks
-    sc, bi = torch.rand(C, generator=g) + 0.5, torch.randn(C, generator=g)
-    got = ops.dwconv_f32(wide.to(cuda)[..., 1:1 + C], w.to(cuda), sc.to(cuda), bi.to(cuda), ks, stride, "hswish")
-    ref = E.dwconv_f32(x.double(), w.double(), sc.double(), bi.double(), ks, stride, "hswish")
-    _close(got, ref.float(), 3e-6, "dwconv_f32")
-
-
-@pytest.mark.parametrize("B,H,W,heads,dim", [(2, 9, 7, 4, 16), (1, 64, 64, 16, 16), (2, 12, 12, 6, 32), (1, 3, 7, 2, 16)])
-def test_litemla_attn_f32(cuda, B, H, W, heads, dim):
-    from efficientsam3_b200 import ops
-    ms = torch.randn(B, H, W, 3 * dim * heads, generator=_g(H + heads))
-    got = ops.litemla_attn_f32(ms.to(cuda), heads, dim, 1e-15)
-    ref = E.litemla_attn_f32(ms.double(), heads, dim, 1e-15)
-    _close(got, ref.float(), 2e-5, "litemla_attn_f32")
-    assert torch.equal(got, ops.litemla_attn_f32(ms.to(cuda), heads, dim, 1e-15))      # fixed reduction order
-
-
-@pytest.mark.parametrize("Hi,Wi,Ho,Wo", [(10, 10, 12, 12), (32, 32, 64, 64), (5, 7, 5, 7), (23, 23, 9, 9)])
-def test_bilinear_nhwc_f32_to_nchw(cuda, Hi, Wi, Ho, Wo):
-    from efficientsam3_b200 import ops
-    x = torch.randn(2, Hi, Wi, 24, generator=_g(Hi + Ho))
-    got = ops.bilinear_nhwc_f32_to_nchw(x.to(cuda), Ho, Wo)
-    ref = E.bilinear_nhwc_f32_to_nchw(x, Ho, Wo)
-    _close(got, ref, 2e-6, "bilinear f32")
-    if (Hi, Wi) == (Ho, Wo):
-        assert torch.equal(got.cpu(), ref)
-
-
 def test_decoder_twins_f32(cuda):
     from efficientsam3_b200 import ops
     g = _g(4)
@@ -97,14 +63,6 @@ def test_decoder_twins_f32(cuda):
     r = torch.randn(2, 18, 14, 32, generator=g)
     got = ops.convt2x2_f32(xt.to(cuda), wt.to(cuda), bt.to(cuda), act="gelu", residual=r.to(cuda), act_after_res=True)
     _close(got, E.convt2x2_f32(xt.double(), wt.double(), bt.double(), act="gelu", residual=r.double(), act_after_res=True).float(), 3e-6, "convt2x2_f32")
-
-
-@pytest.mark.parametrize("B,H,W,C", [(2, 5, 7, 48), (1, 9, 3, 160)])
-def test_scale_channels_f32(cuda, B, H, W, C):
-    from efficientsam3_b200 import ops
-    g = _g(17 + C)
-    x, gate = torch.randn(B, H, W, C, generator=g), torch.rand(B, C, generator=g)
-    assert torch.equal(ops.scale_channels_f32(x.to(cuda), gate.to(cuda)).cpu(), E.scale_channels_f32(x, gate))
 
 
 # ------------------------------------------------------------------------------------------------ student encoders

@@ -9,7 +9,8 @@ and must keep the bits of the v block and of the row padding.  Every case runs t
 alone must be bit-identical to the same image inside the batch; es3_attention_bf16 and the ops wrappers are bit-identical to the
 direct entry point they pick; a shape or pointer an entry point declines writes nothing.  covered_keys() names the route keys
 (tests/routes.py) the tables run, for the route closure of tests/test_route_closure_gpu.py (the 1008 px teacher, bf16 and strict,
-the 336 and vit_small_112 trunks and Sam3PointPromptSegmenter.set_image).
+the 336 and vit_small_112 trunks and Sam3PointPromptSegmenter.set_image).  The strict SGEMM table also holds the strict students'
+GEMM routes: their folded-BatchNorm epilogues and RepViT's SqueezeExcite fc1 (ReLU) and fc2 (sigmoid gate) on the pooled rows.
 
 GAMMA = 2 (ref_train_bwd.GAMMA) holds without change.  Worst err/bound per section in one run on an H100 80GB HBM3 (700 W power
 limit): bf16 attention -- wgmma BN 96 0.888 (windowed) and 0.612 (global), BN 128 0.931 (global) and 0.945 (windowed), mma.sync MT 1
@@ -207,7 +208,11 @@ SG += [(63, 1024, 588, None, False, "none", False),            # the strict teac
        (64, 4736, 1024, "gelu", False, "bias", False),         # fc1
        (257, 16, 27, "hswish", False, "scale_bias", False),    # the strict student encoder: BatchNorm folded into scale and bias
        (300, 128, 64, None, False, "scale_bias", True),
-       (65, 96, 576, "gelu", False, "scale_bias", False)]
+       (65, 96, 576, "gelu", False, "scale_bias", False),
+       (2, 80, 320, "relu", False, "bias", False),             # the strict RepViT SqueezeExcite: fc1 on the pooled [B, C] rows
+       (2, 320, 80, "sigmoid", False, "bias", False),          # fc2, the gate
+       (3, 24, 96, "relu", False, "bias", True),
+       (3, 96, 24, "sigmoid", False, "bias", True)]
 
 
 @pytest.mark.parametrize("M,N,K,act,after,epi,strided", SG)

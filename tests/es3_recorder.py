@@ -1,7 +1,7 @@
 """Records the es3_* calls a piece of native work makes (tests/test_route_closure_gpu.py): every _lib.call, and every _lib.call_rc
 that ran (rc == 0; a declined shape returns -1); and builds the model paths recorded there -- the image students' eval forward and
 training step (the eval forward in both precision modes), the text students' training steps and the SAM3 text teacher, the interactive predictor and the SAM heads' module
-API, the SAM3 image teacher, ViT backbones and the point segmenter's set_image."""
+API, the SAM3 image teacher (bf16, strict and FP8), ViT backbones and the point segmenter's set_image."""
 import numpy as np
 import torch
 
@@ -218,11 +218,15 @@ def module_api_calls(cuda, monkeypatch):
     return record_calls(monkeypatch, run)
 
 
-def teacher_calls(cuda, monkeypatch, strict):
-    """The es3_* calls of SAM3ImageTeacherEncoder at 1008 px (one windowed and one global block, B = 2), in the strict mode or not."""
+def teacher_calls(cuda, monkeypatch, strict, fp8=None):
+    """The es3_* calls of SAM3ImageTeacherEncoder at 1008 px (one windowed and one global block, B = 2), in the strict mode or not;
+    fp8 = "linear" or "attention": with enable_fp8(True, attention=fp8 == "attention"), the weights packed inside the recorded
+    forward."""
     from efficientsam3_b200 import ops
     from efficientsam3_b200.stage1.model import SAM3ImageTeacherEncoder
     t = SAM3ImageTeacherEncoder(embed_size=72, vit_overrides=dict(depth=2, global_att_blocks=(1,))).to(cuda)
+    if fp8 is not None:
+        t.enable_fp8(True, attention=fp8 == "attention")
     x = torch.randn(2, 3, 1008, 1008, device=cuda, generator=torch.Generator(device=cuda).manual_seed(0))
 
     def run():

@@ -70,6 +70,82 @@ def causal_attn_key(L):
     return ("es3_attention_causal_bf16", 2 if L >= 128 else 1)
 
 
+# The wgmma GEMM family (gemm_tc.cu) selects gemm_tc_kernel<BN, STAGES, ACT> by the rules restated here.  In its keys activations
+# go by name, residuals and outputs by dtype ("bf16" / "f32", None when absent), RoPE as None / "window" / "global".
+def pick_bn(N, bn_hint, K=1 << 30, act=None):
+    """gemm_tc.cu pick_bn: the tile width for N output columns, a tile-width hint, K and the activation."""
+    if bn_hint in (32, 64, 128):
+        return bn_hint
+    if bn_hint == 256:
+        return 128
+    if K < 512 and N >= 64:
+        if act == "gelu":
+            return 64
+        return 128 if N >= 384 else 64
+    if N % 128 == 0 or N > 1024:
+        return 128
+    if N % 64 == 0:
+        return 64
+    return 128 if N >= 128 else 32
+
+
+def gemm_bn(N, K, act, rope, bn_hint):
+    """es3_gemm_bf16_ex: pick_bn, except that the RoPE epilogue takes 128-wide tiles when N >= 128 and no hint is given."""
+    return 128 if rope is not None and bn_hint == 0 and N >= 128 else pick_bn(N, bn_hint, K, act)
+
+
+def gemm_stages(bn, num_kb):
+    """gemm_tc.cu dispatch: the operand ring's depth at tile width bn for num_kb 64-wide k-blocks."""
+    if bn == 128:
+        return 2 if num_kb <= 2 else 4
+    return 2 if bn == 64 else 4
+
+
+def conv_tile_w(W):
+    """es3_conv3x3_bf16: the implicit GEMM's tile width in pixels for an image W pixels wide."""
+    return 32 if W % 32 == 0 else (16 if W % 16 == 0 else 8)
+
+
+def conv3x3_num_kb(C):
+    """es3_conv3x3_bf16: nine taps of ceil(C / 64) k-blocks each."""
+    return 9 * -(-C // 64)
+
+
+def gemm_key(name, N, K, act, scale, bias, res, after, out, rope, bn_hint):
+    """es3_gemm_bf16_ex / es3_gemm_bf16: (name, BN, STAGES, act, scale, bias, residual, act after the residual (only when both are
+    present), out, RoPE, ragged last 32-column chunk)."""
+    bn = gemm_bn(N, K, act, rope, bn_hint)
+    return (name, bn, gemm_stages(bn, -(-K // 64)), act, bool(scale), bool(bias), res, bool(after and res and act), out, rope,
+            N % 32 != 0)
+
+
+def conv3x3_key(N, W, act, scale, bias, res, out, bn_hint):
+    return ("es3_conv3x3_bf16", pick_bn(N, bn_hint), conv_tile_w(W), act, bool(scale), bool(bias), res, out)
+
+
+def convt2x2_key(Cin, Cout, act, res, after, out):
+    bn = pick_bn(4 * Cout, 0)
+    return ("es3_convt2x2_bf16", bn, gemm_stages(bn, -(-Cin // 64)), act, res, bool(after and res and act), out)
+
+
+def fp8_attn_key(H, W, win):
+    """es3_attention_fp8: the key tile is 96 when L is a multiple of 96 but not of 128 (attention_fp8.cu), else 128."""
+    L = win * win if win else H * W
+    return ("es3_attention_fp8", 96 if L % 96 == 0 and L % 128 != 0 else 128, win > 0)
+
+
+def _res(ptr, f32):
+    return ("f32" if f32 else "bf16") if _nz(ptr) else None
+
+
+def _dt(f32):
+    return "f32" if f32 else "bf16"
+
+
+def _rope(ptr, win):
+    return ("window" if win else "global") if _nz(ptr) else None
+
+
 # ----------------------------------------------------------------------------------------------------------- KEYS
 _DETAILED = {
     # image students' forward kernels
@@ -131,6 +207,21 @@ _DETAILED = {
     "es3_litemla_attn_f32": lambda a: ("es3_litemla_attn_f32", a[8], a[6] > 2048),          # HW > 2048: more than one chunk
     "es3_bias_act_res_f32": lambda a: ("es3_bias_act_res_f32", _act(a[6]), _nz(a[1]), _nz(a[2]), bool(a[7])),
     "es3_bilinear_nhwc_f32_to_nchw": lambda a: ("es3_bilinear_nhwc_f32_to_nchw", "same" if (a[3], a[4]) == (a[6], a[7]) else "resize"),
+    # GEMMs and convolutions on the wgmma GEMM, the narrow pointwise and CUDA-core GEMMs
+    "es3_gemm_bf16_ex": lambda a: gemm_key("es3_gemm_bf16_ex", a[8], a[9], _act(a[12]), _nz(a[10]), _nz(a[11]), _res(a[13], a[15]),
+                                           a[21], _dt(a[6]), _rope(a[16], a[20]), a[22]),
+    "es3_gemm_bf16": lambda a: gemm_key("es3_gemm_bf16", a[8], a[9], _act(a[12]), _nz(a[10]), _nz(a[11]), _res(a[13], 0), False,
+                                        _dt(a[6]), None, a[15]),
+    "es3_conv3x3_bf16": lambda a: conv3x3_key(a[8], a[6], _act(a[11]), _nz(a[9]), _nz(a[10]), _res(a[12], 0), _dt(a[3]), a[13]),
+    "es3_convt2x2_bf16": lambda a: convt2x2_key(a[7], a[8], _act(a[10]), _res(a[11], a[12]), a[13], _dt(a[3])),
+    "es3_pw_small_bf16": lambda a: ("es3_pw_small_bf16", a[10], a[9], _nz(a[6])),
+    "es3_gemm_simt": lambda a: ("es3_gemm_simt", _dt(a[2]), _dt(a[5]), _act(a[14]), _nz(a[12]), _nz(a[13]), _res(a[15], a[17]),
+                                _dt(a[8])),
+    # the SAM3 ViT teacher's FP8 route
+    "es3_gemm_fp8": lambda a: ("es3_gemm_fp8", ("bf16", "f32", "e4m3")[a[8]], _act(a[14]), _nz(a[15]), _rope(a[17], a[21])),
+    "es3_attention_fp8": lambda a: fp8_attn_key(a[4], a[5], a[8]),
+    "es3_pack_weight_e4m3": lambda a: ("es3_pack_weight_e4m3", _dt(a[1])),
+    "es3_layernorm_f32_e4m3": lambda a: ("es3_layernorm_f32_e4m3", a[7] // 128),
 }
 
 _FWD, _BWD, _TEXT, _SAM, _VIT = ("test_fwd_kernels_gpu.py", "test_train_bwd_gpu.py", "test_text_kernels_gpu.py",
@@ -151,11 +242,11 @@ _FILES = {
     _VIT: """attention_bf16 attention_tc_bf16 attention_mma_bf16 sgemm_f32 rope_f32 attention_f32 im2col_f32 im2col_patch
              tokens_f32_to_nchw ln_rows_f32""",
     _STRICT: "dwconv_f32 litemla_attn_f32 bias_act_res_f32 bilinear_nhwc_f32_to_nchw scale_channels_f32",
-    # files without covered_keys(): they hold the name-only key of the entry points listed for them
     _GEMM: "gemm_bf16 gemm_bf16_ex pw_small_bf16 gemm_simt conv3x3_bf16 convt2x2_bf16",
-    "test_amg_gpu.py": "amg_mask_stats box_nms amg_rle",
     "test_fp8_gpu.py": "gemm_fp8 quantize_bf16_e4m3 pack_weight_e4m3 layernorm_f32_e4m3",
     "test_fp8_attention_gpu.py": "attention_fp8",
+    # files without covered_keys(): they hold the name-only key of the entry points listed for them
+    "test_amg_gpu.py": "amg_mask_stats box_nms amg_rle",
     "test_preprocess_gpu.py": "prepare_images_u8",
     "test_optim_gpu.py": "adamw_flat grad_norm kd_loss_fwd kd_loss_bwd",
     "test_kd_loss_gpu.py": "kd_loss_fwd",

@@ -27,6 +27,7 @@ import torch
 
 from emu_fp8_attention import HEAD, dequantized, key_tile, merge_out, split_qkv
 from helpers import cosine, rel_l2
+from routes import fp8_attn_key
 
 pytestmark = pytest.mark.gpu
 
@@ -141,6 +142,11 @@ def test_attention_fp8_vs_fp64(cuda, B, H, W, heads, win, kind):
     C = heads * HEAD
     qkv = _qkv(B, H, W, C, kind, _gen("attn", B, H, W, heads, win, kind))
     _check(cuda, qkv, B, H, W, C, heads, win, f"B{B} {H}x{W} heads{heads} win{win} {kind}")
+
+
+def covered_keys():
+    """Every route key (tests/routes.py) some row of CASES runs: both key tiles, windowed and global."""
+    return {fp8_attn_key(H, W, win) for B, H, W, heads, win, kind in CASES}
 
 
 def test_attention_fp8_vs_unquantised_inputs(cuda):

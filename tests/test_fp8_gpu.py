@@ -68,7 +68,10 @@ def _rows_with_spread(M, C, g, strided_amax=True):
 
 
 # ---------------------------------------------------------------------------------------------- quantisers
-@pytest.mark.parametrize("M,C,strided", [(1, 128, False), (77, 1024, True), (300, 384, False), (1029, 2048, True)])
+QUANT_ROWS = [(1, 128, False), (77, 1024, True), (300, 384, False), (1029, 2048, True)]
+
+
+@pytest.mark.parametrize("M,C,strided", QUANT_ROWS)
 def test_quantize_bf16_bit_exact(cuda, M, C, strided):
     from efficientsam3_b200 import ops
     x = _rows_with_spread(M, C, _gen("q", M, C)).to(torch.bfloat16)
@@ -85,7 +88,10 @@ def test_quantize_bf16_bit_exact(cuda, M, C, strided):
     _assert_codes(q, s, wq, ws, f"quantize_e4m3 {M}x{C}")
 
 
-@pytest.mark.parametrize("M,C", [(1, 1024), (133, 1024), (517, 2048)])
+LN_ROWS = [(1, 1024), (133, 1024), (517, 2048)]
+
+
+@pytest.mark.parametrize("M,C", LN_ROWS)
 def test_layernorm_e4m3_bit_exact(cuda, M, C):
     """The quantised LayerNorm equals the emulation applied to es3_layernorm_f32's fp32 output (same statistics, same arithmetic)."""
     from efficientsam3_b200 import ops
@@ -99,8 +105,11 @@ def test_layernorm_e4m3_bit_exact(cuda, M, C):
     _assert_codes(q, s, wq, ws, f"layernorm_e4m3 {M}x{C}")
 
 
-@pytest.mark.parametrize("N,K,dtype", [(128, 128, torch.float32), (200, 384, torch.float32), (3072, 1024, torch.bfloat16),
-                                       (4736, 1024, torch.float32), (77, 256, torch.bfloat16)])
+PACK_ROWS = [(128, 128, torch.float32), (200, 384, torch.float32), (3072, 1024, torch.bfloat16), (4736, 1024, torch.float32),
+             (77, 256, torch.bfloat16)]
+
+
+@pytest.mark.parametrize("N,K,dtype", PACK_ROWS)
 def test_pack_weight_bit_exact(cuda, N, K, dtype):
     from efficientsam3_b200 import ops
     g = _gen("w", N, K)
@@ -197,9 +206,11 @@ def _gelu64(x):
 EPS_GELU = 3e-7          # es3_gelu_fast's own error per |x| (test_gemm_epilogue_gpu.py)
 
 
-@pytest.mark.parametrize("M,N,K,spread,strided", [(77, 128, 128, True, False), (300, 1024, 1024, True, True),
-                                                  (1029, 3072, 1024, False, False), (257, 1024, 4736, False, True),
-                                                  (5184, 1024, 4736, True, False)])
+RES_ROWS = [(77, 128, 128, True, False), (300, 1024, 1024, True, True), (1029, 3072, 1024, False, False),
+            (257, 1024, 4736, False, True), (5184, 1024, 4736, True, False)]
+
+
+@pytest.mark.parametrize("M,N,K,spread,strided", RES_ROWS)
 def test_gemm_fp8_residual_f32(cuda, M, N, K, spread, strided):
     """proj / fc2: bias + fp32 residual -> fp32, and the same without residual; M not a multiple of 128."""
     from efficientsam3_b200 import ops
@@ -218,7 +229,10 @@ def test_gemm_fp8_residual_f32(cuda, M, N, K, spread, strided):
         _WORST["err / absprod"] = max(_WORST.get("err / absprod", 0.0), ((got.double() - ref).abs() / absprod.clamp_min(1e-30)).max().item())
 
 
-@pytest.mark.parametrize("win,M_img", [(24, 2), (0, 1)])
+ROPE_ROWS = [(24, 2), (0, 1)]
+
+
+@pytest.mark.parametrize("win,M_img", ROPE_ROWS)
 def test_gemm_fp8_rope_bf16(cuda, win, M_img):
     """qkv: bias + 2-D axial RoPE on q | k -> bf16 at the teacher's geometry (72 x 72 tokens, C = 1024), windowed and global;
     v columns unrotated."""
@@ -250,7 +264,10 @@ def test_gemm_fp8_rope_bf16(cuda, win, M_img):
     _check("bf16 rope", got, ref, bound, f"rope win={win}")
 
 
-@pytest.mark.parametrize("M,N,K", [(77, 128, 128), (1029, 4736, 1024), (300, 1024, 4736)])
+GELU_ROWS = [(77, 128, 128), (1029, 4736, 1024), (300, 1024, 4736)]
+
+
+@pytest.mark.parametrize("M,N,K", GELU_ROWS)
 def test_gemm_fp8_gelu_e4m3(cuda, M, N, K):
     """fc1: bias + GELU(erf).  The fp32 epilogue is checked against fp64; the e4m3 epilogue's codes and per-row / 128-column
     scales must equal the emulation's quantisation of that fp32 result, except where a value lies within one fp32 ulp of an
@@ -292,6 +309,17 @@ def test_gemm_fp8_fc2_reads_fc1_output(cuda):
     acc = a64 @ w64.t()
     ref = acc + b2.cpu().double()
     _check("f32", got, ref, _bound(a64.abs() @ w64.abs().t(), acc, Hd, b2.cpu().double()) + 4 * U * ref.abs(), "fc1 -> fc2")
+
+
+def covered_keys():
+    """Every route key (tests/routes.py) some table row above runs: the quantisers, and the GEMM's epilogues -- fp32 with and
+    without the residual, bf16 with windowed and global RoPE, GELU to fp32 and to e4m3."""
+    keys = {("es3_quantize_bf16_e4m3",) for _ in QUANT_ROWS} | {("es3_layernorm_f32_e4m3", C // 128) for _, C in LN_ROWS}
+    keys |= {("es3_pack_weight_e4m3", "f32" if dt == torch.float32 else "bf16") for _, _, dt in PACK_ROWS}
+    keys |= {("es3_gemm_fp8", "f32", None, res, None) for _ in RES_ROWS for res in (True, False)}
+    keys |= {("es3_gemm_fp8", "bf16", None, False, "window" if win else "global") for win, _ in ROPE_ROWS}
+    keys |= {("es3_gemm_fp8", out, "gelu", False, None) for _ in GELU_ROWS for out in ("f32", "e4m3")}
+    return keys
 
 
 # ---------------------------------------------------------------------------------------------- the teacher end to end

@@ -1,5 +1,7 @@
-"""The fused GEMM epilogue of gemm_tc.cu (1x1 convs, nn.Linear, the implicit-GEMM 3x3 conv, the 2x2 transposed conv) and the
-CUDA-core gemm_simt.cu, element by element against fp64.
+"""The fused GEMM epilogue of gemm_tc.cu (1x1 convs, nn.Linear, the implicit-GEMM 3x3 conv, the 2x2 transposed conv), the
+narrow pointwise pw_small.cu and the CUDA-core gemm_simt.cu, element by element against fp64.  Sections (a) to (g) are covering
+designs over the epilogue's options and the tile geometries; section (i) adds one row for each route key (tests/routes.py: tile,
+pipeline depth, epilogue options) that a model path reaches and those sections do not run.  covered_keys() lists the keys of all.
 
 Operands are bf16-representable (A, W and bf16 residuals are rounded first), so the fp64 statement
 y = act(s * (A W^T) + b) (+ r), in the order the call asks for, is what the kernel would compute with exact arithmetic.  Every
@@ -19,8 +21,9 @@ NaN-padded buffers, so a read outside the slice also shows.
 
 GAMMA = 2 and the eps_act of tests/bounds.py were set from one run on an H100 80GB HBM3 (700 W power limit).  Measured maximum err/bound per
 section, fp32 outputs: (a) epilogue matrix 0.18, (c) act/residual order 0.021, (d) RoPE 0.0037, (e) conv3x3 0.019,
-(f) convt2x2 0.025, (g) gemm_simt 0.054, so the fp32 accumulation stays well inside 2 K u.  bf16 outputs: 0.87 ... 0.996 in
-every section (pw_small 0.995), because the half-step of the output rounding dominates their bound and is reached.
+(f) convt2x2 0.025, (g) gemm_simt 0.054, (i) model routes 0.0082, so the fp32 accumulation stays well inside 2 K u.  bf16 outputs:
+0.87 ... 0.996 in every section (pw_small 0.995, (i) 0.99 and its pw_small rows 0.995), because the half-step of the output
+rounding dominates their bound and is reached.
 (b) reaches 1.0 of its half-step tolerance by construction: the residual sits at a bf16 midpoint.
 """
 import math
@@ -31,6 +34,7 @@ import torch.nn.functional as F
 
 from bounds import (L_ACT, U, _INT, _act64, _assert_untouched, _bf, _check, _eps_act, _flat_out, _gen, _matrix_out, _p, _padded,
                     _pairwise, _st, report_worst, WORST)
+from routes import conv3x3_key, convt2x2_key, gemm_key
 
 pytestmark = pytest.mark.gpu
 
@@ -87,8 +91,9 @@ def _gemm_id(c):
             f"{'-strided' if strided else ''}")
 
 
-def _gemm_case(cuda, M, N, K, act, after, has_s, has_b, res, out, bn, strided, seed=()):
-    from efficientsam3_b200 import ops
+def _gemm_case(cuda, M, N, K, act, after, has_s, has_b, res, out, bn, strided, seed=(), c_entry=False):
+    """One GEMM through ops.gemm, or with c_entry through es3_gemm_bf16's C entry (bf16 residual only, act before it)."""
+    from efficientsam3_b200 import _lib, ops
     g = _gen(cuda, M, N, K, act, after, has_s, has_b, res, out, bn, strided, *seed)
     a = _padded(_bf(torch.randn(M, K, device=cuda, generator=g)), strided)
     w = _bf(torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K))
@@ -100,8 +105,16 @@ def _gemm_case(cuda, M, N, K, act, after, has_s, has_b, res, out, bn, strided, s
         r = _padded(_bf(r) if res == "bf16" else r, strided)
     dt = torch.float32 if out == "f32" else torch.bfloat16
     buf, o, inside = _matrix_out(M, N, dt, strided, cuda)
-    got = ops.gemm(a, w, scale=scale, bias=bias, act=act, residual=r, out=o, bn_hint=bn, act_after_res=after)
-    assert got.data_ptr() == o.data_ptr()
+    if c_entry:
+        assert res != "f32" and not after
+        _lib.init(cuda.index or 0)
+        rc = _lib.call_rc("es3_gemm_bf16", a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), o.data_ptr(), o.stride(0),
+                          int(out == "f32"), M, N, K, _p(scale), _p(bias), ops.ACT[act], _p(r), 0 if r is None else r.stride(0),
+                          bn, _st())
+        assert rc == 0
+    else:
+        got = ops.gemm(a, w, scale=scale, bias=bias, act=act, residual=r, out=o, bn_hint=bn, act_after_res=after)
+        assert got.data_ptr() == o.data_ptr()
     acc = a.double() @ w.double().t()
     absprod = a.double().abs() @ w.double().abs().t()
     ref, bound = _expect(acc, absprod, K, act, scale, bias, r, after, out_bf16=out == "bf16")
@@ -120,9 +133,12 @@ def test_gemm_epilogue(cuda, monkeypatch, M, N, K, act, after, has_s, has_b, res
     _assert_untouched(buf, inside, what)
 
 
+PW_SMALL_ROWS = [(4099, 16, 16, "bf16", True), (231, 64, 32, None, False), (1, 32, 64, "bf16", False), (129, 16, 64, None, True),
+                 (5184, 32, 16, "bf16", False)]
+
+
 @pytest.mark.parametrize("pw_small", [True, False])
-@pytest.mark.parametrize("M,N,K,res,strided", [(4099, 16, 16, "bf16", True), (231, 64, 32, None, False), (1, 32, 64, "bf16", False),
-                                               (129, 16, 64, None, True), (5184, 32, 16, "bf16", False)])
+@pytest.mark.parametrize("M,N,K,res,strided", PW_SMALL_ROWS)
 def test_gemm_pw_small_route(cuda, monkeypatch, M, N, K, res, strided, pw_small):
     """Plain narrow GEMMs (K, N <= 64, no scale / bias / act, bf16 out) on es3_pw_small_bf16 and, with the switch off, on wgmma."""
     from efficientsam3_b200 import ops
@@ -134,9 +150,10 @@ def test_gemm_pw_small_route(cuda, monkeypatch, M, N, K, res, strided, pw_small)
 
 
 # ---------------------------------------------------------------------------------------------- (b) the fp32 residual's precision
-@pytest.mark.parametrize("out", ["f32", "bf16"])
-@pytest.mark.parametrize("N", [96, 80])
-@pytest.mark.parametrize("bn", [32, 64, 128])
+FP32_RES_ROWS = [(bn, N, out) for bn in (32, 64, 128) for N in (96, 80) for out in ("f32", "bf16")]
+
+
+@pytest.mark.parametrize("bn,N,out", FP32_RES_ROWS)
 def test_fp32_residual_keeps_precision(cuda, bn, N, out):
     """|A W^T| ~ 1 on a residual near 4096, where bf16's step is 32.  fp32 out: the residual's fraction survives (|err| <= 1e-3).
     bf16 out: the residual sits within 1 of 4112, the midpoint between two bf16 values, so a sum rounded once at the store is
@@ -162,9 +179,10 @@ def test_fp32_residual_keeps_precision(cuda, bn, N, out):
 
 
 # ---------------------------------------------------------------------------------------------- (c) activation vs residual order
-@pytest.mark.parametrize("res", ["bf16", "f32"])
-@pytest.mark.parametrize("after", [False, True])
-@pytest.mark.parametrize("N", [96, 40])
+ORDER_ROWS = [(N, after, res) for N in (96, 40) for after in (False, True) for res in ("bf16", "f32")]
+
+
+@pytest.mark.parametrize("N,after,res", ORDER_ROWS)
 def test_act_residual_order(cuda, N, after, res):
     """relu on a negative pre-activation (about -2) with a positive residual (3 .. 4): relu(x) + r = r, relu(x + r) = x + r, two
     answers about 2 apart.  N = 96 runs the vectorised chunks only, N = 40 a full chunk and a ragged 8-column one."""
@@ -188,15 +206,21 @@ def test_act_residual_order(cuda, N, after, res):
 
 
 # ---------------------------------------------------------------------------------------------- (d) RoPE epilogue
-@pytest.mark.parametrize("win,out,bn", [(24, "bf16", 128), (24, "f32", 64), (0, "bf16", 64), (0, "f32", 128)])
+ROPE_ROWS = [(24, "bf16", 128), (24, "f32", 64), (0, "bf16", 64), (0, "f32", 128)]
+
+
+@pytest.mark.parametrize("win,out,bn", ROPE_ROWS)
 def test_rope_epilogue_teacher_geometry(cuda, win, out, bn):
     """The SAM3 ViT's QKV projection: 72 x 72 tokens, B = 2, C = 1024, bias; windows of 24 (576 table positions) or global (5184).
     q | k (columns < 2C) rotated per 64-dim head; v (columns >= 2C) bit-identical to the same GEMM without RoPE."""
+    _rope_case(cuda, 2, 72, 72, 1024, win, out, bn)
+
+
+def _rope_case(cuda, B, H, W, C, win, out, bn, seed=(), section="d"):
     from efficientsam3_b200 import ops
     from efficientsam3_b200.model.vitdet import compute_axial_cis
-    B, H, W, C = 2, 72, 72, 1024
     M, N, K = B * H * W, 3 * C, C
-    g = _gen(cuda, "d", win, out, bn)
+    g = _gen(cuda, "d", win, out, bn, *seed)
     a = _bf(torch.randn(M, K, device=cuda, generator=g))
     w = _bf(torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K))
     bias = torch.randn(N, device=cuda, generator=g)
@@ -226,12 +250,12 @@ def test_rope_epilogue_teacher_geometry(cuda, win, out, bn):
     bound[:, :2 * C] += 4 * U * ref[:, :2 * C].abs()
     if out == "bf16":
         bound = bound * (1 + 2.0 ** -8) + 2.0 ** -8 * ref.abs()
-    _check(f"d/{out}", o, ref, bound, f"rope win={win} {out} bn={bn}")
+    _check(f"{section}/{out}", o, ref, bound, f"rope {B}x{H}x{W} C{C} win={win} {out} bn={bn}")
     _assert_untouched(buf, inside, "rope")
 
 
 # ---------------------------------------------------------------------------------------------- (e) es3_conv3x3_bf16
-def _conv3x3(cuda, x, w, epi, bn=0, seed=0):
+def _conv3x3(cuda, x, w, epi, bn=0, seed=0, section="e"):
     """Run the implicit-GEMM conv through its C entry into a NaN-prefilled buffer; check it against fp64 F.conv2d."""
     from efficientsam3_b200 import _lib, ops
     B, H, W, C = x.shape
@@ -253,7 +277,7 @@ def _conv3x3(cuda, x, w, epi, bn=0, seed=0):
     absprod = F.conv2d(xn.abs(), wd.abs(), padding=1).permute(0, 2, 3, 1)
     ref, bound = _expect(acc, absprod, 9 * C, act, scale, bias, res, False, out_bf16=dt == torch.bfloat16)
     what = f"conv3x3 B{B} {H}x{W} C{C}->N{N} {epi} bn{bn}"
-    _check(f"e/{'f32' if dt == torch.float32 else 'bf16'}", buf[:B * H * W * N].view(B, H, W, N), ref, bound, what)
+    _check(f"{section}/{'f32' if dt == torch.float32 else 'bf16'}", buf[:B * H * W * N].view(B, H, W, N), ref, bound, what)
     _assert_untouched(buf, inside, what)
 
 
@@ -275,9 +299,11 @@ def test_conv3x3_geometry(cuda, W, H, C, N, epi):
     _conv3x3(cuda, x, w, epi)
 
 
-@pytest.mark.parametrize("B,H,W,C,N,epi", [(1, 144, 144, 256, 256, "bias_f32"), (2, 144, 144, 256, 256, "bias"),
-                                           (2, 36, 36, 256, 256, "bias"), (2, 64, 64, 1024, 1024, "bias"),
-                                           (1, 64, 64, 1024, 1024, "nobias")])
+CONV_PROD_ROWS = [(1, 144, 144, 256, 256, "bias_f32"), (2, 144, 144, 256, 256, "bias"), (2, 36, 36, 256, 256, "bias"),
+                  (2, 64, 64, 1024, 1024, "bias"), (1, 64, 64, 1024, 1024, "nobias")]
+
+
+@pytest.mark.parametrize("B,H,W,C,N,epi", CONV_PROD_ROWS)
 def test_conv3x3_production_shapes(cuda, B, H, W, C, N, epi):
     """The FPN neck's 3x3 conv at the 2x (144^2, fp32 levels too) and 0.5x (36^2) levels; the student head at 64^2 and its input
     gradient (no bias)."""
@@ -287,7 +313,10 @@ def test_conv3x3_production_shapes(cuda, B, H, W, C, N, epi):
     _conv3x3(cuda, x, w, epi)
 
 
-@pytest.mark.parametrize("W", [64, 48, 23])
+HALO_W = [64, 48, 23]
+
+
+@pytest.mark.parametrize("W", HALO_W)
 def test_conv3x3_halo(cuda, W):
     """Large values (8) in the last column and last row of every image, small ones (< 1/16) elsewhere: column 0 reading its left
     neighbour from the previous row's last column, or an image's last row reading the next image's first row (or the reverse),
@@ -351,10 +380,11 @@ def test_convt2x2_scatter(cuda, Cout, Cin, mode, res, out, HW):
     _convt2x2(cuda, 3, HW[0], HW[1], Cin, Cout, mode, res, out)
 
 
-@pytest.mark.parametrize("B,H,W,Cin,Cout,mode,res,out", [(1, 72, 72, 1024, 512, "gelu_before", None, "bf16"),
-                                                         (1, 144, 144, 512, 256, "none", None, "bf16"),
-                                                         (2, 72, 72, 256, 64, "none", "f32", "f32"),
-                                                         (2, 144, 144, 64, 32, "gelu_after", "f32", "f32")])
+CONVT_PROD_ROWS = [(1, 72, 72, 1024, 512, "gelu_before", None, "bf16"), (1, 144, 144, 512, 256, "none", None, "bf16"),
+                   (2, 72, 72, 256, 64, "none", "f32", "f32"), (2, 144, 144, 64, 32, "gelu_after", "f32", "f32")]
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,mode,res,out", CONVT_PROD_ROWS)
 def test_convt2x2_production_shapes(cuda, B, H, W, Cin, Cout, mode, res, out):
     """The FPN neck's 4x level (1024 -> 512 with GELU, 512 -> 256) and the mask decoder's upscaling (256 -> 64 on an fp32 residual,
     64 -> 32 with GELU after the residual)."""
@@ -380,14 +410,18 @@ SIMT_DESIGN = _pairwise(SIMT_FACTORS, seed=4)
                               for c in SIMT_DESIGN])
 def test_gemm_simt(cuda, dtypes, res, out, M, K, N, act, has_s):
     """The CUDA-core GEMM (SE MLPs and their backward in fp32, the decoder's token MLPs) with every operand dtype pair."""
+    _simt_case(cuda, dtypes, res, out, M, K, N, act, has_s)
+
+
+def _simt_case(cuda, dtypes, res, out, M, K, N, act, has_s, has_b=True, section="g"):
     from efficientsam3_b200 import ops
-    g = _gen(cuda, "g", dtypes, res, out, M, K, N, act, has_s)
+    g = _gen(cuda, "g", dtypes, res, out, M, K, N, act, has_s, *(() if has_b else ("no bias",)))
     a = torch.randn(M, K, device=cuda, generator=g)
     w = torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K)
     a = _bf(a) if dtypes[0] == "bf16" else a
     w = _bf(w) if dtypes[1] == "bf16" else w
     scale = (torch.rand(N, device=cuda, generator=g) + 0.5) if has_s else None
-    bias = torch.randn(N, device=cuda, generator=g)
+    bias = torch.randn(N, device=cuda, generator=g) if has_b else None
     r = None
     if res is not None:
         r = torch.randn(M, N, device=cuda, generator=g)
@@ -398,9 +432,128 @@ def test_gemm_simt(cuda, dtypes, res, out, M, K, N, act, has_s):
     acc = a.double() @ w.double().t()
     absprod = a.double().abs() @ w.double().abs().t()
     ref, bound = _expect(acc, absprod, K, act, scale, bias, r, False, out_bf16=out == "bf16")
-    what = f"gemm_simt {dtypes} res={res} {out} {M}x{N}x{K} {act}"
-    _check(f"g/{out}", o, ref, bound, what)
+    what = f"gemm_simt {dtypes} res={res} {out} {M}x{N}x{K} {act}{'' if has_b else ' no bias'}"
+    _check(f"{section}/{out}", o, ref, bound, what)
     _assert_untouched(buf, inside, what)
+
+
+# ---------------------------------------------------------------------------------------------- (i) the routes the models reach
+# One row per route key (tests/routes.py) that a recorded model path (tests/test_route_closure_gpu.py) reaches and no row above runs,
+# each at a shape that selects it; keys do not depend on M, so M stays small.  The comments name the paths that reach the key.
+#   ("ex" | "c", M, N, K, act, act after the residual, scale, bias, residual, out): es3_gemm_bf16_ex through ops.gemm (pw_small
+#       off), or es3_gemm_bf16 through its C entry; no tile hint
+#   ("rope", B, H, W, C, win, out): the QKV projection of _rope_case, no tile hint
+#   ("pw", M, N, K, residual): es3_pw_small_bf16 through ops.gemm
+#   ("simt", M, N, K, act, scale, bias, residual, out): es3_gemm_simt on fp32 A and W
+#   ("conv3x3", B, H, W, C, N, epi): es3_conv3x3_bf16 as _conv3x3 runs it
+MODEL_ROWS = [
+    # image students' eval forward: folded BN + hswish / GELU, project + bias + residual
+    ("ex", 200, 384, 96, "hswish", False, False, True, None, "bf16"),          # EfficientViT-B2 (two k-blocks: 2 stages)
+    ("ex", 231, 1024, 256, "hswish", False, False, True, None, "bf16"),        # EfficientViT-B1, B2; the EV-B1 point segmenter
+    ("ex", 257, 32, 16, "hswish", False, False, True, None, "bf16"),           # EfficientViT-B0
+    ("ex", 200, 96, 24, "hswish", False, False, True, None, "bf16"),           # EfficientViT-B0, B2
+    ("ex", 257, 24, 96, None, False, False, True, "bf16", "bf16"),             # EfficientViT-B0, B2, RepViT-M0.9 (ragged)
+    ("ex", 257, 8, 16, None, False, False, True, None, "bf16"),                # EfficientViT-B0, B2 (ragged)
+    ("ex", 129, 64, 256, None, False, False, True, "bf16", "bf16"),            # every image student
+    ("ex", 129, 256, 1024, None, False, False, True, "bf16", "bf16"),          # EfficientViT-B1, B2, RepViT, TinyViT
+    ("ex", 160, 80, 160, None, False, False, True, "bf16", "bf16"),            # RepViT-M2.3 (80 channels: ragged on 64-wide tiles)
+    ("ex", 196, 256, 64, "gelu", False, True, True, None, "bf16"),             # TinyViT
+    ("ex", 196, 64, 256, "gelu", True, True, True, "bf16", "bf16"),            # TinyViT (GELU after the residual)
+    ("ex", 196, 128, 64, None, False, True, True, None, "bf16"),               # TinyViT
+    ("ex", 150, 448, 256, None, False, True, True, None, "bf16"),              # TinyViT-11M, 21M
+    ("ex", 77, 384, 128, None, False, False, True, None, "bf16"),              # TinyViT-5M, 11M, eval and training
+    ("ex", 144, 1184, 256, "gelu", False, False, True, None, "bf16"),          # every image student; the ViT backbones
+    ("simt", 2, 40, 448, None, False, True, None, "bf16"),                     # TinyViT
+    # image students' training steps: raw 1x1 convs (no epilogue) and input gradients on the skip gradient
+    ("ex", 131, 512, 128, None, False, False, False, None, "bf16"),            # EfficientViT, TinyViT; EfficientViT-B0, B1 eval
+    ("ex", 300, 32, 8, None, False, False, False, None, "bf16"),               # EfficientViT-B0, B1, RepViT-M0.9 (K = 8)
+    ("ex", 129, 256, 1024, None, False, False, False, "bf16", "bf16"),         # EfficientViT, RepViT
+    ("ex", 129, 64, 256, None, False, False, False, "bf16", "bf16"),           # every image student
+    ("ex", 129, 128, 256, None, False, False, False, None, "f32"),             # every image student
+    ("ex", 160, 80, 160, None, False, False, False, "bf16", "bf16"),           # RepViT-M2.3
+    ("ex", 160, 80, 320, None, False, False, False, None, "bf16"),             # RepViT-M2.3
+    ("pw", 129, 64, 16, None),                                                 # EfficientViT-B0, B1
+    ("pw", 257, 32, 16, None),                                                 # EfficientViT-B0
+    ("pw", 200, 16, 32, None),                                                 # EfficientViT-B0
+    ("pw", 300, 16, 16, None),                                                 # EfficientViT-B1
+    ("pw", 131, 16, 64, "bf16"),                                               # EfficientViT-B0
+    ("pw", 77, 32, 64, None),                                                  # EfficientViT-B0, B1, RepViT-M1.1, TinyViT
+    ("simt", 2, 16, 64, None, False, False, None, "f32"),                      # RepViT (SqueezeExcite gradients)
+    # text encoders, the SAM3 ViT and the SAM heads
+    ("ex", 77, 1536, 512, None, False, False, True, None, "bf16"),             # text encoders, SAM heads, most image students
+    ("ex", 77, 512, 512, None, False, False, True, None, "f32"),               # text students, SAM3 text teacher
+    ("ex", 77, 512, 2048, None, False, False, False, None, "bf16"),            # text and image students' training steps
+    ("ex", 77, 4096, 1024, "gelu", False, False, True, None, "bf16"),          # SAM3 text teacher, SAM3 ViT, RepViT, TinyViT-21M
+    ("ex", 196, 1024, 592, None, False, False, False, None, "f32"),            # ViT patch embedding (also the FP8 teacher's), text
+    ("rope", 2, 12, 12, 1024, 0, "bf16"),                                      # global-RoPE QKV: teacher, ViT backbones
+    ("ex", 100, 1024, 4736, None, False, False, True, "f32", "f32"),           # ViT proj / fc2 on the fp32 residual stream, text
+    ("ex", 64, 32, 256, None, False, False, True, None, "f32"),                # SAM heads' high-resolution features
+    ("ex", 64, 64, 256, None, False, False, True, None, "f32"),                # SAM heads' high-resolution features
+    ("conv3x3", 1, 5, 36, 256, 256, "bias_f32"),                               # the ViT point segmenter's neck (W % 16 != 0)
+    ("simt", 6, 4, 256, "sigmoid", False, True, None, "f32"),                  # mask decoder heads, RepViT SqueezeExcite
+    ("simt", 7, 256, 256, None, False, True, "f32", "f32"),                    # mask decoder
+    ("simt", 5, 32, 256, None, False, True, None, "f32"),                      # mask decoder
+    # es3_gemm_bf16: a header entry point no Python path calls
+    ("c", 150, 96, 64, "hswish", False, True, True, "bf16", "bf16"),
+]
+
+
+def _model_row_key(row):
+    kind, *c = row
+    if kind in ("ex", "c"):
+        M, N, K, act, after, sc, bi, res, out = c
+        return gemm_key("es3_gemm_bf16_ex" if kind == "ex" else "es3_gemm_bf16", N, K, act, sc, bi, res, after, out, None, 0)
+    if kind == "rope":
+        B, H, W, C, win, out = c
+        return gemm_key("es3_gemm_bf16_ex", 3 * C, C, None, False, True, None, False, out, "window" if win else "global", 0)
+    if kind == "pw":
+        M, N, K, res = c
+        return ("es3_pw_small_bf16", K, N, res is not None)
+    if kind == "simt":
+        M, N, K, act, sc, bi, res, out = c
+        return ("es3_gemm_simt", "f32", "f32", act, sc, bi, res, out)
+    B, H, W, C, N, epi = c
+    return conv3x3_key(N, W, *_CONV_EPI[epi], 0)
+
+
+@pytest.mark.parametrize("row", MODEL_ROWS, ids=["-".join(map(str, r)) for r in MODEL_ROWS])
+def test_model_route(cuda, monkeypatch, row):
+    """Each row against fp64 with the bound and NaN sentinels of its section above; the calls it makes are recorded and the row's
+    route key must be among theirs, so the row runs the key covered_keys() claims for it."""
+    from efficientsam3_b200 import ops
+    from es3_recorder import record_calls
+    from routes import KEYS
+    kind, *c = row
+    what = "model route " + "-".join(map(str, row))
+
+    def run():
+        if kind in ("ex", "c"):
+            M, N, K, act, after, sc, bi, res, out = c
+            monkeypatch.setattr(ops, "PW_SMALL", False)
+            buf, o, inside, ref, bound = _gemm_case(cuda, M, N, K, act, after, sc, bi, res, out, 0, False, seed=("i",),
+                                                    c_entry=kind == "c")
+            _check(f"i/{out}", o, ref, bound, what)
+            _assert_untouched(buf, inside, what)
+        elif kind == "rope":
+            B, H, W, C, win, out = c
+            _rope_case(cuda, B, H, W, C, win, out, 0, seed=("i",), section="i")
+        elif kind == "pw":
+            M, N, K, res = c
+            monkeypatch.setattr(ops, "PW_SMALL", True)
+            buf, o, inside, ref, bound = _gemm_case(cuda, M, N, K, None, False, False, False, res, "bf16", 0, False, seed=("i",))
+            _check("i/pw_small", o, ref, bound, what)
+            _assert_untouched(buf, inside, what)
+        elif kind == "simt":
+            M, N, K, act, sc, bi, res, out = c
+            _simt_case(cuda, ("f32", "f32"), res, out, M, K, N, act, sc, bi, section="i")
+        else:
+            B, H, W, C, N, epi = c
+            g = _gen(cuda, "i", B, H, W, C, N, epi)
+            x = _bf(torch.randn(B, H, W, C, device=cuda, generator=g))
+            w = _bf(torch.randn(N, C, 3, 3, device=cuda, generator=g) / math.sqrt(9 * C))
+            _conv3x3(cuda, x, w, epi, section="i")
+    keys = {KEYS[n](a) for n, a in record_calls(monkeypatch, run)}
+    assert _model_row_key(row) in keys, f"{what}: runs {sorted(keys, key=repr)}, not {_model_row_key(row)}"
 
 
 # ---------------------------------------------------------------------------------------------- (h) what the wrappers refuse
@@ -460,3 +613,37 @@ def test_wrapper_rejects_dtype_the_kernel_would_misread(cuda, case):
     with pytest.raises(Es3Error):
         _refusals(cuda)[case]()
     assert ops.launch_count == n0
+
+
+# ---------------------------------------------------------------------------------------------- route keys
+_CONV_EPI = {  # epi -> act, scale, bias, residual, out (as _conv3x3 reads it)
+    "bias": (None, False, True, None, "bf16"), "nobias": (None, False, False, None, "bf16"),
+    "scale_hswish": ("hswish", True, True, None, "bf16"), "scale_gelu": ("gelu", True, True, None, "bf16"),
+    "bias_f32": (None, False, True, None, "f32"), "bias_res": (None, False, True, "bf16", "bf16")}
+
+
+def covered_keys():
+    """Every route key (tests/routes.py) some table row above runs."""
+    return table_keys() | {_model_row_key(r) for r in MODEL_ROWS}
+
+
+def table_keys():
+    """The route keys of the tables of sections (a) to (g)."""
+    ex = "es3_gemm_bf16_ex"
+    keys = {gemm_key(ex, N, K, act, sc, bi, res, after, out, None, bn)
+            for _, N, K, act, after, sc, bi, res, out, bn, _ in GEMM_DESIGN}
+    keys |= {("es3_pw_small_bf16", K, N, res is not None) for M, N, K, res, _ in PW_SMALL_ROWS}
+    keys |= {gemm_key(ex, N, K, None, False, False, res, False, "bf16", None, 0) for M, N, K, res, _ in PW_SMALL_ROWS}
+    keys |= {gemm_key(ex, N, 256, None, False, False, "f32", False, out, None, bn) for bn, N, out in FP32_RES_ROWS}
+    keys |= {gemm_key(ex, N, 64, "relu", False, True, res, after, "f32", None, 0) for N, after, res in ORDER_ROWS}
+    keys |= {gemm_key(ex, 3072, 1024, None, False, True, None, False, out, "window" if win else "global", bn)
+             for win, out, bn in ROPE_ROWS}
+    convs = [(W, C, N, epi) for W, H, C, N, epi in CONV_DESIGN] + [(W, C, N, epi) for B, H, W, C, N, epi in CONV_PROD_ROWS]
+    convs += [(W, 64, 64, "bias") for W in HALO_W]
+    keys |= {conv3x3_key(N, W, *_CONV_EPI[epi], 0) for W, C, N, epi in convs}
+    convts = [(Cin, Cout, mode, res, out) for Cout, Cin, mode, res, out, _ in CONVT_DESIGN]
+    convts += [(Cin, Cout, mode, res, out) for B, H, W, Cin, Cout, mode, res, out in CONVT_PROD_ROWS]
+    keys |= {convt2x2_key(Cin, Cout, None if mode == "none" else "gelu", res, mode == "gelu_after", out)
+             for Cin, Cout, mode, res, out in convts}
+    keys |= {("es3_gemm_simt", *dt, act, sc, True, res, out) for dt, res, out, M, K, N, act, sc in SIMT_DESIGN}
+    return keys

@@ -1,13 +1,20 @@
 """Route closure: the es3_* calls real model paths make (tests/es3_recorder.py records them) select only kernel instantiations
 that some fp64 table row runs.  Each test hands its recorded calls to routes.assert_closed, which keys every call, requires a key
 function for every entry point reached and looks the key up in the tables of the files tests/routes.py lists for its entry point;
-the extra assertions pin routes a model is expected to reach."""
+the extra assertions pin routes a model is expected to reach.  The last test checks that the GEMM tile rules routes.py restates
+from gemm_tc.cu select the instantiations the library launches."""
+import json
+import os
+import re
+import subprocess
+import sys
+
 import pytest
 
 from es3_recorder import (STUDENTS, TEXT_ROUTES, backbone_calls, eval_forward_calls, module_api_calls, point_segmenter,
                           predictor_calls, segmenter_set_image_calls, teacher_calls, text_step_calls, text_teacher_calls,
                           training_step_calls)
-from routes import KEYS, assert_closed
+from routes import KEYS, assert_closed, conv3x3_num_kb, gemm_bn, gemm_stages, pick_bn
 
 pytestmark = pytest.mark.gpu
 
@@ -100,14 +107,36 @@ def test_route_closure_module_api(cuda, monkeypatch):
 
 # ----------------------------------------------------------------------------------------------------------- SAM3 ViT trunk
 def test_route_closure_teacher(cuda, monkeypatch):
-    """SAM3ImageTeacherEncoder at 1008 px, one windowed and one global block, B = 2: both reach attn_tc_kernel<96>."""
+    """SAM3ImageTeacherEncoder at 1008 px, one windowed and one global block, B = 2: both reach attn_tc_kernel<96>, and the global
+    block's QKV projection (N = 3072, K = 1024, bias, bf16 out) takes the RoPE epilogue's 128-wide tile with the 4-stage ring."""
     reached = assert_closed(teacher_calls(cuda, monkeypatch, False), "teacher 1008")
     assert {("es3_attention_bf16", "tc", 96, True), ("es3_attention_bf16", "tc", 96, False)} <= reached
+    assert ("es3_gemm_bf16_ex", 128, 4, None, False, True, None, False, "bf16", "global", False) in reached
 
 
 def test_route_closure_teacher_strict(cuda, monkeypatch):
     reached = assert_closed(teacher_calls(cuda, monkeypatch, True), "teacher 1008 strict")
     assert ("es3_attention_f32", 64, False, False, True) in reached and ("es3_attention_f32", 64, False, False, False) in reached
+
+
+# The FP8 teacher's routes: QKV to bf16 with windowed and global RoPE, proj and fc2 to fp32 on the fp32 residual stream, fc1 to e4m3
+# with GELU, and norm1 / norm2 (C = 1024) to e4m3.
+FP8_TEACHER_PINNED = {("es3_gemm_fp8", "bf16", None, False, "window"), ("es3_gemm_fp8", "bf16", None, False, "global"),
+                      ("es3_gemm_fp8", "f32", None, True, None), ("es3_gemm_fp8", "e4m3", "gelu", False, None),
+                      ("es3_layernorm_f32_e4m3", 8)}
+
+
+@pytest.mark.parametrize("fp8", ["linear", "attention"])
+def test_route_closure_teacher_fp8(cuda, monkeypatch, fp8):
+    """The teacher of test_route_closure_teacher with enable_fp8(True, attention=fp8 == "attention"): the four linear layers on
+    es3_gemm_fp8; with FP8 attention, L = 576 (24-windows) and L = 5184 (global) both on the 96-key tile."""
+    reached = assert_closed(teacher_calls(cuda, monkeypatch, False, fp8=fp8), f"teacher 1008 fp8 {fp8}")
+    pinned = set(FP8_TEACHER_PINNED)
+    if fp8 == "attention":
+        pinned |= {("es3_attention_fp8", 96, True), ("es3_attention_fp8", 96, False)}
+    missing = pinned - reached
+    assert not missing, f"fp8 {fp8}: expected routes not reached: {sorted(missing, key=repr)}"
+    assert (fp8 == "attention") == any(k[0] == "es3_attention_fp8" for k in reached)
 
 
 @pytest.mark.parametrize("which", ["336", "vit_small_112"])
@@ -120,3 +149,72 @@ def test_route_closure_segmenter(cuda, monkeypatch):
     """Sam3PointPromptSegmenter (one windowed block) through the interactive predictor's set_image."""
     reached = assert_closed(segmenter_set_image_calls(cuda, monkeypatch), "segmenter set_image")
     assert ("es3_attention_bf16", "tc", 96, True) in reached
+
+
+# ----------------------------------------------------------------------------------------------------------- the restated tile rules
+# One call per gemm_tc_kernel<BN, STAGES, ACT> instantiation an entry point can launch, each through a different branch of pick_bn,
+# the RoPE override or the stage rule where one exists.  gemm: (N, K, act, bn_hint, rope); conv3x3: (W, C, N, act, bn_hint);
+# convt2x2: (Cin, Cout, act).
+GEMM_PICKS = [(384, 128, None, 0, False), (192, 1024, None, 0, True), (64, 64, "relu", 256, False), (1056, 512, "relu", 0, False),
+              (400, 64, "hswish", 0, False), (160, 512, "hswish", 0, False), (64, 128, "gelu", 128, False),
+              (4736, 1024, "gelu", 0, False), (96, 256, None, 0, False), (192, 512, "relu", 0, False), (32, 64, "hswish", 64, False),
+              (512, 256, "gelu", 0, False), (96, 512, None, 0, False), (48, 64, "relu", 0, False), (256, 1024, "hswish", 32, False),
+              (40, 200, "gelu", 0, False)]
+CONV_PICKS = [(16, 64, 256, None, 0), (23, 32, 160, "relu", 0), (48, 8, 64, "hswish", 128), (32, 96, 1024, "gelu", 0),
+              (64, 64, 192, None, 0), (16, 256, 64, "relu", 0), (8, 32, 256, "hswish", 64), (36, 64, 320, "gelu", 0),
+              (32, 16, 96, None, 0), (24, 64, 32, "relu", 0), (16, 128, 128, "hswish", 32), (40, 8, 32, "gelu", 0)]
+CONVT_PICKS = [(64, 32, None), (256, 64, None), (128, 64, "relu"), (192, 32, "relu"), (32, 256, "hswish"), (1024, 512, "hswish"),
+               (128, 32, "gelu"), (512, 256, "gelu")]
+
+_PICK_SCRIPT = r"""
+import json, sys
+sys.path.insert(0, sys.argv[1])
+import torch
+from efficientsam3_b200 import ops
+ops.PW_SMALL = False
+dev = torch.device("cuda:0")
+kind, rows = sys.argv[2], json.loads(sys.argv[3])
+bf = lambda *s: torch.zeros(*s, device=dev, dtype=torch.bfloat16)
+for r in rows:
+    if kind == "gemm":
+        N, K, act, bn, rope = r
+        tab = torch.zeros(16, 32, 2, device=dev)
+        ops.gemm(bf(32, K), bf(N, K), act=act, bn_hint=bn, rope=(tab, 128, 4, 4, 0) if rope else None)
+    elif kind == "conv3x3":
+        W, C, N, act, bn = r
+        ops.conv3x3(bf(1, 5, W, C), bf(N, 9 * C), act=act, bn_hint=bn)
+    else:
+        Cin, Cout, act = r
+        ops.convt2x2(bf(1, 3, 5, Cin), bf(4 * Cout, Cin), act=act)
+    torch.cuda.synchronize()
+"""
+
+
+def _expected_picks(kind):
+    from efficientsam3_b200.ops import ACT
+    if kind == "gemm":
+        rows = GEMM_PICKS
+        bns = [(gemm_bn(N, K, act, "global" if rope else None, bn), -(-K // 64), act) for N, K, act, bn, rope in rows]
+    elif kind == "conv3x3":
+        rows = CONV_PICKS
+        bns = [(pick_bn(N, bn), conv3x3_num_kb(C), act) for W, C, N, act, bn in rows]
+    else:
+        rows = CONVT_PICKS
+        bns = [(pick_bn(4 * Cout, 0), -(-Cin // 64), act) for Cin, Cout, act in rows]
+    return rows, [(bn, gemm_stages(bn, kb), ACT[act]) for bn, kb, act in bns]
+
+
+@pytest.mark.parametrize("kind", ["gemm", "conv3x3", "convt2x2"])
+def test_restated_tile_rules_match_the_launches(cuda, kind):
+    """tests/routes.py restates pick_bn, the RoPE override, the stage rule and the conv geometry of gemm_tc.cu.  A fresh process with
+    ES3_DEBUG_OCCUPANCY=1 runs one call per expected instantiation; gemm_tc.cu reports each instantiation's template arguments on
+    its first launch, so the reported lines must be the expected (BN, STAGES, ACT) list, in call order."""
+    rows, want = _expected_picks(kind)
+    assert len(set(want)) == len(want), f"{kind}: two calls expect the same instantiation"
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    env = dict(os.environ, ES3_DEBUG_OCCUPANCY="1")
+    p = subprocess.run([sys.executable, "-c", _PICK_SCRIPT, root, kind, json.dumps(rows)], env=env, cwd=root, capture_output=True,
+                       text=True, timeout=600)
+    assert p.returncode == 0, f"{kind}: the launch process exited with {p.returncode}:\n{p.stderr[-4000:]}"
+    got = [tuple(int(v) for v in m) for m in re.findall(r"gemm_tc_kernel<BN=(\d+),STAGES=(\d+),ACT=(\d+),CPR=\d+>", p.stderr)]
+    assert got == want, f"{kind}: launched {got}, the restated rules expect {want}"

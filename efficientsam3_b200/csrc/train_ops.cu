@@ -47,10 +47,11 @@ __global__ void kd_loss_bwd_kernel(const float* __restrict__ pred, const float* 
     const float a = __ldg(pp + (long long)c * HW), t = __ldg(tp + (long long)c * HW);
     dot = fmaf(a, t, dot); np2 = fmaf(a, a, np2); nt2 = fmaf(t, t, nt2);
   }
-  const float na = fmaxf(sqrtf(np2), 1e-8f), nt = fmaxf(sqrtf(nt2), 1e-8f);
+  const float np = sqrtf(np2), na = fmaxf(np, 1e-8f), nt = fmaxf(sqrtf(nt2), 1e-8f);
   const float up = gscale * (scale_dev ? scale_dev[0] : 1.f) / ((float)B * fmaxf(per_sample[b * 3 + 2], 1.f));
-  // d(1 - cos)/da_c = -(t_c / (na nt) - dot a_c / (na^3 nt))
-  const float k_t = -cosine_w * up / (na * nt), k_a = cosine_w * up * dot / (na * na * na * nt);
+  // d(1 - cos)/da_c = -(t_c / (na nt) - dot a_c / (na^2 nt |a|)), na = max(|a|, eps): the clamp keeps the 1 / na factor of cos
+  // constant below eps, but |a|'s own derivative a / |a| is still there (a / |a| := 0 at a = 0, as the norm's backward; text_bwd.cu)
+  const float k_t = -cosine_w * up / (na * nt), k_a = np > 0.f ? cosine_w * up * dot / (na * na * np * nt) : 0.f;
   const float k_mse = 2.f * up;
 #pragma unroll 4
   for (int c = 0; c < C; ++c) {

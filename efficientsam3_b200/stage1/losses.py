@@ -27,7 +27,7 @@ def kd_eval_step(student, teacher_model, images, img_size_before_pad, cosine_wei
 
 
 def kd_train_step(student, optimizer, images, teacher_embeddings, img_size_before_pad, cosine_weight: float = 1.0,
-                  clip_grad: float = 5.0, lr: float | None = None, group=None, accumulation_steps: int = 1,
+                  clip_grad: float | None = 5.0, lr: float | None = None, group=None, accumulation_steps: int = 1,
                   update: bool = True):
     """One iteration of the reference's train_one_epoch (stage1/train_image_encoder_stage1.py:185-230), everything on the
     device and on libes3 kernels:
@@ -61,7 +61,7 @@ def kd_train_step(student, optimizer, images, teacher_embeddings, img_size_befor
 
 
 def kd_train_step_online(student, teacher_model, optimizer, images, img_size_before_pad, cosine_weight: float = 1.0,
-                         clip_grad: float = 5.0, lr: float | None = None, group=None, teacher_chunk: int = 8,
+                         clip_grad: float | None = 5.0, lr: float | None = None, group=None, teacher_chunk: int = 8,
                          accumulation_steps: int = 1, update: bool = True):
     """The north-star wording of the stage-1 iteration (SURVEY.md D1 / N1): the frozen SAM3 teacher embeds the batch on the
     fly (no embedding store), the student is trained against it.  Targets are rounded through fp16 exactly as the stored
@@ -126,7 +126,7 @@ def text_kd_loss(preds: torch.Tensor, teacher: torch.Tensor, pad_mask=None, cosi
 
 
 def text_kd_train_step(student, optimizer, text, teacher_embeddings, *, cosine_weight: float = 1.0, mask_pad_tokens: bool = False,
-                       consistency_weight: float = 0.0, clip_grad: float = 5.0, lr: float | None = None, group=None,
+                       consistency_weight: float = 0.0, clip_grad: float | None = 5.0, lr: float | None = None, group=None,
                        accumulation_steps: int = 1, update: bool = True):
     """One iteration of the reference's text train_one_epoch (stage1/train_text_encoder_stage1.py:221-288) on the native path:
 

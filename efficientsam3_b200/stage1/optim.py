@@ -155,9 +155,10 @@ class FlatAdamW:
             return dist.get_world_size(group)
         return 1
 
-    def step(self, lr: float | None = None, max_norm: float = 5.0, world_size: int = 1):
-        """unscale -> global-norm clip -> AdamW -> scaler update, all on the device.  `world_size`: number of ranks whose
-        gradients were summed into the arena.  The total norm of the last step is state[3] (read it lazily)."""
+    def step(self, lr: float | None = None, max_norm: float | None = 5.0, world_size: int = 1):
+        """unscale -> global-norm clip -> AdamW -> scaler update, all on the device.  `max_norm` None or 0: no clipping, as
+        NativeScalerWithGradNormCount treats TRAIN.CLIP_GRAD.  `world_size`: number of ranks whose gradients were summed into the
+        arena.  The total norm of the last step is state[3] (read it lazily)."""
         if not self.flat_param.is_cuda:
             raise RuntimeError("FlatAdamW.step runs es3_adamw_flat on the GPU; there is no CPU fallback")
         if lr is not None:
@@ -172,7 +173,7 @@ class FlatAdamW:
         bump_weights_epoch()                     # packed training-graph weights (nn_utils.cached_pack) are stale as well
         ops.grad_norm(self.flat_grad, self._part_ws, self._norm_ws)
         ops.adamw_flat(self.flat_param, self.flat_grad, self.exp_avg, self.exp_avg_sq, self.n_decay, self.lr, self.betas,
-                       self.eps, self.weight_decay, max_norm, 1.0 / world_size, self._norm_ws, self.state,
+                       self.eps, self.weight_decay, max_norm or 0.0, 1.0 / world_size, self._norm_ws, self.state,
                        dynamic_scale=self.dynamic, growth_interval=self.growth_interval)
 
     def last_grad_norm(self) -> float:

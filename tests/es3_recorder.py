@@ -1,6 +1,7 @@
 """Records the es3_* calls a piece of native work makes (tests/test_route_closure_gpu.py): every _lib.call, and every _lib.call_rc
 that ran (rc == 0; a declined shape returns -1); and builds the model paths recorded there -- the image students' eval forward and
-training step (the eval forward in both precision modes), the text students' training steps and the SAM3 text teacher, the interactive predictor and the SAM heads' module
+training step (the eval forward in both precision modes), whole stage-1 image and text iterations (train_one_epoch and
+train_text_one_epoch with the optimiser update), the text students' training steps and the SAM3 text teacher, the interactive predictor and the SAM heads' module
 API, the SAM3 image teacher (bf16, strict and FP8), ViT backbones and the point segmenter's set_image."""
 import numpy as np
 import torch
@@ -54,6 +55,64 @@ def training_step_calls(cuda, monkeypatch, name, frozen_bn, img=1024, embed=64, 
     teacher = torch.randn(B, 1024, embed, embed, device=cuda, generator=g)
     sz = torch.tensor([[img, img]] * B, dtype=torch.int32, device=cuda)
     return record_calls(monkeypatch, lambda: KDLossFunction.apply(m(x), teacher, sz, img, 1.0).backward())
+
+
+def _stage1_cfg(**distill):
+    from types import SimpleNamespace as NS
+    return NS(TRAIN=NS(ACCUMULATION_STEPS=2, EPOCHS=3, WARMUP_EPOCHS=1, MIN_LR=1e-5, WARMUP_LR=1e-6, CLIP_GRAD=5.0,
+                       EVAL_BN_WHEN_TRAINING=False), DISTILL=NS(COSINE=1.0, **distill))
+
+
+def image_epoch_calls(cuda, monkeypatch, name, img=1024, embed=64):
+    """The es3_* calls of stage1.train.train_one_epoch over `name` with batch-statistics BatchNorm and FlatAdamW with a dynamic loss
+    scale: a two-iteration loader, ACCUMULATION_STEPS 2 (one update, clipped at 5), each batch two decoded uint8 images of different
+    sizes (prepared on the device, so the masks pad) and the stored fp16 embeddings."""
+    from types import SimpleNamespace as NS
+    from efficientsam3_b200.stage1.optim import FlatAdamW
+    from efficientsam3_b200.stage1.train import train_one_epoch
+    m = student(cuda, name, img, embed)
+    cfg = _stage1_cfg(EMBED_DIM=1024, EMBED_SIZE=embed)
+    cfg.DATA = NS(IMG_SIZE=img)
+    opt = FlatAdamW(m, lr=1e-4, weight_decay=0.05, loss_scale=65536.0, dynamic_loss_scale=True)
+    g = torch.Generator().manual_seed(7)
+    rng = np.random.default_rng(7)
+
+    def batch(i):
+        imgs = [torch.randint(0, 256, hw + (3,), dtype=torch.uint8, generator=g) for hw in ((480, 640), (700, 500))]
+        embs = [(rng.standard_normal(1024 * embed * embed) * 0.5).astype(np.float16) for _ in imgs]
+        return (imgs, None), (embs, [i, i])
+    loader = [batch(i) for i in range(2)]
+    return record_calls(monkeypatch, lambda: train_one_epoch(cfg, m, loader, opt, epoch=0))
+
+
+def text_epoch_calls(cuda, monkeypatch, backbone, layers=2, ctx=32):
+    """The es3_* calls of stage1.train.train_text_one_epoch over a depth-`layers` text student (`backbone`), FlatAdamW without its
+    unused projection, masked loss with consistency, ACCUMULATION_STEPS 2 over a two-iteration loader of stored fp16 embeddings.
+    MobileCLIP-S0 trains with batch-statistics BatchNorm (enable_batch_stat_bn, TRAIN.EVAL_BN_WHEN_TRAINING False)."""
+    import random
+    from efficientsam3_b200.model.text_encoder_student import TextStudentEncoder
+    from efficientsam3_b200.stage1.model import text_student_cfg
+    from efficientsam3_b200.stage1.optim import FlatAdamW
+    from efficientsam3_b200.stage1.train import train_text_one_epoch
+    from oracle.weights import fill_state_dict
+    from test_text_cpu import BPE
+    cfg = text_student_cfg(backbone)
+    cfg["n_transformer_layers"] = layers
+    cfg["context_length"] = ctx
+    m = TextStudentEncoder(cfg=cfg, context_length=ctx, output_dim=256, bpe_path=BPE)
+    m.load_state_dict(fill_state_dict(m.state_dict(), 21))
+    m = m.to(cuda)
+    if backbone == "MobileCLIP-S0":
+        m.enable_batch_stat_bn()
+    opt = FlatAdamW(m, lr=1e-3, weight_decay=0.05, loss_scale=65536.0, dynamic_loss_scale=True,
+                    exclude=TextStudentEncoder.UNUSED_PARAMETERS)
+    tcfg = _stage1_cfg(NUM_EMBED=ctx, EMBED_DIM=256, MASK_PAD_TOKENS=True, CONSISTENCY_LOSS=0.5)
+    caps = _captions(6)
+    rng = np.random.default_rng(8)
+    loader = [[list(caps), [[(rng.standard_normal(ctx * 256) * 0.5).astype(np.float16) for _ in caps], list(range(6))]]
+              for _ in range(2)]
+    random.seed(5)
+    return record_calls(monkeypatch, lambda: train_text_one_epoch(tcfg, m, loader, opt, epoch=0))
 
 
 def eval_forward_calls(cuda, monkeypatch, name, img=1024, embed=64, B=2, strict=False):

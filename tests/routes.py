@@ -134,6 +134,16 @@ def fp8_attn_key(H, W, win):
     return ("es3_attention_fp8", 96 if L % 96 == 0 and L % 128 != 0 else 128, win > 0)
 
 
+def grad_norm_key(n):
+    """es3_grad_norm: (name, ragged n % 4, grid capped: more than 4096 blocks of 16384 elements, so threads loop)."""
+    return ("es3_grad_norm", n % 4 != 0, -(-n // 16384) > 4096)
+
+
+def adamw_key(n, n_decay, max_norm, dynamic):
+    """es3_adamw_flat: (name, clipping on, dynamic loss scale, ragged n % 4, decay split 0 < n_decay < n)."""
+    return ("es3_adamw_flat", max_norm > 0, bool(dynamic), n % 4 != 0, 0 < n_decay < n)
+
+
 def _res(ptr, f32):
     return ("f32" if f32 else "bf16") if _nz(ptr) else None
 
@@ -222,11 +232,16 @@ _DETAILED = {
     "es3_attention_fp8": lambda a: fp8_attn_key(a[4], a[5], a[8]),
     "es3_pack_weight_e4m3": lambda a: ("es3_pack_weight_e4m3", _dt(a[1])),
     "es3_layernorm_f32_e4m3": lambda a: ("es3_layernorm_f32_e4m3", a[7] // 128),
+    # the stage-1 KD loss and optimiser
+    "es3_kd_loss_fwd": lambda a: ("es3_kd_loss_fwd", _nz(a[10])),                                  # per_sample present
+    "es3_kd_loss_bwd": lambda a: ("es3_kd_loss_bwd", _nz(a[4])),                                   # scale_dev present
+    "es3_grad_norm": lambda a: grad_norm_key(a[1]),
+    "es3_adamw_flat": lambda a: adamw_key(a[4], a[5], a[11], a[15]),
 }
 
 _FWD, _BWD, _TEXT, _SAM, _VIT = ("test_fwd_kernels_gpu.py", "test_train_bwd_gpu.py", "test_text_kernels_gpu.py",
                                  "test_sam_kernels_gpu.py", "test_vit_kernels_gpu.py")
-_GEMM, _STRICT = "test_gemm_epilogue_gpu.py", "test_strict_kernels_gpu.py"
+_GEMM, _STRICT, _STAGE1 = "test_gemm_epilogue_gpu.py", "test_strict_kernels_gpu.py", "test_stage1_kernels_gpu.py"
 _FILES = {
     _FWD: """mbconv_bf16 dwproj_tc_bf16 dwconv_tc_bf16 dwconv_tiled_bf16 dwconv_bf16 stem_conv3x3_s2 dsconv_res_bf16 litemla_attn_generic
              conv3x3_s2_narrow_bf16 win_attn_bias_bf16 layernorm_bf16 stem_fused_c16 litemla_aggreg_dwpw litemla_attn_tc channel_mean
@@ -245,11 +260,10 @@ _FILES = {
     _GEMM: "gemm_bf16 gemm_bf16_ex pw_small_bf16 gemm_simt conv3x3_bf16 convt2x2_bf16",
     "test_fp8_gpu.py": "gemm_fp8 quantize_bf16_e4m3 pack_weight_e4m3 layernorm_f32_e4m3",
     "test_fp8_attention_gpu.py": "attention_fp8",
+    _STAGE1: "kd_loss_fwd kd_loss_bwd grad_norm adamw_flat",
     # files without covered_keys(): they hold the name-only key of the entry points listed for them
     "test_amg_gpu.py": "amg_mask_stats box_nms amg_rle",
     "test_preprocess_gpu.py": "prepare_images_u8",
-    "test_optim_gpu.py": "adamw_flat grad_norm kd_loss_fwd kd_loss_bwd",
-    "test_kd_loss_gpu.py": "kd_loss_fwd",
     "test_decoder_gpu.py": "fill_small_components",
     "test_syncbn_gpu.py": "bn_stats_partial bn_stats_combine bn_act_bwd_partial bn_bwd_coef",
     "test_syncbn_repmixer_gpu.py": """repmixer_bn_fwd repmixer_bn_stats_partial repmixer_bn_finalize_sync repmixer_bn_tm_sums

@@ -133,3 +133,20 @@ def test_tensor_core_tap_operand_is_cached_per_tensor_and_version(monkeypatch):
     c = ops._tc_taps(w)
     assert c is not a and len(calls) == 2 and torch.equal(c, w.to(torch.bfloat16).float())
     assert ops._tc_taps(torch.randn(9, 32)) is not c and len(calls) == 3
+
+
+def test_step_without_clipping_passes_max_norm_0(monkeypatch):
+    """TRAIN.CLIP_GRAD None or 0 means no clipping (NativeScalerWithGradNormCount): FlatAdamW.step hands es3_adamw_flat max_norm 0,
+    as kd_train_step(clip_grad=None) and text_kd_train_step do through it.  The two kernels are replaced by recorders and the arena
+    is taken for a device one, so the host side runs without a GPU."""
+    from efficientsam3_b200 import ops
+    m = torch.nn.Sequential(torch.nn.Linear(6, 4), torch.nn.LayerNorm(4))
+    opt = O.FlatAdamW(m, lr=1e-3)
+    seen = []
+    monkeypatch.setattr(ops, "grad_norm", lambda *a: None)
+    monkeypatch.setattr(ops, "adamw_flat", lambda *a, **k: seen.append(float(a[9])))
+    monkeypatch.setattr(torch.Tensor, "is_cuda", property(lambda t: True))
+    for clip in (None, 0, 0.0, 5.0):
+        opt.step(max_norm=clip)
+    monkeypatch.undo()
+    assert seen == [0.0, 0.0, 0.0, 5.0]

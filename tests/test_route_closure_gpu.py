@@ -11,10 +11,15 @@ import sys
 
 import pytest
 
-from es3_recorder import (STUDENTS, TEXT_ROUTES, backbone_calls, eval_forward_calls, module_api_calls, point_segmenter,
-                          predictor_calls, segmenter_set_image_calls, teacher_calls, text_step_calls, text_teacher_calls,
-                          training_step_calls)
+from es3_recorder import (STUDENTS, TEXT_ROUTES, backbone_calls, eval_forward_calls, image_epoch_calls, module_api_calls,
+                          point_segmenter, predictor_calls, segmenter_set_image_calls, teacher_calls, text_epoch_calls, text_step_calls,
+                          text_teacher_calls, training_step_calls)
 from routes import KEYS, assert_closed, conv3x3_num_kb, gemm_bn, gemm_stages, pick_bn
+
+# What every stage-1 update reaches: the loss backward scaled by the device loss scale, the norm of a 16-byte-aligned arena whose
+# length is a multiple of 4 and far below the grid cap, and AdamW clipped at CLIP_GRAD with a dynamic scale and the decay group
+# ending inside the arena
+STAGE1_UPDATE = {("es3_grad_norm", False, False), ("es3_adamw_flat", True, True, False, True)}
 
 pytestmark = pytest.mark.gpu
 
@@ -60,6 +65,28 @@ def test_route_closure_student_strict(cuda, monkeypatch, name):
     assert reached and not [k for k in reached if "bf16" in k[0]], f"{name} strict reaches bf16 kernels"
     missing = STRICT_PINNED.get(name, set()) - reached
     assert not missing, f"{name} strict: expected routes not reached: {sorted(missing, key=repr)}"
+
+
+# ----------------------------------------------------------------------------------------------------------- stage-1 iterations
+@pytest.mark.parametrize("name", ["efficientvit_b1", "repvit_m1_1", "tiny_vit_5m"])
+def test_route_closure_image_epoch(cuda, monkeypatch, name):
+    """stage1.train.train_one_epoch, one student per family: decoded uint8 images of two sizes prepared on the device, the KD loss
+    on padded masks with the stored fp16 embeddings, the backward with batch-statistics BatchNorm, two iterations accumulated into
+    one FlatAdamW update (dynamic loss scale, clipped)."""
+    reached = assert_closed(image_epoch_calls(cuda, monkeypatch, name), f"{name} train_one_epoch")
+    pinned = STAGE1_UPDATE | {("es3_prepare_images_u8",), ("es3_kd_loss_fwd", True), ("es3_kd_loss_bwd", True)}
+    missing = pinned - reached
+    assert not missing, f"{name} train_one_epoch: expected routes not reached: {sorted(missing, key=repr)}"
+
+
+@pytest.mark.parametrize("backbone", ["MobileCLIP-S0", "MobileCLIP-S1"])
+def test_route_closure_text_epoch(cuda, monkeypatch, backbone):
+    """stage1.train.train_text_one_epoch: S0 with batch-statistics BatchNorm (the path it takes by default) and S1, masked loss with
+    consistency, two iterations accumulated into one FlatAdamW update."""
+    reached = assert_closed(text_epoch_calls(cuda, monkeypatch, backbone), f"{backbone} train_text_one_epoch")
+    pinned = STAGE1_UPDATE | ({("es3_repmixer_bn_fwd",)} if backbone == "MobileCLIP-S0" else set())
+    missing = pinned - reached
+    assert not missing, f"{backbone} train_text_one_epoch: expected routes not reached: {sorted(missing, key=repr)}"
 
 
 # ----------------------------------------------------------------------------------------------------------- text encoders

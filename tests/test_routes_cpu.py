@@ -15,7 +15,7 @@ from test_boundary import _declared
 HERE = os.path.dirname(os.path.abspath(__file__))
 KERNEL_TEST_FILES = ["test_gemm_epilogue_gpu.py", "test_train_bwd_gpu.py", "test_fwd_kernels_gpu.py", "test_text_kernels_gpu.py",
                      "test_sam_kernels_gpu.py", "test_vit_kernels_gpu.py", "test_strict_kernels_gpu.py", "test_fp8_gpu.py",
-                     "test_fp8_attention_gpu.py"]
+                     "test_fp8_attention_gpu.py", "test_stage1_kernels_gpu.py"]
 MBCONV_B1_STAGE3 = (0,) * 13 + (128, 512, 128, 1, 1, 2, 0)     # es3_mbconv_bf16 arguments: Cin 128, mid 512, Cout 128, stride 1
 # es3_dwconv_f32 arguments of LiteMLA's strict 5 x 5 aggregation (EfficientViT-B1 stage 3 at 1024^2): no scale, no bias, no act
 LITEMLA_AGGREG_F32 = (0, 768, 0, 0, 0, 0, 384, 2, 64, 64, 384, 5, 1, 0, 0)
@@ -25,6 +25,8 @@ GLOBAL_ROPE_QKV = (1, 1024, 2, 1024, 3, 3072, 0, 10368, 3072, 1024, 0, 4, 0, 0, 
 GLOBAL_ROPE_QKV_KEY = ("es3_gemm_bf16_ex", 128, 4, None, False, True, None, False, "bf16", "global", False)
 # es3_pw_small_bf16 arguments of an expand 16 -> 64 without residual (EfficientViT-B0 / B1 training forward at 1024^2)
 PW_SMALL_16_64 = (1, 16, 2, 16, 3, 64, 0, 0, 2 * 256 * 256, 64, 16, 0)
+# es3_adamw_flat arguments of a stage-1 update: a 9M-element arena whose decay group ends at 8M, clipped at 5, dynamic loss scale
+ADAMW_STAGE1 = (1, 2, 3, 4, 9_000_000, 8_000_000, 1e-4, 0.9, 0.999, 1e-8, 0.05, 5.0, 1.0, 5, 6, 1, 2.0, 0.5, 2000, 0)
 
 
 def test_keys_are_the_kernel_entry_points_of_the_header():
@@ -144,3 +146,23 @@ def test_closure_rejects_a_strict_dwconv_whose_table_row_is_gone(monkeypatch):
     monkeypatch.setattr(strict, "DW", [c for c in strict.DW if (c[4], c[5], c[6], c[7], c[8]) != (5, 1, None, False, False)])
     with pytest.raises(AssertionError, match="no table row runs"):
         assert_closed([call], "strict dwconv row removed")
+
+
+def test_closure_rejects_a_clipped_decay_split_adamw_once_its_row_is_gone(monkeypatch):
+    call = ("es3_adamw_flat", ADAMW_STAGE1)
+    key = ("es3_adamw_flat", True, True, False, True)
+    assert assert_closed([call], "stage-1 adamw") == {key}
+    stage1 = importlib.import_module("test_stage1_kernels_gpu")
+    monkeypatch.setattr(stage1, "ADAMW", [c for c in stage1.ADAMW if routes.adamw_key(c[0], stage1._n_decay(c[0], c[1]), c[4], c[9]) != key])
+    with pytest.raises(AssertionError, match="no table row runs"):
+        assert_closed([call], "stage-1 adamw row removed")
+
+
+def test_stage1_keys_follow_what_the_arguments_select():
+    assert KEYS["es3_grad_norm"]((1, 16384 * 4096, 2, 3, 0)) == ("es3_grad_norm", False, False)
+    assert KEYS["es3_grad_norm"]((1, 16384 * 4096 + 4, 2, 3, 0)) == ("es3_grad_norm", False, True)
+    assert KEYS["es3_grad_norm"]((1, 1021, 2, 3, 0)) == ("es3_grad_norm", True, False)
+    assert KEYS["es3_adamw_flat"](ADAMW_STAGE1[:4] + (8, 8) + ADAMW_STAGE1[6:11] + (0.0,) + ADAMW_STAGE1[12:15] + (0,) +
+                                  ADAMW_STAGE1[16:]) == ("es3_adamw_flat", False, False, False, False)
+    assert KEYS["es3_kd_loss_fwd"]((1, 2, 3, 2, 1024, 64, 1024, 1.0, 4, 5, 0, 0)) == ("es3_kd_loss_fwd", False)
+    assert KEYS["es3_kd_loss_bwd"]((1, 2, 3, 4, 5, 1.0, 2, 1024, 64, 1024, 1.0, 6, 0)) == ("es3_kd_loss_bwd", True)
